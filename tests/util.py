@@ -42,6 +42,43 @@ def rel_l2(a, b):
     return float(np.sqrt(np.sum((a - b) ** 2)) / den) if den > 0 else float(np.sqrt(np.sum((a - b) ** 2)))
 
 
+def write_buffer(engine, cam, name, array):
+    """Overwrites a per-camera device buffer with `array` (float32 words; uint32 bit patterns are taken as they are), through
+    st_buffer_device_ptr and a zero-copy torch view.  The engine is synchronised before and after, so the write lands between
+    two `render_range` calls."""
+    import torch
+    from strolle_b200.multigpu import _DevArray
+    ptr, nbytes = engine.buffer_device_ptr(cam, name)
+    a = np.ascontiguousarray(np.asarray(array)).reshape(-1).view(np.float32)
+    assert a.size * 4 == nbytes, f"{name}: {a.size * 4} bytes for a {nbytes}-byte buffer"
+    engine.synchronize()
+    torch.as_tensor(_DevArray(ptr, a.size), device="cuda").copy_(torch.from_numpy(a.copy()))
+    torch.cuda.synchronize()
+    engine.synchronize()
+
+
+def check_within(got, want, bound, what=""):
+    """Per-value comparison with a per-value bound: NaN expected -> NaN, +-inf expected -> the same inf, otherwise
+    |got - want| <= bound.  Returns the largest |got - want| / bound over the finite values (0 where both are 0)."""
+    got = np.asarray(got, dtype=np.float64)
+    want = np.broadcast_to(np.asarray(want, dtype=np.float64), got.shape)
+    bound = np.broadcast_to(np.asarray(bound, dtype=np.float64), got.shape)
+    nan, inf = np.isnan(want), np.isinf(want)
+    bad = (nan & ~np.isnan(got)) | (inf & (got != want))
+    fin = ~nan & ~inf
+    with np.errstate(invalid="ignore", divide="ignore"):
+        err = np.where(fin, np.abs(got - want), 0.0)
+        ratio = np.where(err == 0, 0.0, err / bound)
+    ratio = np.where(fin & np.isnan(ratio), np.inf, ratio)
+    bad |= fin & ~(ratio <= 1.0)
+    if bad.any():
+        idx = np.flatnonzero(bad.reshape(-1))[:5]
+        g, w, b = got.reshape(-1)[idx], want.reshape(-1)[idx], bound.reshape(-1)[idx]
+        raise AssertionError(f"{what}: {int(bad.sum())}/{bad.size} values outside the bound; first at flat {idx.tolist()}: "
+                             f"got {g.tolist()} want {w.tolist()} bound {b.tolist()}")
+    return float(ratio.max()) if ratio.size else 0.0
+
+
 def primary_rays(scene_camera, engine_like, cam):
     """Camera rays of every pixel as an (n, 8) ray stream, rebuilt from the G-buffer-independent
     camera uniform so that both implementations get identical inputs."""
