@@ -71,6 +71,15 @@ void orc_update_camera(void* e, int cam, int mode, int denoise, int ref_depth, i
 }
 void orc_tick(void* e) { ((Engine*)e)->tick(); }
 void orc_render_camera(void* e, int cam) { ((Engine*)e)->render_camera(cam); }
+void orc_render_range(void* e, int cam, int first, int last) { ((Engine*)e)->render_range(cam, first, last); }
+// pass ids of this frame's steps (the device's PassId values); returns the step count, copies min(cap, count)
+int orc_frame_schedule(void* e, int cam, int* ids, int cap) {
+    Engine* en = (Engine*)e;
+    en->run_atmosphere();
+    std::vector<Engine::Step> steps = en->schedule(cam);
+    for (int i = 0; i < cap && i < (int)steps.size(); i++) ids[i] = steps[i].pass;
+    return (int)steps.size();
+}
 
 // returns number of floats available; copies min(cap, n)
 long orc_read_buffer(void* e, int cam, const char* name, float* dst, long cap) {

@@ -6,6 +6,7 @@
 // LUT generation, and the per-frame pass schedule of CameraController::render.
 #pragma once
 #include <algorithm>
+#include <functional>
 #include <deque>
 #include <map>
 #include <string>
@@ -739,73 +740,112 @@ struct Engine {
         if (!luts.have_static) { atm_generate_transmittance(luts.transmittance); atm_generate_scattering(luts.transmittance, luts.scattering); luts.have_static = true; }
         if (!luts.have_sky || luts.sky_altitude != sun_altitude) { atm_generate_sky(luts.transmittance, luts.scattering, world.sun_altitude, luts.sky); luts.sky_altitude = sun_altitude; luts.have_sky = true; }
     }
-    // CameraController::render (camera_controller.rs:87-174); `upto` stops after
-    // that many passes (test hook for per-pass buffer comparison), 0 = all.
-    void render_camera(int h) {
-        Cam* c = cameras[h]; CamState& cs = c->st; u32 f = c->frame; bool alt = (f % 2) == 1;
-        const HostCamera& hc = c->cam;
-        run_atmosphere();
+    // CameraController::render (camera_controller.rs:87-174) as an explicit step list: (pass id, work).  The ids are the device's
+    // PassId values and the list is the device's schedule with strict arithmetic and one launch per reference dispatch
+    // (ST_OPT_FUSED_PASSES = 0; K20 for both signals is one step, like the device's default fused reproject launch), so that a test
+    // can stop between two passes (render_range) and read a pass's inputs before it overwrites them.
+    struct Step { int pass; std::function<void()> run; };
+    enum { S_PRIM_GBUFFER = 0, S_DI_SPATIAL_TRACE = 4, S_DI_RESOLVING = 6, S_GI_REPROJECTION = 7, S_GI_SPATIAL_TRACE = 12, S_GI_RESOLVING = 15,
+           S_FRAME_REPROJECTION = 16, S_DENOISE_REPROJECT = 17, S_DENOISE_VARIANCE = 18, S_DENOISE_WAVELET = 19, S_COMPOSITION = 20,
+           S_REF_TRACING = 21, S_REF_SHADING = 22, S_BVH_HEATMAP = 23 };
+    std::vector<Step> schedule(int h) {
+        Cam* c = cameras[h]; CamState* csp = &c->st; u32 f = c->frame; bool alt = (f % 2) == 1;
+        const HostCamera hc = c->cam;
         Scene sc = scene();
+        std::vector<Step> out;
+        auto add = [&](int pass, std::function<void()> fn) { out.push_back(Step{pass, std::move(fn)}); };
         auto seed = [&](u32 k) { return dispatch_seed(seed_base, f, k); };
-        if (hc.mode == MODE_BVH_HEATMAP) { pass_bvh_heatmap(cs, sc); pass_frame_composition(cs, alt, 5, false, false); return; }
+        if (hc.mode == MODE_BVH_HEATMAP) {
+            add(S_BVH_HEATMAP, [=] { pass_bvh_heatmap(*csp, sc); });
+            add(S_COMPOSITION, [=] { pass_frame_composition(*csp, alt, 5, false, false); });
+            return out;
+        }
         if (hc.mode == MODE_REFERENCE) {
-            for (u32 d = 0; d <= hc.ref_depth; d++) { pass_ref_tracing(cs, sc, d); pass_ref_shading(cs, sc, seed(D_REF_SHADING + d), d); }
-            pass_ref_shading(cs, sc, seed(D_REF_SHADING + 31), 255);
-            pass_frame_composition(cs, alt, 6, false, false);
-            return;
+            for (u32 d = 0; d <= hc.ref_depth; d++) {
+                u32 sd = seed(D_REF_SHADING + d);
+                add(S_REF_TRACING, [=] { pass_ref_tracing(*csp, sc, d); });
+                add(S_REF_SHADING, [=] { pass_ref_shading(*csp, sc, sd, d); });
+            }
+            u32 sd = seed(D_REF_SHADING + 31);
+            add(S_REF_SHADING, [=] { pass_ref_shading(*csp, sc, sd, 255); });
+            add(S_COMPOSITION, [=] { pass_frame_composition(*csp, alt, 6, false, false); });
+            return out;
         }
         bool needs_di = hc.mode == MODE_IMAGE || hc.mode == MODE_DI_DIFFUSE || hc.mode == MODE_DI_SPECULAR;
         bool needs_gi = hc.mode == MODE_IMAGE || hc.mode == MODE_GI_DIFFUSE || hc.mode == MODE_GI_SPECULAR;
-        pass_prim_gbuffer(cs, sc, alt);
+        add(S_PRIM_GBUFFER, [=] { pass_prim_gbuffer(*csp, sc, alt); });
         if (!instances.empty()) {
-            pass_frame_reprojection(cs, alt);
+            add(S_FRAME_REPROJECTION, [=] { pass_frame_reprojection(*csp, alt); });
             if (needs_di) {
-                pass_di_sampling(cs, sc, alt, seed(D_DI_SAMPLING), f);
-                pass_di_temporal(cs, sc, alt, seed(D_DI_TEMPORAL));
-                pass_di_spatial_pick(cs, sc, alt, seed(D_DI_SPATIAL_PICK), f);
-                pass_spatial_trace(cs, sc, cs.di_diff_samples, cs.di_diff_curr_colors, cs.di_diff_stash);
-                pass_di_spatial_sample(cs, seed(D_DI_SPATIAL_SAMPLE), f);
-                pass_di_resolving(cs, sc, alt);
+                u32 s1 = seed(D_DI_SAMPLING), s2 = seed(D_DI_TEMPORAL), s3 = seed(D_DI_SPATIAL_PICK), s5 = seed(D_DI_SPATIAL_SAMPLE);
+                add(D_DI_SAMPLING, [=] { pass_di_sampling(*csp, sc, alt, s1, f); });
+                add(D_DI_TEMPORAL, [=] { pass_di_temporal(*csp, sc, alt, s2); });
+                add(D_DI_SPATIAL_PICK, [=] { pass_di_spatial_pick(*csp, sc, alt, s3, f); });
+                add(S_DI_SPATIAL_TRACE, [=] { pass_spatial_trace(*csp, sc, csp->di_diff_samples, csp->di_diff_curr_colors, csp->di_diff_stash); });
+                add(D_DI_SPATIAL_SAMPLE, [=] { pass_di_spatial_sample(*csp, s5, f); });
+                add(S_DI_RESOLVING, [=] { pass_di_resolving(*csp, sc, alt); });
             }
             if (needs_gi) {
+                u32 sa = seed(D_GI_SAMPLING_A), sb = seed(D_GI_SAMPLING_B), st = seed(D_GI_TEMPORAL), sp = seed(D_GI_SPATIAL_PICK), ss = seed(D_GI_SPATIAL_SAMPLE);
+                u32 ps = seed(D_GI_PREVIEW);   // both preview passes share one seed (passes/gi_preview_resampling.rs:58)
                 u32 source;
-                pass_gi_reprojection(cs, alt);
+                add(S_GI_REPROJECTION, [=] { pass_gi_reprojection(*csp, alt); });
+                auto sampling = [&] {
+                    add(D_GI_SAMPLING_A, [=] { pass_gi_sampling_a(*csp, sc, alt, sa, f); });
+                    add(D_GI_SAMPLING_B, [=] { pass_gi_sampling_b(*csp, sc, alt, sb, f); });
+                };
                 if (frame_is_gi_tracing(f)) {
-                    if (f % 2 == 0) { pass_gi_sampling_a(cs, sc, alt, seed(D_GI_SAMPLING_A), f); pass_gi_sampling_b(cs, sc, alt, seed(D_GI_SAMPLING_B), f); }
-                    pass_gi_temporal(cs, alt, seed(D_GI_TEMPORAL), f);
+                    if (f % 2 == 0) sampling();
+                    add(D_GI_TEMPORAL, [=] { pass_gi_temporal(*csp, alt, st, f); });
                     if (f % 2 == 1) {
-                        pass_gi_spatial_pick(cs, alt, seed(D_GI_SPATIAL_PICK), f);
-                        pass_spatial_trace(cs, sc, cs.gi_d0, cs.gi_d1, cs.gi_d2);
-                        pass_gi_spatial_sample(cs, seed(D_GI_SPATIAL_SAMPLE), f);
+                        add(D_GI_SPATIAL_PICK, [=] { pass_gi_spatial_pick(*csp, alt, sp, f); });
+                        add(S_GI_SPATIAL_TRACE, [=] { pass_spatial_trace(*csp, sc, csp->gi_d0, csp->gi_d1, csp->gi_d2); });
+                        add(D_GI_SPATIAL_SAMPLE, [=] { pass_gi_spatial_sample(*csp, ss, f); });
                         source = 1;
                     } else source = 0;
                 } else {
-                    pass_gi_sampling_a(cs, sc, alt, seed(D_GI_SAMPLING_A), f); pass_gi_sampling_b(cs, sc, alt, seed(D_GI_SAMPLING_B), f);
-                    pass_gi_temporal(cs, alt, seed(D_GI_TEMPORAL), f);
+                    sampling();
+                    add(D_GI_TEMPORAL, [=] { pass_gi_temporal(*csp, alt, st, f); });
                     source = 0;
                 }
-                u32 ps = seed(D_GI_PREVIEW);   // both preview passes share one seed (passes/gi_preview_resampling.rs:58)
-                pass_gi_preview(cs, alt, ps, source, 0, cs.gi_reservoirs[1], cs.gi_reservoirs[2], cs.gi_reservoirs[3]);
-                pass_gi_preview(cs, alt, ps, 1, 1, cs.gi_reservoirs[1], cs.gi_reservoirs[3], cs.gi_reservoirs[0]);
-                pass_gi_resolving(cs, alt, source);
+                add(D_GI_PREVIEW, [=] { pass_gi_preview(*csp, alt, ps, source, 0, csp->gi_reservoirs[1], csp->gi_reservoirs[2], csp->gi_reservoirs[3]); });
+                add(D_GI_PREVIEW, [=] { pass_gi_preview(*csp, alt, ps, 1, 1, csp->gi_reservoirs[1], csp->gi_reservoirs[3], csp->gi_reservoirs[0]); });
+                add(S_GI_RESOLVING, [=] { pass_gi_resolving(*csp, alt, source); });
             }
         }
         if (hc.denoise) {  // passes/frame_denoising.rs:143-190
             int cur = alt ? 1 : 0, prv = alt ? 0 : 1;
-            pass_denoise_reproject(cs, alt, cs.di_diff_prev_colors, cs.di_diff_moments[prv], cs.di_diff_samples, cs.di_diff_curr_colors, cs.di_diff_moments[cur]);
-            pass_denoise_reproject(cs, alt, cs.gi_diff_prev_colors, cs.gi_diff_moments[prv], cs.gi_diff_samples, cs.gi_diff_curr_colors, cs.gi_diff_moments[cur]);
-            pass_denoise_estimate_variance(cs, alt);
-            Buf* di_io[5][2] = {{&cs.di_diff_stash, &cs.di_diff_prev_colors}, {&cs.di_diff_prev_colors, &cs.di_diff_stash}, {&cs.di_diff_stash, &cs.di_diff_curr_colors},
-                                {&cs.di_diff_curr_colors, &cs.di_diff_stash}, {&cs.di_diff_stash, &cs.di_diff_curr_colors}};
-            Buf* gi_io[5][2] = {{&cs.gi_diff_stash, &cs.gi_diff_prev_colors}, {&cs.gi_diff_prev_colors, &cs.gi_diff_stash}, {&cs.gi_diff_stash, &cs.gi_diff_curr_colors},
-                                {&cs.gi_diff_curr_colors, &cs.gi_diff_stash}, {&cs.gi_diff_stash, &cs.gi_diff_curr_colors}};
-            for (u32 nth = 0; nth < 5; nth++)
-                pass_denoise_wavelet(cs, sc, alt, f, 1u << nth, (float)(1 + nth), *di_io[nth][0], *di_io[nth][1], *gi_io[nth][0], *gi_io[nth][1]);
+            add(S_DENOISE_REPROJECT, [=] {
+                CamState& cs = *csp;
+                pass_denoise_reproject(cs, alt, cs.di_diff_prev_colors, cs.di_diff_moments[prv], cs.di_diff_samples, cs.di_diff_curr_colors, cs.di_diff_moments[cur]);
+                pass_denoise_reproject(cs, alt, cs.gi_diff_prev_colors, cs.gi_diff_moments[prv], cs.gi_diff_samples, cs.gi_diff_curr_colors, cs.gi_diff_moments[cur]);
+            });
+            add(S_DENOISE_VARIANCE, [=] { pass_denoise_estimate_variance(*csp, alt); });
+            for (u32 nth = 0; nth < 5; nth++) {
+                add(S_DENOISE_WAVELET, [=] {
+                    CamState& cs = *csp;
+                    Buf* di_io[5][2] = {{&cs.di_diff_stash, &cs.di_diff_prev_colors}, {&cs.di_diff_prev_colors, &cs.di_diff_stash}, {&cs.di_diff_stash, &cs.di_diff_curr_colors},
+                                        {&cs.di_diff_curr_colors, &cs.di_diff_stash}, {&cs.di_diff_stash, &cs.di_diff_curr_colors}};
+                    Buf* gi_io[5][2] = {{&cs.gi_diff_stash, &cs.gi_diff_prev_colors}, {&cs.gi_diff_prev_colors, &cs.gi_diff_stash}, {&cs.gi_diff_stash, &cs.gi_diff_curr_colors},
+                                        {&cs.gi_diff_curr_colors, &cs.gi_diff_stash}, {&cs.gi_diff_stash, &cs.gi_diff_curr_colors}};
+                    pass_denoise_wavelet(cs, sc, alt, f, 1u << nth, (float)(1 + nth), *di_io[nth][0], *di_io[nth][1], *gi_io[nth][0], *gi_io[nth][1]);
+                });
+            }
         }
         bool den_di = hc.denoise && (hc.mode == MODE_IMAGE || hc.mode == MODE_DI_DIFFUSE);
         bool den_gi = hc.denoise && (hc.mode == MODE_IMAGE || hc.mode == MODE_GI_DIFFUSE);
-        pass_frame_composition(cs, alt, (u32)hc.mode, den_di, den_gi);
+        u32 mode = (u32)hc.mode;
+        add(S_COMPOSITION, [=] { pass_frame_composition(*csp, alt, mode, den_di, den_gi); });
+        return out;
     }
+    // steps [first, last] of this frame's schedule (last < 0: to the end)
+    void render_range(int h, int first, int last) {
+        run_atmosphere();
+        std::vector<Step> steps = schedule(h);
+        if (last < 0 || last >= (int)steps.size()) last = (int)steps.size() - 1;
+        for (int i = std::max(first, 0); i <= last; i++) steps[i].run();
+    }
+    void render_camera(int h) { render_range(h, 0, -1); }
 };
 
 }  // namespace orc

@@ -50,6 +50,8 @@ def _load(libm=False):
         "orc_update_camera": [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p],
         "orc_tick": [C.c_void_p],
         "orc_render_camera": [C.c_void_p, C.c_int],
+        "orc_render_range": [C.c_void_p, C.c_int, C.c_int, C.c_int],
+        "orc_frame_schedule": [C.c_void_p, C.c_int, C.c_void_p, C.c_int],
         "orc_read_buffer": [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_long],
         "orc_read_scene": [C.c_void_p, C.c_char_p, C.c_void_p, C.c_long],
         "orc_bvh_depth": [C.c_void_p],
@@ -194,6 +196,17 @@ class OracleEngine:
 
     def render_camera(self, cam):
         self.lib.orc_render_camera(self.h, cam)
+
+    def render_range(self, cam, first, last):
+        """Steps [first, last] of this frame's schedule (last < 0: to the end); same step list as the CUDA engine's strict,
+        unfused schedule."""
+        self.lib.orc_render_range(self.h, cam, first, last)
+
+    def frame_schedule(self, cam):
+        """Pass ids (the CUDA engine's PassId values) of this frame's steps."""
+        ids = (C.c_int * 64)()
+        n = self.lib.orc_frame_schedule(self.h, cam, ids, 64)
+        return list(ids[:n])
 
     def read_buffer(self, cam, name):
         n = self.lib.orc_read_buffer(self.h, cam, name.encode(), None, 0)

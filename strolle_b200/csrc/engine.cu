@@ -1558,12 +1558,15 @@ int st_trace_any(st_engine* e, const float* rays, size_t n, uint32_t* out, float
 
 int st_device_math(st_engine* e, int op, const float* a, const float* b, float* out, size_t n) {
     if (!e || !a || !out) return fail(ST_ERR_INVALID, "null argument");
+    if (n == 0) return ST_OK;   // nothing to evaluate (a zero-block grid would be a launch error)
     CK(cudaSetDevice(e->device));
     DevMem da, db, dc; int rc;
     if ((rc = da.ensure(n * 4)) || (rc = db.ensure(n * 4)) || (rc = dc.ensure(n * 4))) return rc;
     CK(cudaMemcpyAsync(da.p, a, n * 4, cudaMemcpyHostToDevice, e->stream));
     if (b) CK(cudaMemcpyAsync(db.p, b, n * 4, cudaMemcpyHostToDevice, e->stream));
-    launch_math(op, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
+    // op 0-6: the strict elementary functions; op 16-21: the fast-shading build's sin, cos, exp, pow, sqrt and division
+    if (op >= 16) stf::launch_math_shading(op - 16, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
+    else launch_math(op, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
     CK(cudaMemcpyAsync(out, dc.p, n * 4, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     da.release(); db.release(); dc.release();

@@ -1535,6 +1535,19 @@ __global__ void k_atm_sky(const float4* __restrict__ tl, const float4* __restric
 
 #endif   // ST_EXACT_ONLY
 
+// elementary-function test hook for the shading kernels' own flavour: in the fast build these are the SFU / approximate forms
+// (sincos_det = __sincosf, exp_det = __expf, pow_det = __powf outside its product exponents, sqrtf = sqrt.approx, a / b = div.full)
+__global__ void k_math_shading(int op, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out, long n) {
+    long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float r = 0.f, x = a[i], y = b[i];
+    switch (op) {
+        case 0: r = sin_det(x); break; case 1: r = cos_det(x); break; case 2: r = exp_det(x); break;
+        case 3: r = pow_det(x, y); break; case 4: r = sqrtf(x); break; case 5: r = x / y; break;
+    }
+    out[i] = r;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Host-side launchers
 // ---------------------------------------------------------------------------------------------
@@ -1561,6 +1574,7 @@ void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32
 void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_sampling_fused, c, st, c, s, cur, seed_a, seed_b, frame); }
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st) { k_gi_preview_resolve<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, in, source); }
+void launch_math_shading(int op, const float* a, const float* b, float* out, long n, cudaStream_t st) { k_math_shading<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n); }
 #if ST_EXACT_ONLY
 void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, cudaStream_t st) { k_prim_gbuffer<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, with_reprojection); }
 void launch_frame_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_frame_reprojection<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }

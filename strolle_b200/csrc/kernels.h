@@ -109,4 +109,5 @@ void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32
 void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, cudaStream_t st);
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st);
+void launch_math_shading(int op, const float* a, const float* b, float* out, long n, cudaStream_t st);   // test hook: this build's sin/cos/exp/pow/sqrt/div
 }  // namespace stf

@@ -9,7 +9,7 @@ import pytest
 
 from strolle_b200 import scenes
 from tests import ref64_svgf as R
-from tests.util import check_within, write_buffer
+from tests.util import Frame, check_within, write_buffer
 
 pytestmark = pytest.mark.gpu
 
@@ -29,29 +29,6 @@ def _engine(gpu, blue_noise, strict, options=()):
     for k, v in options:
         e.set_option(k, v)
     return e
-
-
-class Frame:
-    """Steps through one frame's schedule and reads buffers as (H, W, 4)."""
-
-    def __init__(self, e, cam, w, h):
-        self.e, self.cam, self.w, self.h = e, cam, w, h
-        self.sched = e.frame_schedule(cam)
-        self.done = -1
-
-    def read(self, name):
-        return self.e.read_buffer(self.cam, name).reshape(self.h, self.w, 4)
-
-    def write(self, name, a):
-        write_buffer(self.e, self.cam, name, np.asarray(a, dtype=np.float32))
-
-    def steps(self, pass_id):
-        return [i for i, p in enumerate(self.sched) if p == pass_id]
-
-    def run_to(self, last):
-        if last > self.done:
-            self.e.render_range(self.cam, self.done + 1, last)
-            self.done = last
 
 
 def _move(e, cam, scene, f):

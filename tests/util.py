@@ -57,6 +57,29 @@ def write_buffer(engine, cam, name, array):
     engine.synchronize()
 
 
+class Frame:
+    """Steps through one frame's schedule and reads buffers as (H, W, 4)."""
+
+    def __init__(self, e, cam, w, h):
+        self.e, self.cam, self.w, self.h = e, cam, w, h
+        self.sched = e.frame_schedule(cam)
+        self.done = -1
+
+    def read(self, name):
+        return self.e.read_buffer(self.cam, name).reshape(self.h, self.w, 4)
+
+    def write(self, name, a):
+        write_buffer(self.e, self.cam, name, np.asarray(a, dtype=np.float32))
+
+    def steps(self, pass_id):
+        return [i for i, p in enumerate(self.sched) if p == pass_id]
+
+    def run_to(self, last):
+        if last > self.done:
+            self.e.render_range(self.cam, self.done + 1, last)
+            self.done = last
+
+
 def check_within(got, want, bound, what=""):
     """Per-value comparison with a per-value bound: NaN expected -> NaN, +-inf expected -> the same inf, otherwise
     |got - want| <= bound.  Returns the largest |got - want| / bound over the finite values (0 where both are 0)."""
