@@ -1,6 +1,13 @@
-"""Float64 restatement of the DI spatial merge (K9) and DI resolving (K10), with a per-value error bound for either arithmetic tier.
+"""Float64 restatement of the DI temporal resampling (K6), the DI spatial merge (K9) and DI resolving (K10), with a per-value error
+bound for either arithmetic tier, and a check of the spatial visibility pass (K8) against the traversal.
 
 Written from the reference's definitions (paths relative to the reference tree), not from the CUDA kernels or the oracle:
+  * K6  `di_temporal_resampling::main`    strolle-shaders/src/di_temporal_resampling.rs:4-112
+  * K8  `di_spatial_resampling::trace`    strolle-shaders/src/di_spatial_resampling.rs:150-209
+  * `Mis::di_temporal`                    strolle-gpu/src/reservoir/mis.rs:36-65
+  * `DiSample::pdf` / `pdf_prev` / `pdf_ex`   strolle-gpu/src/reservoir/di.rs:95-117; `Light::contains` / slots / `rollback`
+                                          strolle-gpu/src/light.rs:83-85, :107-141; `LightsView::get_prev` strolle-gpu/src/lights.rs:19-24
+  * `Reprojection::prev_pos_round`        strolle-gpu/src/reprojection.rs:46-48; `Reservoir::clamp_m` strolle-gpu/src/reservoir.rs:55-57
   * K9  `di_spatial_resampling::sample`   strolle-shaders/src/di_spatial_resampling.rs:212-297
   * K10 `di_resolving::main`              strolle-shaders/src/di_resolving.rs:4-119
   * `Mis::eval`                           strolle-gpu/src/reservoir/mis.rs:96-145 (`m(q0, q1)` = (q1 / q0).min(1).powf(8).saturate())
@@ -27,7 +34,8 @@ absolute bound on |f32 evaluation - f64 value| (u = 2^-24, the unit roundoff of 
                  2 u).  |b| <= eb gives an infinite bound.
   sqrt a         |sqrt(a~) - sqrt(a)| <= min(ea / sqrt(a), sqrt(ea)), plus rel sqrt(a): u (strict) or 2^-23 (sqrt.approx.f32, PTX ISA).
                  1 / sqrt as a division of a square root also covers a fused rsqrt.approx.f32 (2^-22.9 < 2^-22 + 2^-23).
-  min, max, clamp, saturate, |x|   1-Lipschitz: the input bound passes through.
+  min, max, clamp, saturate, |x|   1-Lipschitz: the input bound passes through; where the value is past a limit by more than its
+                 bound the f32 result is that limit, exactly (bound 0).
   powf(x, k)     for k = 3, 5, 8 the reference's exponents are evaluated as the products x x x, (x^2)^2 x, ((x^2)^2)^2 in both tiers.
   Every rounding of a result in the f32 subnormal range adds 2^-149 (neither build flushes denormals).
 Inputs read from device buffers are exact (e = 0).  The base colour is (b / 255)^2.2 from a 256-entry table the strict pow builds:
@@ -45,7 +53,13 @@ Discrete decisions.  Each is evaluated on the f64 values with its bound:
     A product with an exactly zero factor is exactly zero; a comparison of exact values is decided.
   * `q0 <= 0`, `sum == 0`, `rhs_idx > 0`, `pdf * 1 == 0` and `lhs_rhs_vis == 0` act on values that are exact f32 inputs or exact
     products of them, so they are decided.
-Visibility (Ray::intersect) is not restated: K9 takes it from the scratch texels, K10 from the occluded bit it stores.
+  * K6: `Light::contains(light_point)` in pdf_ex compares a rounded distance with the radius; where |d - R| is inside d's bound the
+    pdf may be 0 or the value, and the pixel is counted as undecided and not compared.  The same holds for the specular early-out in
+    any of K6's three pdfs.  `q0 <= 0` in m(q0, q1) acts on the recomputed lhs_rhs_pdf: where 0 < q0 <= its bound (or q0 = 0 with a
+    nonzero bound) m is left unbounded and the pixel is counted, as is any pixel whose pdfs have no finite bound.  `round()` of the
+    reprojection and the slot markers act on exact inputs.
+Visibility (Ray::intersect) is not restated: K9 takes it from the scratch texels, K10 from the occluded bit it stores, and K8's bit is
+compared with the engine's any-hit traversal of the ray decoded from K7's texels (`oct_decode_f32`: the strict build's decode exactly).
 """
 import numpy as np
 
@@ -72,7 +86,8 @@ class Num:
 
     def __init__(self, v, e=0.0, fast=False):
         self.v = np.asarray(v, dtype=np.float64)
-        self.e = np.zeros(self.v.shape) + np.asarray(e, dtype=np.float64)
+        e = np.zeros(self.v.shape) + np.asarray(e, dtype=np.float64)
+        self.e = np.where(np.isnan(e), np.inf, e)      # a bound lost to inf * 0 or inf - inf is no bound
         self.fast = fast
 
     def _n(self, x):
@@ -143,16 +158,19 @@ class Num:
             return Num(s, prop + rel * s + self._sub(s, self.e), self.fast)
 
     def clip(self, lo, hi):
-        return Num(np.clip(self.v, lo, hi), self.e, self.fast)
+        """Where the f32 value is certainly past a limit (by more than its bound) the result is that limit, exactly."""
+        with np.errstate(invalid="ignore"):
+            pinned = (self.v < lo - self.e) | (self.v > hi + self.e)
+        return Num(np.clip(self.v, lo, hi), np.where(pinned, 0.0, self.e), self.fast)
 
     def sat(self):
         return self.clip(0.0, 1.0)
 
     def maximum(self, c):
-        return Num(np.maximum(self.v, c), self.e, self.fast)
+        return self.clip(c, np.inf)
 
     def minimum(self, c):
-        return Num(np.minimum(self.v, c), self.e, self.fast)
+        return self.clip(-np.inf, c)
 
     def abs(self):
         return Num(np.abs(self.v), self.e, self.fast)
@@ -452,6 +470,17 @@ def _decide(r, W, weight):
         return margin > 0, (~(np.abs(margin) <= bound) | ((margin == 0) & (W.e == 0) & (weight.e == 0))) & np.isfinite(margin)
 
 
+def _mis_eval(lm, rm, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, rpdf):
+    """Mis::eval (mis.rs:96-145) with rhs_jacobian = 1: (m, lhs_mis, rhs_mis)."""
+    mm_a, mm_b = _mis_m(rpdf, rhs_lhs_pdf), _mis_m(lhs_rhs_pdf, lpdf)
+    mmin = where(mm_a.v <= mm_b.v, mm_a, mm_b)
+    mmin = Num(mmin.v, np.maximum(mm_a.e, mm_b.e), lm.fast)
+    t = _ratio(lm, rm)
+    lhs_mis = t + (1.0 - t) * _ratio(lm * lpdf, rm * lhs_rhs_pdf)
+    rhs_mis = (1.0 - t) * _ratio((rm * rpdf) * 1.0, lm * rhs_lhs_pdf)
+    return rm * mmin, lhs_mis, rhs_mis
+
+
 def di_spatial_sample(res_in, stash, seed, frame, w, h, fast):
     """K9 on every checkerboard pair.  Returns dict(idx (P,), cands: list of dicts of expected (P, 8) words + bound on m / w, per-pair
     `allowed` mask per candidate; decided (P,) bool; copies (Q,) indices of the pass-through pixels)."""
@@ -485,13 +514,7 @@ def di_spatial_sample(res_in, stash, seed, frame, w, h, fast):
     lhs_rhs_pdf = z(d1[:, 1]) * lhs_rhs_vis
     rhs_lhs_pdf = z(d1[:, 2]) * rhs_lhs_vis
     with np.errstate(invalid="ignore", over="ignore"):
-        mm_a, mm_b = _mis_m(rpdf, rhs_lhs_pdf), _mis_m(lhs_rhs_pdf, lpdf)
-        mmin = where(mm_a.v <= mm_b.v, mm_a, mm_b)
-        mmin = Num(mmin.v, np.maximum(mm_a.e, mm_b.e), fast)
-        mis_m = rm * mmin
-        t = _ratio(lm, rm)
-        lhs_mis = t + (1.0 - t) * _ratio(lm * lpdf, rm * lhs_rhs_pdf)
-        rhs_mis = (1.0 - t) * _ratio((rm * rpdf) * 1.0, lm * rhs_lhs_pdf)
+        mis_m, lhs_mis, rhs_mis = _mis_eval(lm, rm, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, rpdf)
         wl = (lhs_mis * lpdf) * lw
         wr = (rhs_mis * rhs_lhs_pdf) * rw
         rng = WhiteNoise(seed, lx, gy)
@@ -522,6 +545,260 @@ def di_spatial_sample(res_in, stash, seed, frame, w, h, fast):
     cands.append(dict(allowed=~merge, words=lhs.copy(), m=lhs[:, 0].astype(np.float64), m_e=np.zeros(len(gx)),
                       w=lhs[:, 1].astype(np.float64), w_e=np.zeros(len(gx))))
     return dict(idx=lidx, cands=cands, undecided=merge & ~(dec1 & dec2), merge=merge, copies=copies)
+
+
+# ---- K6: temporal resampling -------------------------------------------------------------------------------------------------
+
+LUMA = (_f32c(0.2126), _f32c(0.7152), _f32c(0.0722))
+SLOT_KILLED = 0xCAFEBABE
+
+
+def _take(x, idx):
+    """Pixels `idx` (flat) of a per-pixel (H, W, ...) value: Num, array, or a dict of them (a hit)."""
+    if isinstance(x, dict):
+        return {k: _take(v, idx) for k, v in x.items()}
+    if isinstance(x, Num):
+        return Num(x.v.reshape((-1,) + x.v.shape[2:])[idx], x.e.reshape((-1,) + x.e.shape[2:])[idx], x.fast)
+    a = np.asarray(x)
+    return a.reshape((-1,) + a.shape[2:])[idx]
+
+
+def di_pdf(L, ht, point):
+    """DiSample::pdf_ex (di.rs:108-117) with per-pixel light records L (N, 28) and hits ht (N, ...): luma(radiance * (diff + spec))
+    of Light::radiance with the base colour set to 1 (Vec3Ext::luma, utils/vec3_ext.rs:52-54; DiffuseBrdf::eval, brdf.rs:20-24), or 0
+    for a Light::TYPE_NONE slot or a light point outside the light (Light::contains, light.rs:83-85: |center - point| <= radius).
+    Returns (pdf, contains undecided, specular undecided)."""
+    fast = ht["point"].fast
+    L = np.asarray(L, np.float32)
+    g = dict(ht["g"], base=Num(np.ones(ht["g"]["base"].v.shape), 0.0, fast))
+    lr = light_radiance(L, dict(ht, g=g))
+    diff = (1.0 - g["metallic"]) / PI
+    s = lr["radiance"] * (diff.x3() + lr["spec"])
+    luma = (s.col(0) * LUMA[0] + s.col(1) * LUMA[1]) + s.col(2) * LUMA[2]
+    p = np.asarray(point, np.float32).astype(np.float64)
+    c = Num(L[:, 0:3].astype(np.float64), 0.0, fast) - p
+    dist = dot3(c, c).sqrt()
+    radius = L[:, 3].astype(np.float64)
+    live = L[:, 8].view(np.uint32) != 0
+    inside = dist.v <= radius
+    pdf = where(live & inside, luma, Num(np.zeros(len(L)), 0.0, fast))
+    return pdf, live & (np.abs(radius - dist.v) <= dist.e), live & inside & lr["undecided"]
+
+
+def _round_u(x):
+    """Vec2::round (half away from zero) then as_uvec2 (saturating) of exact f32 inputs."""
+    x = np.asarray(x, np.float32).astype(np.float64)
+    r = np.where(x < 0, -np.floor(-x + 0.5), np.floor(x + 0.5))
+    return np.clip(np.nan_to_num(r, nan=0.0), 0, 2.0 ** 32 - 1).astype(np.int64)
+
+
+def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_prev, seed, fast):
+    """K6 di_temporal_resampling::main (di_temporal_resampling.rs:4-112) for every pixel with a surface.  gb / gb_prev: this and the
+    previous frame's G-buffer (d0, d1); reproj: the reprojection map (Reprojection::deserialize, reprojection.rs:22-29); res_cur: what
+    K5 left in di_reservoirs[1]; res_prev: di_reservoirs[0].
+      * lhs: K5's sample, its pdf recomputed with the current light (:47-51).
+      * rhs: di_reservoirs[0] at prev_pos().round().as_uvec2() (reprojection.rs:46-48), M clamped to 64 (reservoir.rs:55-57), a killed
+        slot zeroes w, a remapped one moves the id to slot - 1 (light.rs:107-129); its hit is rebuilt with the *previous* camera from
+        the previous G-buffer (:61-89).
+      * Mis::di_temporal (mis.rs:36-65): lhs_rhs_pdf with the rolled-back light (LightsView::get_prev, lights.rs:19-24), rhs_lhs_pdf
+        with the current one, 0 for a killed rhs; then Mis::eval, two Reservoir::update and norm_mis (:93-111), confidence 0 for a
+        killed rhs and 1 otherwise.
+    Every light id dereferenced is asserted to lie inside `lights` (the table as read).  Returns dict(idx, cands, undecided per
+    decision type, skip (pixels with an undecided pdf), surf)."""
+    f32 = np.float32
+    lights = np.asarray(lights, f32).reshape(-1, 28)
+    nl = len(lights)
+    npx = w * h
+    z = lambda a: Num(np.asarray(a, np.float64), 0.0, fast)
+    ht = hit(n2w, w, h, gb[0], gb[1], fast)
+    idx = np.flatnonzero(ht["g"]["some"].reshape(-1))
+    n = len(idx)
+    zero = z(np.zeros(n))
+    lh = _take(ht, idx)
+    cur, prv = di_fields(res_cur), di_fields(res_prev)
+    lm, lw, lid, lpoint = cur["m"][idx], cur["w"][idx], cur["id"][idx].astype(np.int64), cur["point"][idx]
+    assert (lid[lm != 0] < nl).all(), "K6 lhs light id outside the light table"
+    lid_c = np.minimum(lid, nl - 1)
+    lp, und_c1, und_s1 = di_pdf(lights[lid_c], lh, lpoint)
+    lpdf = where(lm != 0, lp, z(cur["pdf"][idx]))
+    rp = np.asarray(reproj, f32).reshape(-1, 4)[idx]
+    has_rp = rp[:, 2] > 0
+    rx, ry = _round_u(rp[:, 0]), _round_u(rp[:, 1])
+    assert ((rx < w) & (ry < h))[has_rp].all(), "reprojected position outside the frame"
+    ridx = ry * w + rx
+    read = has_rp & (ridx < npx)
+    ri = np.where(read, ridx, 0)
+    pick = lambda a, dflt=0: np.where(read.reshape((-1,) + (1,) * (np.ndim(a) - 1)), a[ri], dflt)
+    rm = np.minimum(pick(prv["m"]), 64.0)
+    rw, rpdf, rocc, rconf, rpoint, rid = pick(prv["w"]), pick(prv["pdf"]), pick(prv["occ"], False), pick(prv["conf"]), pick(prv["point"]), pick(prv["id"]).astype(np.int64)
+    ne = rm != 0
+    assert (rid[ne] < nl).all(), "K6 rhs light id outside the light table"
+    slot = lights[np.minimum(rid, nl - 1), 12].view(np.uint32).astype(np.int64)
+    killed = ne & (slot == SLOT_KILLED)
+    remap = ne & ~killed & (slot > 0)
+    rw = np.where(killed, 0.0, rw)
+    rid = np.where(remap, slot - 1, rid)
+    assert (rid[remap] < nl).all(), "K6 remapped light id outside the light table"
+    rid_c = np.minimum(rid, nl - 1)
+    htp = hit(n2w_prev, w, h, gb_prev[0], gb_prev[1], fast)
+    rh = _take(htp, ri)
+    rhs_some = ne & rh["g"]["some"]
+    prev_L = lights[lid_c].copy()
+    prev_L[:, 0:12] = lights[lid_c, 16:28]          # Light::rollback (light.rs:137-141)
+    lrp, und_c2, und_s2 = di_pdf(prev_L, rh, lpoint)
+    use_lr = (lm > 0) & rhs_some
+    lhs_rhs_pdf = where(use_lr, lrp, zero)
+    rlp, und_c3, und_s3 = di_pdf(lights[rid_c], lh, rpoint)
+    use_rl = (rm > 0) & ~killed
+    rhs_lhs_pdf = where(use_rl, rlp, zero)
+    und = {"contains": (und_c1 & (lm != 0)) | (und_c2 & use_lr) | (und_c3 & use_rl),
+           "specular": (und_s1 & (lm != 0)) | (und_s2 & use_lr) | (und_s3 & use_rl)}
+    skip = und["contains"] | und["specular"]
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        lmN, rmN = z(lm), z(rm)
+        mis_m, lhs_mis, rhs_mis = _mis_eval(lmN, rmN, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, z(rpdf))
+        # m(q0, q1) branches on q0 <= 0: for the recomputed lhs_rhs_pdf that is a decision on a bounded value
+        und["mis q0"] = (lhs_rhs_pdf.e > 0) & (lhs_rhs_pdf.v <= lhs_rhs_pdf.e) & (rm > 0)
+        m_out = lmN + mis_m
+        m_e = np.where(und["mis q0"], np.inf, m_out.e)
+        # a recomputed pdf without a finite bound (GGX at minimum roughness on a normal along the view: the (n.h a^2 - n.h) n.h + 1
+        # cancellation) leaves the pixel's m and w unbounded: counted
+        und["unbounded"] = ~np.isfinite(m_e) | ~np.isfinite(lpdf.e) | ~np.isfinite(lhs_rhs_pdf.e) | ~np.isfinite(rhs_lhs_pdf.e)
+        wl = (lhs_mis * lpdf) * z(lw)
+        wr = (rhs_mis * rhs_lhs_pdf) * z(rw)
+        rng = WhiteNoise(seed, idx % w, idx // w)
+        r1, r2 = rng.sample(), rng.sample()
+        W1 = zero + wl
+        W2 = W1 + wr
+        acc1, dec1 = _decide(r1, W1, wl)
+        acc2, dec2 = _decide(r2, W2, wr)
+    und["update"] = ~(dec1 & dec2)
+    conf = np.where(killed, 0, 1).astype(np.uint32)
+    cands = []
+    for a1 in (False, True):
+        for a2 in (False, True):
+            allowed = np.where(dec1, acc1 == a1, True) & np.where(dec2, acc2 == a2, True)
+            if a2:
+                pdf, occ, point, lid_o = rhs_lhs_pdf, rocc, rpoint, rid
+            elif a1:
+                pdf, occ, point, lid_o = lpdf, cur["occ"][idx], lpoint, lid
+            else:
+                pdf, occ, point, lid_o = zero, np.zeros(n, bool), np.zeros((n, 3), f32), np.zeros(n, np.int64)
+            with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+                wn = W2 / pdf
+            exact0 = (pdf.v == 0) & (pdf.e == 0)
+            firm = pdf.v > pdf.e        # the f32 pdf is certainly nonzero
+            out = np.zeros((n, 8), f32)
+            out[:, 3] = (occ.astype(np.uint32) | (conf << 8)).view(f32)
+            out[:, 4:7] = point
+            out[:, 7] = lid_o.astype(np.uint32).view(f32)
+            cands.append(dict(allowed=allowed, words=out, m=m_out.v, m_e=m_e, pdf=pdf.v, pdf_e=pdf.e,
+                              w=np.where(exact0 | ~firm, 0.0, wn.v), w_e=np.where(exact0, 0.0, np.where(firm, wn.e, np.inf))))
+    return dict(idx=idx, cands=cands, undecided=und, skip=skip, surf=ht["g"]["some"].reshape(-1), killed=int(killed.sum()),
+                remapped=int(remap.sum()), reprojected=int(read.sum()))
+
+
+def check_temporal(got, res_before, r, what):
+    """K6's reservoirs: at every surface pixel without an undecided pdf, one admissible outcome with the discrete words (occluded,
+    confidence, light point, light id) bit for bit and m, w, pdf within their bounds; every other pixel untouched.  Returns (largest
+    error / bound ratio, undecided counts per decision type, pixels checked)."""
+    got = np.asarray(got, np.float32).reshape(-1, 8)
+    before = np.asarray(res_before, np.float32).reshape(-1, 8)
+    assert (got[~r["surf"]].view(np.uint32) == before[~r["surf"]].view(np.uint32)).all(), f"{what}: K6 wrote a sky pixel"
+    g = got[r["idx"]]
+    gb = g.view(np.uint32)
+    ok = r["skip"].copy()
+    best = np.zeros(len(g))
+    found = np.zeros(len(g), bool)
+    for c in r["cands"]:
+        disc = (gb[:, 3:8] == c["words"].view(np.uint32)[:, 3:8]).all(1)
+        rat = []
+        with np.errstate(invalid="ignore", divide="ignore"):
+            for k, key in ((0, "m"), (1, "w"), (2, "pdf")):
+                err = np.abs(g[:, k].astype(np.float64) - c[key])
+                rk = np.where(err == 0, 0.0, err / c[key + "_e"])
+                rat.append(np.where(np.isnan(rk), np.inf, rk))
+        ratio = np.maximum(np.maximum(rat[0], rat[1]), rat[2])
+        good = c["allowed"] & disc & (ratio <= 1.0) & ~r["skip"]
+        best = np.where(good & ~found, ratio, np.where(good, np.minimum(best, ratio), best))
+        found |= good
+        ok |= good
+    if not ok.all():
+        i = np.flatnonzero(~ok)[:4]
+        raise AssertionError(f"{what}: {int((~ok).sum())}/{len(ok)} pixels match no admissible outcome; first pixels {r['idx'][i].tolist()}: "
+                             f"got {g[i].tolist()}")
+    und = {k: int(v.sum()) for k, v in r["undecided"].items()}
+    return float(best.max()) if len(best) else 0.0, und, len(g)
+
+
+def temporal_tight(r):
+    """{key: (tightly bounded, finite nonzero)} for K6's m, w and pdf over the decided outcome of each decided pixel.  m is the
+    loosest of the three: Mis::eval raises a ratio of two recomputed pdfs to the 8th power, which multiplies its relative bound by 8."""
+    out = {}
+    sel0 = ~r["skip"] & ~r["undecided"]["update"] & ~r["undecided"]["unbounded"]
+    for key in ("m", "w", "pdf"):
+        n = t = 0
+        for c in r["cands"]:
+            sel = c["allowed"] & sel0
+            v, e = c[key][sel], c[key + "_e"][sel]
+            fin = np.isfinite(v) & (v != 0)
+            n += int(fin.sum()); t += int((e[fin] < 1e-3 * np.abs(v[fin])).sum())
+        out[key] = (t, n)
+    return out
+
+
+# fraction of K6's values whose bound must be below 1e-3 relative (temporal_tight).  Cornell with spot lights is the loosest scene
+# (H100, strict, 224x126): m 94.1 %, w 98.7 %, pdf 99.4 %; the acos_approx cone term loosens the recomputed pdfs there, and m takes
+# their ratio to the 8th power
+TIGHT_MIN = {"m": 0.9, "w": 0.98, "pdf": 0.99}
+
+
+def tight_ok(acc):
+    """acc: {key: [tight, n]} summed over frames.  Every key has values and enough of them are tightly bounded."""
+    return all(acc[k][1] > 0 and acc[k][0] >= TIGHT_MIN[k] * acc[k][1] for k in TIGHT_MIN)
+
+
+# ---- K8: visibility of K7's rays -----------------------------------------------------------------------------------------------
+
+def oct_decode_f32(e):
+    """Normal::decode (normal.rs) of (..., 2) f32 inputs, evaluated in f32 operation by operation (no contraction), with glam's
+    normalize = v * (1 / sqrt(dot(v, v))): the strict build's rounding, exactly."""
+    f = np.float32
+    e = np.asarray(e, f)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        mx, my = e[..., 0] * f(2) - f(1), e[..., 1] * f(2) - f(1)
+        nz = (f(1) - np.abs(mx)) - np.abs(my)
+        t = np.maximum(-nz, f(0))
+        nx, ny = mx - np.copysign(t, mx), my - np.copysign(t, my)
+        inv = f(1) / np.sqrt((nx * nx + ny * ny) + nz * nz)
+        return np.stack([nx * inv, ny * inv, nz * inv], -1).astype(f)
+
+
+def check_spatial_trace(buf_d0, buf_d1, buf_d2, trace_any, what):
+    """K8 di_spatial_resampling::trace (di_spatial_resampling.rs:150-209) on every texel: a texel whose d1 is zero gives d2 = 0; any
+    other gives (visibility, d1.z, d1.w, 0) with d1.z / d1.w copied bit for bit, and the visibility is compared with `trace_any` of
+    the ray rebuilt from the texels (origin d0.xyz, Normal::decode(d1.xy), length d0.w).  K7's zero ray (origin 0, length 0,
+    oct(0) = NaN direction) must come out visible.  Returns (texels traced, visibility disagreements)."""
+    d0 = np.asarray(buf_d0, np.float32).reshape(-1, 4)
+    d1 = np.asarray(buf_d1, np.float32).reshape(-1, 4)
+    d2 = np.asarray(buf_d2, np.float32).reshape(-1, 4)
+    b1, b2 = d1.view(np.uint32), d2.view(np.uint32)
+    empty = (d1 == 0).all(1)
+    assert (b2[empty] == 0).all(), f"{what}: K8 texel with a zero d1 is not zero"
+    live = ~empty
+    assert (b2[live][:, 1:3] == b1[live][:, 2:4]).all(), f"{what}: K8 d2.yz are not d1.zw"
+    assert (b2[live][:, 3] == 0).all() and np.isin(d2[live][:, 0], (0.0, 1.0)).all(), f"{what}: K8 texel layout"
+    if not live.any():
+        return 0, 0
+    rays = np.zeros((int(live.sum()), 8), np.float32)
+    rays[:, 0:3] = d0[live][:, 0:3]
+    rays[:, 3] = d0[live][:, 3]
+    rays[:, 4:7] = oct_decode_f32(d1[live][:, 0:2])
+    vis = d2[live][:, 0]
+    nan = np.isnan(rays[:, 4:7]).any(1)
+    assert (vis[nan] == 1).all(), f"{what}: a ray with an undefined direction (K7's zero ray) is not visible"
+    want = 1.0 - np.asarray(trace_any(rays), np.float64)
+    return int(live.sum()), int((vis != want).sum())
 
 
 # ---- checks shared by the CPU chain test and the GPU tests --------------------------------------------------------------------
@@ -604,6 +881,7 @@ def tight_fraction(nums, some):
 # What a bound on a pass that evaluates these in the fast build assumes (PTX ISA / CUDA programming guide limits, with margin), on
 # the arguments the ReSTIR kernels pass: angles 2 pi r for r in [0, 1) and the sun's altitude / azimuth (sin / cos), exponents in
 # [-100, 0] (the sun bloom), pow bases in (0, 1] with the exponents of the lights and LUTs, sqrt of [0, 1e6], and divisions.
+SIN_ABS = 2.0 ** -23            # the strict build's Cephes sinf / cosf on [0, 2 pi], absolute: 7.6e-8 measured (test_ref64_constants)
 SIN_ABS_FAST = 2.0 ** -20       # __sincosf on [0, 2 pi], absolute: 2^-21.4 on [-pi, pi] (CUDA guide), 7.1e-7 measured on an H100 for cos
 EXP_REL_FAST = 2.0 ** -21       # __expf(x) = ex2.approx(x log2 e), relative, plus 2 u |x| log2 e for the scaled argument
 POW_REL_FAST = 2.0 ** -20       # __powf(x, y) = ex2.approx(y lg2.approx(x)), relative, plus 2^-22 |y log2 x| for lg2's absolute error

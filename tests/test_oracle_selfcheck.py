@@ -274,8 +274,8 @@ def test_ray_stream_matches_float64_brute_force(cornell_oracle):
 
 
 def test_ref64_constants(oracle):
-    """The Cephes error constants tests/ref64_svgf.py builds its strict bounds on, measured through oracle.math (bit-identical to
-    the device functions, test_device_math_bit_exact)."""
+    """The Cephes error constants tests/ref64_svgf.py and tests/ref64_restir.py build their strict bounds on, measured through
+    oracle.math (bit-identical to the device functions, test_device_math_bit_exact)."""
     from tests import ref64_svgf as R
     x = np.linspace(-87.0, 0.0, 400001).astype(np.float32)
     t = np.exp(x.astype(np.float64))
@@ -287,6 +287,11 @@ def test_ref64_constants(oracle):
     p = np.float32(1.0) / np.float32(2.4)
     t = x.astype(np.float64) ** float(p)
     assert (np.abs(oracle.math("pow", x, np.full_like(x, p)) - t) / t).max() <= R.POW_INV24_REL
+    # the strict sin / cos on the angles 2 pi r, r in [0, 1), that the ReSTIR disk and sphere samples take (tests/ref64_restir.py)
+    from tests import ref64_restir as Q
+    x = np.concatenate([np.linspace(0.0, 2 * np.pi, 400001), np.random.RandomState(1).uniform(0, 2 * np.pi, 10 ** 6)]).astype(np.float32)
+    for op, fn in (("sin", np.sin), ("cos", np.cos)):
+        assert np.abs(oracle.math(op, x) - fn(x.astype(np.float64))).max() <= Q.SIN_ABS, op
 
 
 def _svgf_chain_check(oracle, blue_noise, scene, frames=6, moves=(3, 4, 5)):
@@ -376,21 +381,28 @@ def test_transmittance_lut_is_physically_plausible(oracle, blue_noise):
     assert (t >= 0).all() and (t <= 1).all()
 
 
-def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11), edge_lights=False):
-    """K9 (DI spatial merge) and K10 (DI resolving) of the strict oracle against tests/ref64_restir.py, pass by pass: the frame is
-    stepped with render_range, each pass's inputs are read right before it runs and its outputs right after."""
+def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11), edge_lights=False, extra_lights=0, remove=9001):
+    """K6 (DI temporal resampling), K8 (the spatial visibility rays), K9 (DI spatial merge) and K10 (DI resolving) of the strict
+    oracle against tests/ref64_restir.py, pass by pass: the frame is stepped with render_range, each pass's inputs are read right
+    before it runs and its outputs right after.  `extra_lights` small point lights are added before the first frame; `remove` is
+    the light taken out on frame 10 (9001, the last one, kills its slot; one from the middle of the list remaps the last slot)."""
     from tests import ref64_restir as Q
     c = scene["camera"]
     w, h = c["w"], c["h"]
     e = oracle.OracleEngine(blue_noise=blue_noise)
     cam = scenes.apply(e, scene)
     t = np.asarray(c["transform"], np.float32).reshape(16).copy()
-    stats = {"K9": [0.0, 0, 0], "K10": [0.0, 0], "K9 tight": [0, 0]}
+    t_prev = t.copy()          # the camera before the last update_camera: what the engine keeps as the previous camera
+    stats = {"K6": [0.0, {}, 0], "K6 tight": {k: [0, 0] for k in ("m", "w", "pdf")}, "K6 branches": [0, 0, 0], "K8": [0, 0],
+             "K9": [0.0, 0, 0], "K10": [0.0, 0], "K9 tight": [0, 0]}
     if edge_lights:
         from tests.test_restir_reference import edge_lights as add_lights
         add_lights(e)
+    from tests.test_restir_reference import many_lights
+    many_lights(e, extra_lights)
     for f in range(1, frames + 1):
         if f in moves:
+            t_prev = t.copy()
             t[12] += np.float32(0.013 * f); t[13] += np.float32(0.004 * f)
             e.update_camera(cam, c["mode"], c["denoise"], c["ref_depth"], w, h, t, c["projection"])
         if f == 4:
@@ -398,13 +410,33 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
         if f == 7:
             e.insert_light(9001, scenes.LIGHT_POINT, scenes.point_light((-0.3, 0.8, 0.1), 0.08, (3.0, 2.0, 1.0), 6.0))
         if f == 10:
-            e.remove_light(9001)
+            e.remove_light(remove)
         e.tick()
         sched = e.frame_schedule(cam)
-        k9, k10 = sched.index(5), sched.index(6)
+        k6, k8, k9, k10 = sched.index(2), sched.index(4), sched.index(5), sched.index(6)
         rd = lambda n: e.read_buffer(cam, n)
         cur = "b" if f % 2 == 1 else "a"
-        e.render_range(cam, 0, k9 - 1)
+        old = "a" if cur == "b" else "b"
+        e.render_range(cam, 0, k6 - 1)
+        gb = [rd(f"prim_gbuffer_d{k}_{cur}").reshape(h, w, 4) for k in (0, 1)]
+        gb_prev = [rd(f"prim_gbuffer_d{k}_{old}").reshape(h, w, 4) for k in (0, 1)]
+        r1, r0 = rd("di_reservoirs_1"), rd("di_reservoirs_0")
+        k6r = Q.di_temporal(Q.ndc_to_world(t, c["projection"]), Q.ndc_to_world(t_prev, c["projection"]), w, h, gb, gb_prev,
+                            rd("reprojection_map"), e.read_scene("lights"), r1, r0, Q.dispatch_seed(0xC0FFEE, f, 2), fast=False)
+        e.render_range(cam, k6, k6)
+        ratio, und, npx = Q.check_temporal(rd("di_reservoirs_1"), r1, k6r, f"f{f} K6")
+        s = stats["K6"]
+        stats["K6"] = [max(s[0], ratio), {k: s[1].get(k, 0) + v for k, v in und.items()}, s[2] + npx]
+        for k, (tt, nn) in Q.temporal_tight(k6r).items():
+            stats["K6 tight"][k][0] += tt; stats["K6 tight"][k][1] += nn
+        stats["K6 branches"] = [a + k6r[b] for a, b in zip(stats["K6 branches"], ("reprojected", "killed", "remapped"))]
+        e.render_range(cam, k6 + 1, k8 - 1)
+        b0, b1 = rd("di_diff_samples"), rd("di_diff_curr_colors")
+        e.render_range(cam, k8, k8)
+        traced, bad = Q.check_spatial_trace(b0, b1, rd("di_diff_stash"), e.trace_any, f"f{f} K8")
+        assert bad == 0, f"f{f} K8: {bad} of {traced} visibility bits differ from trace_any"
+        stats["K8"] = [stats["K8"][0] + traced, stats["K8"][1] + bad]
+        e.render_range(cam, k8 + 1, k9 - 1)
         r1, stash = rd("di_reservoirs_1"), rd("di_diff_stash")
         e.render_range(cam, k9, k9)
         r2 = rd("di_reservoirs_2")
@@ -448,17 +480,34 @@ def test_oracle_render_range_is_render_camera(oracle, blue_noise):
         assert_bits_equal(outs[0][n], outs[1][n], n)
 
 
-@pytest.mark.parametrize("which", ["cornell", "demo_level", "cornell_spots", "textured_room", "cornell_edge_lights"])
+@pytest.mark.parametrize("which", ["cornell", "demo_level", "cornell_spots", "textured_room", "cornell_edge_lights",
+                                   "cornell_many_lights", "cornell_remap"])
 def test_restir_float64_chain_matches_oracle(oracle, blue_noise, which):
-    """The float64 restatement of K9 and K10 reproduces the strict oracle within its bound over 13 frames (both GI cycles), with the
-    camera moving and a light inserted, moved and removed mid-run; the textured room's metallic box exercises the specular lobe.  The oracle and the CUDA kernels were written from one reading of
-    the reference; this checks that reading against an independent one without a GPU."""
+    """The float64 restatement of K6, K8, K9 and K10 reproduces the strict oracle within its bound over 13 frames (both GI cycles),
+    with the camera moving and a light inserted, moved and removed mid-run; the textured room's metallic box exercises the specular
+    lobe.  Many lights: 23 in all, so K5 draws 16 of them and K6 resamples among lights that are not the first few.  Remap: a light
+    is removed from the middle of the list, so K6 sees a remapped slot as well as the killed one.  The oracle and the CUDA kernels
+    were written from one reading of the reference; this checks that reading against an independent one without a GPU."""
     scene = {"cornell": lambda: scenes.cornell(96, 64), "demo_level": lambda: scenes.demo_level(80, 45),
              "cornell_spots": lambda: scenes.cornell_spots(72, 48), "textured_room": lambda: scenes.textured_room(80, 44),
-             "cornell_edge_lights": lambda: scenes.cornell(72, 48)}[which]()
-    stats = _restir_chain_check(oracle, blue_noise, scene, edge_lights=which == "cornell_edge_lights")
-    print(f"\n{which}: K9 ratio {stats['K9'][0]:.3g}, undecided {stats['K9'][1]} of {stats['K9'][2]} merges; "
-          f"K10 ratio {stats['K10'][0]:.3g}, undecided specular {stats['K10'][1]}")
+             "cornell_edge_lights": lambda: scenes.cornell(72, 48), "cornell_many_lights": lambda: scenes.cornell(72, 48),
+             "cornell_remap": lambda: scenes.cornell(72, 48)}[which]()
+    from tests.test_restir_reference import MANY_LIGHTS, REMAP_REMOVED
+    stats = _restir_chain_check(oracle, blue_noise, scene, edge_lights=which == "cornell_edge_lights",
+                                extra_lights=MANY_LIGHTS if which in ("cornell_many_lights", "cornell_remap") else 0,
+                                remove=REMAP_REMOVED if which == "cornell_remap" else 9001)
+    k6 = stats["K6"]
+    print(f"\n{which}: K6 ratio {k6[0]:.3g} over {k6[2]} pixels, undecided {k6[1]}, reprojected / killed / remapped "
+          f"{stats['K6 branches']}; K8 {stats['K8'][0]} rays traced, {stats['K8'][1]} differ; K9 ratio {stats['K9'][0]:.3g}, "
+          f"undecided {stats['K9'][1]} of {stats['K9'][2]} merges; K10 ratio {stats['K10'][0]:.3g}, undecided specular {stats['K10'][1]}")
     assert stats["K9"][2] > 0 and stats["K9"][1] <= 0.01 * stats["K9"][2]
-    assert 0 < stats["K10"][0] <= 1 and 0 < stats["K9"][0] <= 1
+    assert 1e-3 < stats["K10"][0] <= 1 and 1e-3 < stats["K9"][0] <= 1 and 1e-3 < k6[0] <= 1
     assert stats["K9 tight"][0] >= 0.99 * stats["K9 tight"][1] > 0, stats["K9 tight"]
+    from tests.ref64_restir import tight_ok
+    assert tight_ok(stats["K6 tight"]), stats["K6 tight"]
+    assert all(v <= 0.01 * k6[2] for v in k6[1].values()), k6[1]
+    assert stats["K6 branches"][0] > 0 and stats["K8"][0] > 0
+    if which.startswith("cornell"):     # a reprojected reservoir named light 9001 (or the light removed) after its removal
+        assert stats["K6 branches"][1] > 0
+    if which == "cornell_remap":
+        assert stats["K6 branches"][2] > 0, "no reprojected reservoir named the remapped slot"

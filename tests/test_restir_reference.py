@@ -1,4 +1,5 @@
-"""The DI spatial merge (K9) and DI resolving (K10) on the device, pass by pass and value by value, against the float64 restatement in
+"""The DI temporal resampling (K6), spatial merge (K9) and resolving (K10) on the device, pass by pass and value by value, against the
+float64 restatement in
 tests/ref64_restir.py within its derived bound for the arithmetic tier that ran (strict IEEE, or the fast-shading build: FMA
 contraction, div.full / sqrt.approx).  Also the fast build's elementary functions against the constants a bound on them assumes.
 
@@ -14,15 +15,19 @@ from tests.util import Frame, check_within, write_buffer
 
 pytestmark = pytest.mark.gpu
 
-P_DI_SPATIAL_SAMPLE, P_DI_RESOLVING = 5, 6
+P_DI_TEMPORAL, P_DI_SPATIAL_TRACE, P_DI_SPATIAL_SAMPLE, P_DI_RESOLVING = 2, 4, 5, 6
 SEED_BASE = 0xC0FFEE
 SCENES = {"cornell": scenes.cornell, "demo_level": scenes.demo_level, "textured_room": scenes.textured_room,
-          "cornell_spots": lambda w, h: scenes.cornell_spots(w, h)}
+          "cornell_spots": lambda w, h: scenes.cornell_spots(w, h), "cornell_many_lights": scenes.cornell, "cornell_remap": scenes.cornell}
 # undecided decisions allowed per pass, as a fraction of the values checked.  None were seen in the scene runs on an H100 (24 runs, both
 # tiers); the injected M = 1e6 / w = 1e6 reservoirs put 3.6 % of K9's merges inside the bound of `rng W < weight` (W dominated by the
 # huge weight, the other weight below its rounding), hence the looser limit there.
 UNDECIDED_MAX = 0.001
 UNDECIDED_MAX_EDGES = 0.1
+# K8's visibility bit against trace_any of the ray decoded in strict f32, as a fraction of the rays traced.  The strict build must
+# agree on every ray; the fast build decodes the octahedral direction with FMA contraction, so a ray grazing an edge may differ.
+# Worst seen in the fast scene runs on an H100: 3 of 29164 rays (1.0e-4, textured room 67x45); the cap is 1e-3 of the rays traced.
+K8_DISAGREE_MAX = 1e-3
 
 
 @pytest.fixture(scope="module")
@@ -39,7 +44,7 @@ def _engine(gpu, blue_noise, strict, fused):
 
 
 class Chain:
-    """Drives one camera frame by frame and checks K9 / K10 as they run."""
+    """Drives one camera frame by frame and checks K6, K8 (unfused schedule), K9 (unfused) and K10 as they run."""
 
     def __init__(self, gpu, blue_noise, scene, strict, fused):
         self.e = _engine(gpu, blue_noise, strict, fused)
@@ -48,25 +53,56 @@ class Chain:
         c = scene["camera"]
         self.w, self.h = c["w"], c["h"]
         self.t = np.asarray(c["transform"], np.float32).reshape(16).copy()
+        self.t_prev = self.t.copy()     # the camera before the last update_camera: the engine's previous camera
         self.fast = not strict
-        self.stats = {"K9": [0.0, 0, 0], "K10": [0.0, 0, 0]}
+        self.stats = {"K9": [0.0, 0, 0], "K10": [0.0, 0, 0], "K6": [0.0, {}, 0], "K8": [0, 0]}
+        self.k6_tight = {k: [0, 0] for k in ("m", "w", "pdf")}
+        self.k6_branches = [0, 0, 0]    # reprojected, killed, remapped
         self.k9_tight = [0, 0]     # (tightly bounded, finite nonzero) m and w of the merged pairs
         self.bounds = []
         self.f = 0
 
     def move(self, f):
         c = self.scene["camera"]
+        self.t_prev = self.t.copy()
         self.t[12] += np.float32(0.013 * f); self.t[13] += np.float32(0.004 * f)
         self.e.update_camera(self.cam, c["mode"], c["denoise"], c["ref_depth"], self.w, self.h, self.t, c["projection"])
 
-    def frame(self, inject_k9=None, inject_k10=None):
+    def frame(self, inject_k9=None, inject_k10=None, inject_k6=None):
         e, cam, w, h = self.e, self.cam, self.w, self.h
         self.f += 1
         f = self.f
         e.tick()
         fr = Frame(e, cam, w, h)
         cur = "b" if f % 2 == 1 else "a"
+        old = "a" if cur == "b" else "b"
         k9 = fr.steps(P_DI_SPATIAL_SAMPLE)
+        if k9:   # unfused schedule: K6 reads K5's samples from di_reservoirs[1]
+            k6 = fr.steps(P_DI_TEMPORAL)[0]
+            fr.run_to(k6 - 1)
+            if inject_k6:
+                inject_k6(fr)
+            gb = [fr.read(f"prim_gbuffer_d{k}_{cur}") for k in (0, 1)]
+            gb_prev = [fr.read(f"prim_gbuffer_d{k}_{old}") for k in (0, 1)]
+            r1, r0 = e.read_buffer(cam, "di_reservoirs_1"), e.read_buffer(cam, "di_reservoirs_0")
+            proj = self.scene["camera"]["projection"]
+            r = Q.di_temporal(Q.ndc_to_world(self.t, proj), Q.ndc_to_world(self.t_prev, proj), w, h, gb, gb_prev, fr.read("reprojection_map"),
+                              e.read_scene("lights"), r1, r0, Q.dispatch_seed(SEED_BASE, f, P_DI_TEMPORAL), self.fast)
+            fr.run_to(k6)
+            ratio, und, n = Q.check_temporal(e.read_buffer(cam, "di_reservoirs_1"), r1, r, f"f{f} K6")
+            s = self.stats["K6"]
+            self.stats["K6"] = [max(s[0], ratio), {k: s[1].get(k, 0) + v for k, v in und.items()}, s[2] + n]
+            for k, (tt, nn) in Q.temporal_tight(r).items():
+                self.k6_tight[k][0] += tt; self.k6_tight[k][1] += nn
+            self.k6_branches = [a + r[b] for a, b in zip(self.k6_branches, ("reprojected", "killed", "remapped"))]
+            k8 = fr.steps(P_DI_SPATIAL_TRACE)[0]
+            fr.run_to(k8 - 1)
+            b0, b1 = fr.read("di_diff_samples"), fr.read("di_diff_curr_colors")
+            fr.run_to(k8)
+            traced, bad = Q.check_spatial_trace(b0, b1, fr.read("di_diff_stash"), e.trace_any, f"f{f} K8")
+            if not self.fast:
+                assert bad == 0, f"f{f} K8: {bad} of {traced} visibility bits differ from trace_any"
+            self.stats["K8"] = [self.stats["K8"][0] + traced, self.stats["K8"][1] + bad]
         if k9:   # unfused schedule: K9 reads K8's visibility texels from di_diff_stash
             fr.run_to(k9[0] - 1)
             if inject_k9:
@@ -96,13 +132,18 @@ class Chain:
         return r
 
     def report(self, tag, limit=UNDECIDED_MAX):
-        s9, s10 = self.stats["K9"], self.stats["K10"]
-        print(f"\n{tag}: K9 ratio {s9[0]:.3g} undecided {s9[1]}/{s9[2]}; K10 ratio {s10[0]:.3g} undecided specular {s10[1]}/{s10[2]}")
+        s9, s10, s6, s8 = self.stats["K9"], self.stats["K10"], self.stats["K6"], self.stats["K8"]
+        print(f"\n{tag}: K6 ratio {s6[0]:.3g} undecided {s6[1]} of {s6[2]}, reprojected / killed / remapped {self.k6_branches}; "
+              f"K8 visibility differs {s8[1]}/{s8[0]}; K9 ratio {s9[0]:.3g} undecided {s9[1]}/{s9[2]}; "
+              f"K10 ratio {s10[0]:.3g} undecided specular {s10[1]}/{s10[2]}")
         assert s9[1] <= limit * max(s9[2], 1) and s10[1] <= limit * max(s10[2], 1)
+        assert all(v <= limit * max(s6[2], 1) for v in s6[1].values()), s6[1]
+        assert s8[1] <= K8_DISAGREE_MAX * s8[0], s8
 
 
-def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11)):
+def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11), extra_lights=0, remove=9001):
     ch = Chain(gpu, blue_noise, scene, strict, fused)
+    many_lights(ch.e, extra_lights)
     for f in range(1, frames + 1):
         if f in moves:
             ch.move(f)
@@ -111,26 +152,32 @@ def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11)):
         if f == 7:
             ch.e.insert_light(9001, scenes.LIGHT_POINT, scenes.point_light((-0.3, 0.8, 0.1), 0.08, (3.0, 2.0, 1.0), 6.0))
         if f == 10:
-            ch.e.remove_light(9001)
+            ch.e.remove_light(remove)
         ch.frame()
     return ch
 
 
 @pytest.mark.parametrize("size", [(224, 126), (67, 45), (37, 29)])
-@pytest.mark.parametrize("scene_name", ["cornell", "demo_level", "textured_room", "cornell_spots"])
+@pytest.mark.parametrize("scene_name", ["cornell", "demo_level", "textured_room", "cornell_spots", "cornell_many_lights", "cornell_remap"])
 @pytest.mark.parametrize("strict", [True, False], ids=["strict", "fast"])
 def test_di_merge_and_resolve_within_float64_bound(gpu, blue_noise, strict, scene_name, size):
-    """K9 and K10 in the unfused schedule, every pair / pixel, frames 1-13 (both GI cycles) with the camera moving and a light
-    inserted, moved and removed; 67x45 leaves columns outside the half grid, 37x29 is smaller than the 128 px tap radius."""
-    ch = _run(gpu, blue_noise, SCENES[scene_name](*size), strict, fused=False)
-    assert ch.stats["K9"][2] > 0 and 0 < ch.stats["K10"][0] <= 1
+    """K6, K8, K9 and K10 in the unfused schedule, every pixel / texel / pair, frames 1-13 (both GI cycles) with the camera moving
+    and a light inserted, moved and removed; 67x45 leaves columns outside the half grid, 37x29 is smaller than the 128 px tap radius.
+    Many lights: 23, so K5 draws 16 of them; remap: the light removed is from the middle of the list, so K6 meets a remapped slot."""
+    many = scene_name in ("cornell_many_lights", "cornell_remap")
+    ch = _run(gpu, blue_noise, SCENES[scene_name](*size), strict, fused=False, extra_lights=MANY_LIGHTS if many else 0,
+              remove=REMAP_REMOVED if scene_name == "cornell_remap" else 9001)
+    assert ch.stats["K9"][2] > 0 and 0 < ch.stats["K10"][0] <= 1 and 0 < ch.stats["K6"][0] <= 1 and ch.stats["K8"][0] > 0
+    assert ch.k6_branches[0] > 0 and Q.tight_ok(ch.k6_tight), (ch.k6_branches, ch.k6_tight)
+    if scene_name == "cornell_remap":
+        assert ch.k6_branches[2] > 0, "no reprojected reservoir named the remapped slot"
     ch.report(f"{scene_name} {size} {'strict' if strict else 'fast'}")
     # the bound is not vacuous: most values are bounded tightly, and some error uses a visible part of its bound
     b, some = ch.bounds[-1]
     frac, n = Q.tight_fraction(list(b), some)
     assert n > 0 and frac >= 0.99, frac
     assert ch.k9_tight[1] > 0 and ch.k9_tight[0] >= 0.99 * ch.k9_tight[1], ch.k9_tight
-    assert ch.stats["K10"][0] > 1e-3 and ch.stats["K9"][0] > 1e-3
+    assert ch.stats["K10"][0] > 1e-3 and ch.stats["K9"][0] > 1e-3 and ch.stats["K6"][0] > 1e-3
 
 
 @pytest.mark.parametrize("scene_name", ["cornell", "demo_level"])
@@ -197,20 +244,58 @@ def edge_lights(engine):
     engine.insert_light(9104, scenes.LIGHT_SPOT, scenes.spot_light((0.0, 1.7, 0.0), 0.02, (4.0, 4.0, 3.0), 10.0, (0.0, -1.0, 0.0), 0.15))
 
 
+def _temporal_edges(seed):
+    """Rewrites K6's inputs: in di_reservoirs[0] M at 63, 64, 65 and 1e6 and w at 0, a denormal and 1e6; in the reprojection map,
+    previous positions at exact .5 fractions (round half away from zero) and on the last row and column.  No position is moved
+    outside the frame: frame reprojection never produces one, and the reference would read outside its buffers."""
+    def inject(fr):
+        rng = np.random.RandomState(seed)
+        r = fr.e.read_buffer(fr.cam, "di_reservoirs_0").reshape(-1, 8).copy()
+        live = r[:, 0] > 0
+        k = rng.randint(0, 8, len(r))
+        r[:, 0] = np.where(live & (k == 1), 63, np.where(live & (k == 2), 64, np.where(live & (k == 3), 65, np.where(live & (k == 4), 1e6, r[:, 0]))))
+        r[:, 1] = np.where(live & (k == 5), 0, np.where(live & (k == 6), np.float32(1e-41), np.where(live & (k == 7), 1e6, r[:, 1])))
+        write_buffer(fr.e, fr.cam, "di_reservoirs_0", r.astype(np.float32))
+        m = fr.read("reprojection_map").copy()
+        some = m[..., 2] > 0
+        j = rng.randint(0, 5, some.shape)
+        half = lambda v, n: np.minimum(np.floor(v), n - 2) + np.float32(0.5)     # rounds up to at most n - 1
+        m[..., 0] = np.where(some & (j == 1), half(m[..., 0], fr.w), np.where(some & (j == 3), fr.w - 1, m[..., 0]))
+        m[..., 1] = np.where(some & (j == 2), half(m[..., 1], fr.h), np.where(some & (j == 4), fr.h - 1, m[..., 1]))
+        fr.write("reprojection_map", m)
+    return inject
+
+
+MANY_LIGHTS = 21        # with Cornell's point light and the sun: 23 lights, so K5 draws 16 of them and `% light_count` is not trivial
+REMAP_REMOVED = 9210    # a light from the middle of that list: removing it remaps the last slot as well as killing its own
+
+
+def many_lights(engine, n):
+    """n small point lights on a ring under the Cornell box's ceiling, handles 9200 + i."""
+    for i in range(n):
+        a = 2 * np.pi * i / max(n, 1)
+        engine.insert_light(9200 + i, scenes.LIGHT_POINT, scenes.point_light((0.7 * np.cos(a), 1.6 + 0.1 * (i % 3), 0.7 * np.sin(a)),
+                                                                             0.03, (0.4 + 0.1 * (i % 4), 0.5, 0.6 - 0.1 * (i % 3)), 4.0))
+
+
 @pytest.mark.parametrize("strict", [True, False], ids=["strict", "fast"])
 @pytest.mark.parametrize("scene_name", ["cornell", "cornell_spots"])
 def test_di_edge_inputs_within_bound(gpu, blue_noise, strict, scene_name):
-    """Edge contents injected before K9 (M at the cap region and far past it, w 0 / denormal / 1e6, pdf 0) and before K10 (metallic
-    and reflectance bytes 0 / 255, roughness byte 0, normals along the view direction at minimum roughness), with the edge lights."""
+    """Edge contents injected before K6 (last frame's M around the clamp of 64 and far past it, w 0 / denormal / 1e6, reprojected
+    positions on .5 fractions and on the last row and column), before K9 (M at the cap region and far past it, w 0 / denormal / 1e6,
+    pdf 0) and before K10 (metallic and reflectance bytes 0 / 255, roughness byte 0, normals along the view direction at minimum
+    roughness), with the edge lights and the camera moving."""
     ch = Chain(gpu, blue_noise, SCENES[scene_name](67, 45), strict, fused=False)
     edge_lights(ch.e)
     for f in range(1, 6):
-        ch.frame(_reservoir_edges(10 * f), _gbuffer_edges(10 * f + 1, ch))
+        if f in (2, 4):
+            ch.move(f)
+        ch.frame(_reservoir_edges(10 * f), _gbuffer_edges(10 * f + 1, ch), _temporal_edges(10 * f + 2))
     ch.report(f"edges {scene_name} {'strict' if strict else 'fast'}", UNDECIDED_MAX_EDGES)
 
 
 def test_fast_shading_build_is_not_strict(gpu, blue_noise):
-    """The fast-tier runs above really ran the fast build: the same inputs through the strict K9 and the strict K10 give different bits
+    """The fast-tier runs above really ran the fast build: the same inputs through the strict K6, K9 and K10 give different bits
     somewhere in each pass's output."""
     from strolle_b200.engine import OPT_SHADING_FAST_MATH
     e = _engine(gpu, blue_noise, False, False)
@@ -219,10 +304,14 @@ def test_fast_shading_build_is_not_strict(gpu, blue_noise):
         e.tick(); e.render_camera(cam)
     e.tick()
     fr = Frame(e, cam, 67, 45)
-    k9, k10 = fr.steps(P_DI_SPATIAL_SAMPLE)[0], fr.steps(P_DI_RESOLVING)[0]
+    k6, k9, k10 = fr.steps(P_DI_TEMPORAL)[0], fr.steps(P_DI_SPATIAL_SAMPLE)[0], fr.steps(P_DI_RESOLVING)[0]
+    fr.run_to(k6 - 1)
+    pre6 = {n: e.read_buffer(cam, n).copy() for n in ("di_reservoirs_0", "di_reservoirs_1")}   # K6's reservoir inputs
+    fr.run_to(k6)
+    fast6 = e.read_buffer(cam, "di_reservoirs_1").copy()
     fr.run_to(k9)                        # K9 reads di_reservoirs[1] and the stash, which it leaves as they were
     fast9 = e.read_buffer(cam, "di_reservoirs_2").copy()
-    fr.run_to(k10)                       # K10 reads di_reservoirs[2] and the G-buffer, and writes neither
+    fr.run_to(k10)                       # K10 reads di_reservoirs[2] and the G-buffer; it writes di_reservoirs[0]
     fast10 = fr.read("di_spec_samples").copy(), fr.read("di_diff_samples").copy()
     e.set_option(OPT_SHADING_FAST_MATH, 0)
     e.render_range(cam, k10, k10)
@@ -231,6 +320,19 @@ def test_fast_shading_build_is_not_strict(gpu, blue_noise):
     strict9 = e.read_buffer(cam, "di_reservoirs_2")
     assert (fast9.view(np.uint32) != strict9.view(np.uint32)).any(), "K9"
     assert any((a.view(np.uint32) != b.view(np.uint32)).any() for a, b in zip(fast10, strict10)), "K10"
+
+    def rerun_k6(fast):
+        """K6 again on its own inputs: last frame's reservoirs (which K10 has since overwritten) and K5's samples (which K6 updates
+        in place) are put back first."""
+        for n, a in pre6.items():
+            write_buffer(e, cam, n, a)
+        e.set_option(OPT_SHADING_FAST_MATH, int(fast))
+        e.render_range(cam, k6, k6)
+        return e.read_buffer(cam, "di_reservoirs_1").copy()
+    strict6 = rerun_k6(False)
+    # the inputs are restored completely: the fast K6 run again gives its first result bit for bit
+    assert (rerun_k6(True).view(np.uint32) == fast6.view(np.uint32)).all(), "K6 re-run on restored inputs"
+    assert (fast6.view(np.uint32) != strict6.view(np.uint32)).any(), "K6"
 
 
 # ---- the fast build's elementary functions ------------------------------------------------------------------------------------
