@@ -394,7 +394,8 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
     t = np.asarray(c["transform"], np.float32).reshape(16).copy()
     t_prev = t.copy()          # the camera before the last update_camera: what the engine keeps as the previous camera
     stats = {"K6": [0.0, {}, 0], "K6 tight": {k: [0, 0] for k in ("m", "w", "pdf")}, "K6 branches": [0, 0, 0], "K8": [0, 0],
-             "K9": [0.0, 0, 0], "K10": [0.0, 0], "K9 tight": [0, 0]}
+             "K9": [0.0, 0, 0], "K10": [0.0, 0], "K9 tight": [0, 0], "K5": [0.0, {}, 0, 0],
+             "K5 tight": {k: [0, 0] for k in ("w", "light_point")}}
     if edge_lights:
         from tests.test_restir_reference import edge_lights as add_lights
         add_lights(e)
@@ -413,11 +414,26 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
             e.remove_light(remove)
         e.tick()
         sched = e.frame_schedule(cam)
-        k6, k8, k9, k10 = sched.index(2), sched.index(4), sched.index(5), sched.index(6)
+        k5, k6, k8, k9, k10 = sched.index(1), sched.index(2), sched.index(4), sched.index(5), sched.index(6)
         rd = lambda n: e.read_buffer(cam, n)
         cur = "b" if f % 2 == 1 else "a"
         old = "a" if cur == "b" else "b"
-        e.render_range(cam, 0, k6 - 1)
+        e.render_range(cam, 0, k5 - 1)
+        r1 = rd("di_reservoirs_1")
+        k5r = Q.di_sampling(Q.ndc_to_world(t, c["projection"]), w, h, rd(f"prim_gbuffer_d0_{cur}").reshape(h, w, 4),
+                            rd(f"prim_gbuffer_d1_{cur}").reshape(h, w, 4), e.read_scene("lights"),
+                            e.read_scene("world")[:1].view(np.uint32)[0], blue_noise, Q.dispatch_seed(0xC0FFEE, f, 1), f, fast=False)
+        e.render_range(cam, k5, k5)
+        s5 = Q.check_sampling(rd("di_reservoirs_1"), r1, k5r, lambda x: oracle.math("sin", x), lambda x: oracle.math("cos", x),
+                              e.trace_any, f"f{f} K5")
+        assert s5["disagree"] == 0, f"f{f} K5: {s5['disagree']} of {s5['traced']} occluded bits differ from trace_any"
+        assert_bits_equal(s5["got"][:, 4:7], s5["lp_f32"], f"f{f} K5 light point against its strict f32 rebuild")
+        k5s = stats["K5"]
+        stats["K5"] = [max(k5s[0], s5["ratio"]), {k: k5s[1].get(k, 0) + v for k, v in s5["undecided"].items()}, k5s[2] + s5["n"],
+                       k5s[3] + s5["traced"]]
+        for k, (tt, nn) in s5["tight"].items():
+            stats["K5 tight"][k][0] += tt; stats["K5 tight"][k][1] += nn
+        e.render_range(cam, k5 + 1, k6 - 1)
         gb = [rd(f"prim_gbuffer_d{k}_{cur}").reshape(h, w, 4) for k in (0, 1)]
         gb_prev = [rd(f"prim_gbuffer_d{k}_{old}").reshape(h, w, 4) for k in (0, 1)]
         r1, r0 = rd("di_reservoirs_1"), rd("di_reservoirs_0")
@@ -496,17 +512,21 @@ def test_restir_float64_chain_matches_oracle(oracle, blue_noise, which):
     stats = _restir_chain_check(oracle, blue_noise, scene, edge_lights=which == "cornell_edge_lights",
                                 extra_lights=MANY_LIGHTS if which in ("cornell_many_lights", "cornell_remap") else 0,
                                 remove=REMAP_REMOVED if which == "cornell_remap" else 9001)
-    k6 = stats["K6"]
-    print(f"\n{which}: K6 ratio {k6[0]:.3g} over {k6[2]} pixels, undecided {k6[1]}, reprojected / killed / remapped "
+    k6, k5 = stats["K6"], stats["K5"]
+    print(f"\n{which}: K5 ratio {k5[0]:.3g} over {k5[2]} pixels, undecided {k5[1]}, {k5[3]} shadow rays, tight {stats['K5 tight']}; "
+          f"K6 ratio {k6[0]:.3g} over {k6[2]} pixels, undecided {k6[1]}, reprojected / killed / remapped "
           f"{stats['K6 branches']}; K8 {stats['K8'][0]} rays traced, {stats['K8'][1]} differ; K9 ratio {stats['K9'][0]:.3g}, "
           f"undecided {stats['K9'][1]} of {stats['K9'][2]} merges; K10 ratio {stats['K10'][0]:.3g}, undecided specular {stats['K10'][1]}")
     assert stats["K9"][2] > 0 and stats["K9"][1] <= 0.01 * stats["K9"][2]
     assert 1e-3 < stats["K10"][0] <= 1 and 1e-3 < stats["K9"][0] <= 1 and 1e-3 < k6[0] <= 1
     assert stats["K9 tight"][0] >= 0.99 * stats["K9 tight"][1] > 0, stats["K9 tight"]
+    from tests import ref64_restir as Q
     from tests.ref64_restir import tight_ok
     assert tight_ok(stats["K6 tight"]), stats["K6 tight"]
     assert all(v <= 0.01 * k6[2] for v in k6[1].values()), k6[1]
     assert stats["K6 branches"][0] > 0 and stats["K8"][0] > 0
+    assert 1e-3 < k5[0] <= 1 and k5[3] > 0 and Q.sampling_tight_ok(stats["K5 tight"]), stats["K5 tight"]
+    assert all(v <= 0.01 * k5[2] for v in k5[1].values()), k5[1]
     if which.startswith("cornell"):     # a reprojected reservoir named light 9001 (or the light removed) after its removal
         assert stats["K6 branches"][1] > 0
     if which == "cornell_remap":

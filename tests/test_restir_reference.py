@@ -1,4 +1,4 @@
-"""The DI temporal resampling (K6), spatial merge (K9) and resolving (K10) on the device, pass by pass and value by value, against the
+"""The DI sampling (K5), temporal resampling (K6), spatial merge (K9) and resolving (K10) on the device, pass by pass and value by value, against the
 float64 restatement in
 tests/ref64_restir.py within its derived bound for the arithmetic tier that ran (strict IEEE, or the fast-shading build: FMA
 contraction, div.full / sqrt.approx).  Also the fast build's elementary functions against the constants a bound on them assumes.
@@ -15,7 +15,7 @@ from tests.util import Frame, check_within, write_buffer
 
 pytestmark = pytest.mark.gpu
 
-P_DI_TEMPORAL, P_DI_SPATIAL_TRACE, P_DI_SPATIAL_SAMPLE, P_DI_RESOLVING = 2, 4, 5, 6
+P_DI_SAMPLING, P_DI_TEMPORAL, P_DI_SPATIAL_TRACE, P_DI_SPATIAL_SAMPLE, P_DI_RESOLVING = 1, 2, 4, 5, 6
 SEED_BASE = 0xC0FFEE
 SCENES = {"cornell": scenes.cornell, "demo_level": scenes.demo_level, "textured_room": scenes.textured_room,
           "cornell_spots": lambda w, h: scenes.cornell_spots(w, h), "cornell_many_lights": scenes.cornell, "cornell_remap": scenes.cornell}
@@ -28,6 +28,7 @@ UNDECIDED_MAX_EDGES = 0.1
 # agree on every ray; the fast build decodes the octahedral direction with FMA contraction, so a ray grazing an edge may differ.
 # Worst seen in the fast scene runs on an H100: 3 of 29164 rays (1.0e-4, textured room 67x45); the cap is 1e-3 of the rays traced.
 K8_DISAGREE_MAX = 1e-3
+K5_EVERY_FRAME_PX = 67 * 45     # screens up to this size check K5 on every frame, larger ones on every third (Chain.frame)
 
 
 @pytest.fixture(scope="module")
@@ -44,7 +45,7 @@ def _engine(gpu, blue_noise, strict, fused):
 
 
 class Chain:
-    """Drives one camera frame by frame and checks K6, K8 (unfused schedule), K9 (unfused) and K10 as they run."""
+    """Drives one camera frame by frame and checks K5, K6, K8, K9 (these four in the unfused schedule) and K10 as they run."""
 
     def __init__(self, gpu, blue_noise, scene, strict, fused):
         self.e = _engine(gpu, blue_noise, strict, fused)
@@ -55,7 +56,9 @@ class Chain:
         self.t = np.asarray(c["transform"], np.float32).reshape(16).copy()
         self.t_prev = self.t.copy()     # the camera before the last update_camera: the engine's previous camera
         self.fast = not strict
-        self.stats = {"K9": [0.0, 0, 0], "K10": [0.0, 0, 0], "K6": [0.0, {}, 0], "K8": [0, 0]}
+        self.blue_noise = blue_noise
+        self.stats = {"K9": [0.0, 0, 0], "K10": [0.0, 0, 0], "K6": [0.0, {}, 0], "K8": [0, 0], "K5": [0.0, {}, 0, 0, 0]}
+        self.k5_tight = {k: [0, 0] for k in ("w", "light_point")}
         self.k6_tight = {k: [0, 0] for k in ("m", "w", "pdf")}
         self.k6_branches = [0, 0, 0]    # reprojected, killed, remapped
         self.k9_tight = [0, 0]     # (tightly bounded, finite nonzero) m and w of the merged pairs
@@ -68,6 +71,27 @@ class Chain:
         self.t[12] += np.float32(0.013 * f); self.t[13] += np.float32(0.004 * f)
         self.e.update_camera(self.cam, c["mode"], c["denoise"], c["ref_depth"], self.w, self.h, self.t, c["projection"])
 
+    def _check_sampling(self, fr, cur):
+        e, cam, w, h, f = self.e, self.cam, self.w, self.h, self.f
+        k5 = fr.steps(P_DI_SAMPLING)[0]
+        fr.run_to(k5 - 1)
+        r1 = e.read_buffer(cam, "di_reservoirs_1")
+        r = Q.di_sampling(Q.ndc_to_world(self.t, self.scene["camera"]["projection"]), w, h, fr.read(f"prim_gbuffer_d0_{cur}"),
+                          fr.read(f"prim_gbuffer_d1_{cur}"), e.read_scene("lights"), e.read_scene("world")[:1].view(np.uint32)[0],
+                          self.blue_noise, Q.dispatch_seed(SEED_BASE, f, P_DI_SAMPLING), f, self.fast)
+        fr.run_to(k5)
+        s5 = Q.check_sampling(e.read_buffer(cam, "di_reservoirs_1"), r1, r, lambda x: e.device_math("sin", x),
+                              lambda x: e.device_math("cos", x), e.trace_any, f"f{f} K5")
+        if not self.fast:
+            assert s5["disagree"] == 0, f"f{f} K5: {s5['disagree']} of {s5['traced']} occluded bits differ from trace_any"
+            lp = s5["got"][:, 4:7]
+            assert (lp.view(np.uint32) == s5["lp_f32"].view(np.uint32)).all(), f"f{f} K5: light point differs from its strict f32 rebuild"
+        s = self.stats["K5"]
+        self.stats["K5"] = [max(s[0], s5["ratio"]), {k: s[1].get(k, 0) + v for k, v in s5["undecided"].items()}, s[2] + s5["n"],
+                            s[3] + s5["traced"], s[4] + s5["disagree"]]
+        for k, (tt, nn) in s5["tight"].items():
+            self.k5_tight[k][0] += tt; self.k5_tight[k][1] += nn
+
     def frame(self, inject_k9=None, inject_k10=None, inject_k6=None):
         e, cam, w, h = self.e, self.cam, self.w, self.h
         self.f += 1
@@ -77,7 +101,11 @@ class Chain:
         cur = "b" if f % 2 == 1 else "a"
         old = "a" if cur == "b" else "b"
         k9 = fr.steps(P_DI_SPATIAL_SAMPLE)
-        if k9:   # unfused schedule: K6 reads K5's samples from di_reservoirs[1]
+        if k9:   # unfused schedule: K5 writes its samples to di_reservoirs[1], K6 reads them from there
+            # K5 carries no state from frame to frame, so above K5_EVERY_FRAME_PX pixels it is checked on every third frame (1, 4, 7,
+            # 10, 13: the frames that insert, move and remove a light); its f64 restatement is the costliest of the chain
+            if w * h <= K5_EVERY_FRAME_PX or f % 3 == 1:
+                self._check_sampling(fr, cur)
             k6 = fr.steps(P_DI_TEMPORAL)[0]
             fr.run_to(k6 - 1)
             if inject_k6:
@@ -132,13 +160,16 @@ class Chain:
         return r
 
     def report(self, tag, limit=UNDECIDED_MAX):
-        s9, s10, s6, s8 = self.stats["K9"], self.stats["K10"], self.stats["K6"], self.stats["K8"]
-        print(f"\n{tag}: K6 ratio {s6[0]:.3g} undecided {s6[1]} of {s6[2]}, reprojected / killed / remapped {self.k6_branches}; "
+        s9, s10, s6, s8, s5 = self.stats["K9"], self.stats["K10"], self.stats["K6"], self.stats["K8"], self.stats["K5"]
+        print(f"\n{tag}: K5 ratio {s5[0]:.3g} undecided {s5[1]} of {s5[2]}, shadow rays differ {s5[4]}/{s5[3]}, tight {self.k5_tight}; "
+              f"K6 ratio {s6[0]:.3g} undecided {s6[1]} of {s6[2]}, reprojected / killed / remapped {self.k6_branches}; "
               f"K8 visibility differs {s8[1]}/{s8[0]}; K9 ratio {s9[0]:.3g} undecided {s9[1]}/{s9[2]}; "
               f"K10 ratio {s10[0]:.3g} undecided specular {s10[1]}/{s10[2]}")
         assert s9[1] <= limit * max(s9[2], 1) and s10[1] <= limit * max(s10[2], 1)
         assert all(v <= limit * max(s6[2], 1) for v in s6[1].values()), s6[1]
         assert s8[1] <= K8_DISAGREE_MAX * s8[0], s8
+        assert all(v <= limit * max(s5[2], 1) for v in s5[1].values()), s5[1]
+        assert s5[4] <= K8_DISAGREE_MAX * s5[3], s5
 
 
 def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11), extra_lights=0, remove=9001):
@@ -161,7 +192,7 @@ def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11), 
 @pytest.mark.parametrize("scene_name", ["cornell", "demo_level", "textured_room", "cornell_spots", "cornell_many_lights", "cornell_remap"])
 @pytest.mark.parametrize("strict", [True, False], ids=["strict", "fast"])
 def test_di_merge_and_resolve_within_float64_bound(gpu, blue_noise, strict, scene_name, size):
-    """K6, K8, K9 and K10 in the unfused schedule, every pixel / texel / pair, frames 1-13 (both GI cycles) with the camera moving
+    """K5, K6, K8, K9 and K10 in the unfused schedule, every pixel / texel / pair, frames 1-13 (both GI cycles) with the camera moving
     and a light inserted, moved and removed; 67x45 leaves columns outside the half grid, 37x29 is smaller than the 128 px tap radius.
     Many lights: 23, so K5 draws 16 of them; remap: the light removed is from the middle of the list, so K6 meets a remapped slot."""
     many = scene_name in ("cornell_many_lights", "cornell_remap")
@@ -178,6 +209,9 @@ def test_di_merge_and_resolve_within_float64_bound(gpu, blue_noise, strict, scen
     assert n > 0 and frac >= 0.99, frac
     assert ch.k9_tight[1] > 0 and ch.k9_tight[0] >= 0.99 * ch.k9_tight[1], ch.k9_tight
     assert ch.stats["K10"][0] > 1e-3 and ch.stats["K9"][0] > 1e-3 and ch.stats["K6"][0] > 1e-3
+    assert 1e-3 < ch.stats["K5"][0] <= 1 and ch.stats["K5"][3] > 0 and Q.sampling_tight_ok(ch.k5_tight), ch.k5_tight
+
+
 
 
 @pytest.mark.parametrize("scene_name", ["cornell", "demo_level"])
@@ -284,18 +318,28 @@ def test_di_edge_inputs_within_bound(gpu, blue_noise, strict, scene_name):
     """Edge contents injected before K6 (last frame's M around the clamp of 64 and far past it, w 0 / denormal / 1e6, reprojected
     positions on .5 fractions and on the last row and column), before K9 (M at the cap region and far past it, w 0 / denormal / 1e6,
     pdf 0) and before K10 (metallic and reflectance bytes 0 / 255, roughness byte 0, normals along the view direction at minimum
-    roughness), with the edge lights and the camera moving."""
-    ch = Chain(gpu, blue_noise, SCENES[scene_name](67, 45), strict, fused=False)
+    roughness), with the edge lights and the camera moving.  The light table is filled up to K5's boundaries: 16 lights on Cornell,
+    where max_samples = min(light_count, 16) first reaches its cap, and 17 with the spot lights, the first count past it, where
+    `% light_count` leaves some lights undrawn (23, further past it, is the many-lights scene run)."""
+    scene = SCENES[scene_name](67, 45)
+    ch = Chain(gpu, blue_noise, scene, strict, fused=False)
     edge_lights(ch.e)
+    want = EDGE_LIGHT_COUNT[scene_name]
+    many_lights(ch.e, want - (len(scene["lights"]) + 1 + 4))       # + the sun and the four edge lights
     for f in range(1, 6):
         if f in (2, 4):
             ch.move(f)
         ch.frame(_reservoir_edges(10 * f), _gbuffer_edges(10 * f + 1, ch), _temporal_edges(10 * f + 2))
-    ch.report(f"edges {scene_name} {'strict' if strict else 'fast'}", UNDECIDED_MAX_EDGES)
+        assert ch.e.read_scene("world")[:1].view(np.uint32)[0] == want
+    assert 0 < ch.stats["K5"][0] <= 1 and ch.stats["K5"][2] > 0
+    ch.report(f"edges {scene_name} {want} lights {'strict' if strict else 'fast'}", UNDECIDED_MAX_EDGES)
+
+
+EDGE_LIGHT_COUNT = {"cornell": 16, "cornell_spots": 17}
 
 
 def test_fast_shading_build_is_not_strict(gpu, blue_noise):
-    """The fast-tier runs above really ran the fast build: the same inputs through the strict K6, K9 and K10 give different bits
+    """The fast-tier runs above really ran the fast build: the same inputs through the strict K5, K6, K9 and K10 give different bits
     somewhere in each pass's output."""
     from strolle_b200.engine import OPT_SHADING_FAST_MATH
     e = _engine(gpu, blue_noise, False, False)
@@ -304,7 +348,11 @@ def test_fast_shading_build_is_not_strict(gpu, blue_noise):
         e.tick(); e.render_camera(cam)
     e.tick()
     fr = Frame(e, cam, 67, 45)
-    k6, k9, k10 = fr.steps(P_DI_TEMPORAL)[0], fr.steps(P_DI_SPATIAL_SAMPLE)[0], fr.steps(P_DI_RESOLVING)[0]
+    k5, k6, k9, k10 = fr.steps(P_DI_SAMPLING)[0], fr.steps(P_DI_TEMPORAL)[0], fr.steps(P_DI_SPATIAL_SAMPLE)[0], fr.steps(P_DI_RESOLVING)[0]
+    fr.run_to(k5 - 1)
+    pre5 = e.read_buffer(cam, "di_reservoirs_1").copy()      # K5 reads the G-buffer, the lights and the blue noise; it writes this
+    fr.run_to(k5)
+    fast5 = e.read_buffer(cam, "di_reservoirs_1").copy()
     fr.run_to(k6 - 1)
     pre6 = {n: e.read_buffer(cam, n).copy() for n in ("di_reservoirs_0", "di_reservoirs_1")}   # K6's reservoir inputs
     fr.run_to(k6)
@@ -333,6 +381,15 @@ def test_fast_shading_build_is_not_strict(gpu, blue_noise):
     # the inputs are restored completely: the fast K6 run again gives its first result bit for bit
     assert (rerun_k6(True).view(np.uint32) == fast6.view(np.uint32)).all(), "K6 re-run on restored inputs"
     assert (fast6.view(np.uint32) != strict6.view(np.uint32)).any(), "K6"
+
+    def rerun_k5(fast):
+        write_buffer(e, cam, "di_reservoirs_1", pre5)
+        e.set_option(OPT_SHADING_FAST_MATH, int(fast))
+        e.render_range(cam, k5, k5)
+        return e.read_buffer(cam, "di_reservoirs_1").copy()
+    strict5 = rerun_k5(False)
+    assert (rerun_k5(True).view(np.uint32) == fast5.view(np.uint32)).all(), "K5 re-run on restored inputs"
+    assert (fast5.view(np.uint32) != strict5.view(np.uint32)).any(), "K5"
 
 
 # ---- the fast build's elementary functions ------------------------------------------------------------------------------------
