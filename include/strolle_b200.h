@@ -100,7 +100,8 @@ int st_remove_material(st_engine* e, st_handle material);
 int st_insert_image(st_engine* e, st_handle image, const uint8_t* rgba8, uint32_t width, uint32_t height);
 int st_remove_image(st_engine* e, st_handle image);
 /* The Option<ImageHandle> fields of strolle::Material (strolle/src/material.rs:13-22); bit i of `mask` = texture i set
- * (0 base_color, 1 emissive, 2 metallic_roughness, 3 normal_map — the last is carried but unused, as in the reference). */
+ * (0 base_color, 1 emissive, 2 metallic_roughness, 3 normal_map).  The normal map is ignored, as in the reference, unless
+ * ST_OPT_NORMAL_MAPS is on; it is then decoded linearly (byte / 255), the other three with the sRGB curve. */
 typedef struct st_material_textures { st_handle base_color, emissive, metallic_roughness, normal_map; uint32_t mask; } st_material_textures;
 int st_set_material_textures(st_engine* e, st_handle material, const st_material_textures* textures);
 /* Engine::insert_instance / remove_instance (lib.rs:217-229); affine = glam::Affine3A as
@@ -172,7 +173,13 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14 };
+/* ST_OPT_NORMAL_MAPS (default 0): materials with a normal map shade with the mapped normal, n' = normalize((t.x T + t.y B) + t.z N) with
+ * t = 2 texel / 255 - 1, T the interpolated mesh tangent (not renormalised), B = w (N x T), w its handedness (mirrored instances flip
+ * it); where n' is not finite (meshes without tangents) or n'.N <= 0 the interpolated normal N stays.  Back faces flip the result as
+ * they flip N.  It reaches the G-buffer, the surface maps, the GI bounce hits and Reference mode's hits - everything shaded - but not
+ * traversal, depth, velocity, triangle ids or the ray-stream entry points.  The reference ignores normal maps, so the default keeps
+ * parity with it; while no material has a normal map the option changes nothing.  Takes effect at the next st_tick (DESIGN.md §2). */
 /* ST_OPT_WAVELET_PAIRED (default 1; only with ST_OPT_SVGF_FAST_MATH, and never under the exchange-point strip transports, which ship the
  * named buffers between iterations): the wide-stride à-trous iterations, whose taps are scattered by the per-pixel jitter, read the DI and
  * GI signal as one interleaved 32-byte record per pixel (private scratch; one full sector per tap, loaded as two 128-bit loads on sm_90a,
@@ -234,7 +241,8 @@ int st_set_option(st_engine* e, int option, int value);
  * CTAs gave up waiting for their tensor copies (must stay 0). */
 enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_STAT_BVH_GRAFTED_SUBTREES = 3, ST_STAT_VARIANCE_TILED_LAUNCHES = 4,
        ST_STAT_STRIP_PULLED_ROWS = 5 /* rows x buffers fetched from other ranks by the temporal pull since linking */, ST_STAT_LAST_FRAME_FUSED_STRIPS = 6 /* 1 = the last strip frame used the fused transport */,
-       ST_STAT_STRIP_FIRST_TIMEOUT = 7 /* 0, or 0x80000000 | slot << 16 | awaited rank << 8 | sequence & 0xff of the first strip flag wait that gave up */ };
+       ST_STAT_STRIP_FIRST_TIMEOUT = 7 /* 0, or 0x80000000 | slot << 16 | awaited rank << 8 | sequence & 0xff of the first strip flag wait that gave up */,
+       ST_STAT_NORMAL_MAP_LAUNCHES = 8 /* launches of the normal-mapped kernel variants (ST_OPT_NORMAL_MAPS) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,

@@ -7,7 +7,7 @@
 //!
 //! `STROLLE_B200_DEVICES=0,1,2,3` selects the GPUs (default `0`); several devices = row strips of every camera's frame.
 pub mod prelude {
-    pub use crate::{StrolleCamera, StrollePlugin, StrolleSun};
+    pub use crate::{StrolleCamera, StrollePlugin, StrolleSettings, StrolleSun};
 }
 
 mod sync;
@@ -40,6 +40,14 @@ pub struct StrolleSun {
     sun: st::Sun,
 }
 
+/// Engine-wide settings, read once when the plugin finishes building; insert the resource before `StrollePlugin` to change them.
+/// `normal_maps`: shade with `StandardMaterial::normal_map_texture` and the mesh's `ATTRIBUTE_TANGENT` (off by default, as in the
+/// reference, which ignores normal maps).
+#[derive(Clone, Debug, Default, Resource)]
+pub struct StrolleSettings {
+    pub normal_maps: bool,
+}
+
 #[derive(Clone, Debug)]
 pub struct EngineParams;
 
@@ -70,13 +78,15 @@ impl Plugin for StrollePlugin {
     }
 
     fn finish(&self, app: &mut App) {
+        let settings = app.world.get_resource::<StrolleSettings>().cloned().unwrap_or_default();
         let Ok(render_app) = app.get_sub_app_mut(RenderApp) else { return };
         let devices: Vec<i32> = std::env::var("STROLLE_B200_DEVICES")
             .ok()
             .map(|v| v.split(',').filter_map(|d| d.trim().parse().ok()).collect())
             .filter(|v: &Vec<i32>| !v.is_empty())
             .unwrap_or_else(|| vec![0]);
-        let engine = st::Engine::new(&devices).expect("strolle_b200: no usable CUDA device (this engine has no CPU fallback)");
+        let mut engine = st::Engine::new(&devices).expect("strolle_b200: no usable CUDA device (this engine has no CPU fallback)");
+        engine.set_normal_maps(settings.normal_maps).expect("strolle_b200: ST_OPT_NORMAL_MAPS");
         render_app.insert_resource(EngineResource(engine));
     }
 }

@@ -421,6 +421,12 @@ impl<P: Params> Engine<P> {
         })
     }
 
+    /// Shades with the materials' normal maps (`ST_OPT_NORMAL_MAPS`, off by default: the reference ignores them).  Takes effect
+    /// with the next frame's scene update.
+    pub fn set_normal_maps(&mut self, on: bool) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_NORMAL_MAPS, on as c_int) })
+    }
+
     /// Creates or updates a mesh (`lib.rs:161-164`).
     pub fn insert_mesh(&mut self, handle: P::MeshHandle, item: Mesh) {
         let id = self.meshes.id(handle);

@@ -442,6 +442,9 @@ struct st_engine {
     bool fuse_reproject = ST_FUSE_REPROJECT_DEFAULT != 0;   // ST_OPT_FUSE_REPROJECT
     bool bvh_reuse = true;   // ST_OPT_BVH_REUSE
     bool variance_tiled = ST_VARIANCE_TILED_DEFAULT != 0; uint64_t variance_tiled_launches = 0;   // ST_OPT_VARIANCE_TILED
+    // ST_OPT_NORMAL_MAPS: `normal_maps` is the option, `any_normal_map` whether some material has a normal-map rect (set when materials
+    // are uploaded), `nmap_frame` their conjunction taken at st_tick: the frame's hit-shading kernels run their NMAP instantiation
+    bool normal_maps = false, any_normal_map = false, nmap_frame = false; uint64_t normal_map_launches = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -658,6 +661,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     const int cur = (f % 2u) == 1u ? 1 : 0;   // is_alternate (camera_controller.rs:185-187)
     const st_camera& d = cs->desc;
     const bool fs = e->shading_fast;   // ReSTIR kernels from the fast-shading build (ST_OPT_SHADING_FAST_MATH)
+    const bool nm = e->nmap_frame;     // normal-mapped shading normals (ST_OPT_NORMAL_MAPS)
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
     auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
@@ -670,7 +674,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     if (d.mode == ST_MODE_REFERENCE) {
         for (uint32_t depth = 0; depth <= (uint32_t)d.ref_depth; depth++) {
             uint32_t sd = seed(P_REF_SHADING_SEED + depth);
-            add(P_REF_TRACING, [=](cudaStream_t s) { launch_ref_tracing(cam, sc, depth, s); });
+            add(P_REF_TRACING, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_ref_tracing(cam, sc, depth, nm, s); });
             add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, sd, depth, s); });
         }
         add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, s); });
@@ -682,7 +686,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     // K4 inside the G-buffer launch: only where nothing has to happen between the two (a strip pulls last frame's rows in between,
     // unless nothing moved: then every reprojected read is the pixel itself)
     const int k4_in_k0 = (e->fused_passes && (ext == nullptr || ext->still) && !e->instances.empty()) ? 1 : 0;
-    add(P_PRIM_GBUFFER, [=](cudaStream_t s) { launch_prim_gbuffer(camG, sc, cur, k4_in_k0, s); });
+    add(P_PRIM_GBUFFER, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_prim_gbuffer(camG, sc, cur, k4_in_k0, nm, s); });
     // ST_OPT_FUSED_PASSES: passes whose hand-over is private to a pixel (or to a checkerboard pair) run as one launch; the step keeps
     // the pass id of the member that gathers from other pixels, which is what the strip plans key on.
     const bool fp = e->fused_passes;
@@ -709,8 +713,8 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
             const int inline_rp = (fp && tracing) ? 1 : 0;   // K11 inside K14; validation frames keep K11 (K12 / K13 read its output)
             if (!inline_rp) add(P_GI_REPROJECTION, [=](cudaStream_t s) { (fs ? stf::launch_gi_reprojection : st::launch_gi_reprojection)(cam, sc, cur, s); });
             auto sampling = [&]() {
-                if (fp) { add(P_GI_SAMPLING_B, [=](cudaStream_t s) { (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, s); }); return; }
-                add(P_GI_SAMPLING_A, [=](cudaStream_t s) { (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, s); });
+                if (fp) { add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, nm, s); }); return; }
+                add(P_GI_SAMPLING_A, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, nm, s); });
                 add(P_GI_SAMPLING_B, [=](cudaStream_t s) { (fs ? stf::launch_gi_sampling_b : st::launch_gi_sampling_b)(cam, sc, cur, sb, f, s); });
             };
             if (tracing) {
@@ -1358,6 +1362,11 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
             g.base_color_texture = rect(mt, 0); g.emissive_texture = rect(mt, 1); g.metallic_roughness_texture = rect(mt, 2); g.normal_map_texture = rect(mt, 3);
             e->h_materials[i] = g;
         }
+        e->any_normal_map = false;
+        for (const GpuMaterial& g : e->h_materials) {
+            const float4 r = g.normal_map_texture;
+            if (r.x != 0.0f || r.y != 0.0f || r.z != 0.0f || r.w != 0.0f) e->any_normal_map = true;
+        }
         if ((rc = upload(e, e->d_materials, e->h_materials.data(), e->h_materials.size() * sizeof(GpuMaterial)))) return rc;
         if ((rc = e->d_matpacked.ensure(e->h_materials.size() * 4))) return rc;
         launch_material_derive((const GpuMaterial*)e->d_materials.p, (uint32_t)e->h_materials.size(), (uint32_t*)e->d_matpacked.p, e->stream);
@@ -1417,6 +1426,7 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
         e->lights_dirty = again;   // commit()/clear_slot() re-dirty the mirror: uploaded on the next tick (mapped_storage_buffer.rs:167-168)
     }
     for (CameraSlot* c : e->cameras) if (c->alive) c->frame = e->frame;   // CameraController::flush (camera_controller.rs:81-85)
+    e->nmap_frame = e->normal_maps && e->any_normal_map;
     e->frame += 1;
     if (too_deep) return fail(ST_ERR_LIMIT, "BVH deeper than the 24-entry traversal stack (strolle-gpu/src/lib.rs:72-76): the scene is not drawn until it changes");
     return ST_OK;
@@ -1588,6 +1598,7 @@ int st_set_option(st_engine* e, int option, int value) {
     if (option == ST_OPT_BVH_REUSE) { e->bvh_reuse = value != 0; return ST_OK; }
     if (option == ST_OPT_FUSE_REPROJECT) { e->fuse_reproject = value != 0; return ST_OK; }
     if (option == ST_OPT_WAVELET_TILE_CFG) { e->wavelet_cfg = value & 0xfffff; return ST_OK; }
+    if (option == ST_OPT_NORMAL_MAPS) { e->normal_maps = value != 0; return ST_OK; }   // takes effect at the next st_tick
     return fail(ST_ERR_INVALID, "unknown option");
 }
 // ---- host-side BVH builder without a device (test / tool hook; strolle/src/bvh/builder.rs, serializer.rs) ----
@@ -1628,6 +1639,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_WAVELET_TILED_LAUNCHES) { *value = e->wavelet_tiled_launches; return ST_OK; }
     if (stat == ST_STAT_VARIANCE_TILED_LAUNCHES) { *value = e->variance_tiled_launches; return ST_OK; }
     if (stat == ST_STAT_BVH_GRAFTED_SUBTREES) { *value = e->bvh.grafted; return ST_OK; }
+    if (stat == ST_STAT_NORMAL_MAP_LAUNCHES) { *value = e->normal_map_launches; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
         CK(cudaSetDevice(e->device)); CK(cudaStreamSynchronize(e->stream));
         uint64_t total = 0;

@@ -152,6 +152,8 @@ template <int ALL, int ONE> struct LbMin { static constexpr int value = ALL > 0 
 // ---------------------------------------------------------------------------------------------
 ST_DEV float4 frame_reprojection_px(const CameraDev& cam, int cur, Px p, float4 surface_texel, float4 vel);
 // `with_reprojection` (ST_OPT_FUSED_PASSES; single GPU, or a strip on a frame where nothing moved): K4 runs in this launch too — its inputs for the pixel are still in registers
+// NMAP (ST_OPT_NORMAL_MAPS, only while some material has a normal map): the shading normal is the mapped one (nmap_normal)
+template <bool NMAP>
 __global__ void ST_LB_PRIM_GBUFFER k_prim_gbuffer(KPARAMS, int cur, int with_reprojection) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
@@ -162,6 +164,7 @@ __global__ void ST_LB_PRIM_GBUFFER k_prim_gbuffer(KPARAMS, int cur, int with_rep
     float4 g0 = f4zero(), g1 = f4zero(), surf = f4zero(), vel = f4zero(), tid = f4(bitsf(0xffffffffu), 0.f, 0.f, 0.f), nd = f4zero();
     if (trihit_some(th)) {
         const GpuMaterial m = sc.materials[th.material_id];
+        if (NMAP) th.normal = nmap_normal(sc, th, m.normal_map_texture);
         GBuf g;
         float2 mr = mat_metallic_roughness(sc, m, th.uv);
         g.base_color = mat_base_color(sc, m, th.uv); g.normal = th.normal; g.metallic = mr.x; g.emissive = mat_emissive(sc, m, th.uv);
@@ -492,6 +495,7 @@ __global__ void __launch_bounds__(ST_BLOCK) k_gi_reprojection(KPARAMS, int cur) 
 // K12 gi_sampling_a::main (gi_sampling_a.rs:4-122)
 // returns false where the kernel leaves without writing its three scratch texels (gi_d0: ray direction + pdf, gi_d1/gi_d2: the packed
 // G-buffer entry of what the ray hit)
+template <bool NMAP>
 ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4* t0, float4* t1, float4* t2) {
     bool tracing = gi_tracing_frame(frame);
     uint2 sp = tracing ? checker(g.x, g.y, frame / 2u) : checker(g.x, g.y, frame);
@@ -517,7 +521,7 @@ ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const T
     if (trihit_some(gh)) {
         GpuMaterial m = sc.materials[gh.material_id];
         m.roughness = rmax(m.roughness, 0.75f * 0.75f);   // Material::regularize (material.rs:25-27)
-        gg.base_color = mat_base_color(sc, m, gh.uv); gg.normal = gh.normal; gg.metallic = m.metallic; gg.emissive = mat_emissive(sc, m, gh.uv);
+        gg.base_color = mat_base_color(sc, m, gh.uv); gg.normal = NMAP ? nmap_normal(sc, gh, m.normal_map_texture) : gh.normal; gg.metallic = m.metallic; gg.emissive = mat_emissive(sc, m, gh.uv);
         gi_color_bits = all_zero(m.base_color_texture) ? __ldg(sc.material_packed + gh.material_id) : gbuf_pack_color(gg.base_color);
         gg.roughness = m.roughness; gg.reflectance = m.reflectance; gg.depth = dist(gi_r.o, gh.point);
     }
@@ -525,12 +529,13 @@ ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const T
     *t0 = f4(gi_r.d, gi_pdf_);
     return true;
 }
+template <bool NMAP>
 __global__ void ST_LB_GI_SAMPLING_A k_gi_sampling_a(KPARAMS, int cur, u32 seed, u32 frame) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
-    if (!gi_sampling_a_pair(cam, sc, stk, cur, seed, frame, g, &t0, &t1, &t2)) return;
+    if (!gi_sampling_a_pair<NMAP>(cam, sc, stk, cur, seed, frame, g, &t0, &t1, &t2)) return;
     size_t gi = pix(cam, g.x, g.y);
     cam.gi_d0[gi] = t0; cam.gi_d1[gi] = t1; cam.gi_d2[gi] = t2;
 }
@@ -602,12 +607,13 @@ __global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, 
 }
 // K12 + K13 in one launch (ST_OPT_FUSED_PASSES): the bounce ray is traced and shaded by the same thread; the hit still goes through
 // GBufferEntry's pack / unpack (its 8-bit quantisation is part of the result), just not through memory.
+template <bool NMAP>
 __global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_fused(KPARAMS, int cur, u32 seed_a, u32 seed_b, u32 frame) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
-    if (!gi_sampling_a_pair(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2)) return;
+    if (!gi_sampling_a_pair<NMAP>(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2)) return;
     gi_sampling_b_pair(cam, sc, stk, cur, seed_b, frame, g, t0, t1, t2);
 }
 
@@ -1244,7 +1250,8 @@ __global__ void __launch_bounds__(ST_BLOCK) k_output_rgba8(KPARAMS, uchar4* __re
     out[i] = make_uchar4((unsigned char)q[0], (unsigned char)q[1], (unsigned char)q[2], 255);
 }
 
-// K1 ref_tracing::main (ref_tracing.rs:4-60)
+// K1 ref_tracing::main (ref_tracing.rs:4-60); NMAP: the packed normal is the mapped one, which K2 shades with and nudges along
+template <bool NMAP>
 __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
@@ -1258,6 +1265,7 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
         ray = ray_make(xyz(d0), xyz(d1));
     }
     TriHit h = trace_closest(ray, sc, stk);
+    if (NMAP && trihit_some(h)) h.normal = nmap_normal(sc, h, ldg4(&sc.materials[h.material_id].normal_map_texture));
     float4 h0, h1; trihit_pack(h, &h0, &h1);
     cam.ref_hits[2 * idx] = h0; cam.ref_hits[2 * idx + 1] = h1;
 }
@@ -1562,7 +1570,9 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_sample, c, st, c, s, seed, frame); }
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_di_resolving<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_gi_reprojection<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_sampling_a, c, st, c, s, cur, seed, frame); }
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, cudaStream_t st) {
+    if (nmap) HALF_LAUNCH(k_gi_sampling_a<true>, c, st, c, s, cur, seed, frame); else HALF_LAUNCH(k_gi_sampling_a<false>, c, st, c, s, cur, seed, frame);
+}
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_sampling_b, c, st, c, s, cur, seed, frame); }
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st) { k_gi_temporal<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, frame, inline_reprojection); }
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_pick, c, st, c, s, cur, seed, frame); }
@@ -1571,12 +1581,16 @@ void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed,
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st) { k_gi_resolving<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, in); }
 void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, cudaStream_t st) { k_di_sample_temporal<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed_sampling, seed_temporal, frame); }
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_sampling_fused, c, st, c, s, cur, seed_a, seed_b, frame); }
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, cudaStream_t st) {
+    if (nmap) HALF_LAUNCH(k_gi_sampling_fused<true>, c, st, c, s, cur, seed_a, seed_b, frame); else HALF_LAUNCH(k_gi_sampling_fused<false>, c, st, c, s, cur, seed_a, seed_b, frame);
+}
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st) { k_gi_preview_resolve<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, in, source); }
 void launch_math_shading(int op, const float* a, const float* b, float* out, long n, cudaStream_t st) { k_math_shading<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n); }
 #if ST_EXACT_ONLY
-void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, cudaStream_t st) { k_prim_gbuffer<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, with_reprojection); }
+void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, cudaStream_t st) {
+    if (nmap) k_prim_gbuffer<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, with_reprojection); else k_prim_gbuffer<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, with_reprojection);
+}
 void launch_frame_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_frame_reprojection<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
 void launch_denoise_reproject(const CameraDev& c, const SceneDev& s, int cur, const float4* pc, const float4* pm, const float4* smp, float4* col, float4* mom, cudaStream_t st) { k_denoise_reproject<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, pc, pm, smp, col, mom); }
 void launch_denoise_reproject_pair(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) {
@@ -1777,7 +1791,9 @@ bool launch_denoise_variance_tiled(const CameraDev& c, const SceneDev& s, int cu
 }
 void launch_composition(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, cudaStream_t st) { k_composition<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, mode, di_diff, gi_diff); }
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st) { k_output_rgba8<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out); }
-void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, cudaStream_t st) { k_ref_tracing<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); }
+void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {
+    if (nmap) k_ref_tracing<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); else k_ref_tracing<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth);
+}
 void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, cudaStream_t st) { k_ref_shading<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth); }
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st) { k_bvh_heatmap<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s); }
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st) { k_trace_stream_closest<<<(unsigned)((n + ST_BLOCK - 1) / ST_BLOCK), ST_BLOCK, 0, st>>>(s, rays, n, out); }

@@ -6,7 +6,8 @@
 namespace st {
 typedef uint32_t u32;
 
-void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, cudaStream_t st);
+// nmap: the NMAP instantiation (normal-mapped shading normal, ST_OPT_NORMAL_MAPS) of the kernels that shade a closest hit
+void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, cudaStream_t st);
 void launch_frame_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
 void launch_di_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, cudaStream_t st);
@@ -15,7 +16,7 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, cudaStream_t st);
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
@@ -24,7 +25,7 @@ void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed,
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st);
 void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, cudaStream_t st);
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, cudaStream_t st);
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, cudaStream_t st);
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st);
 void launch_denoise_reproject(const CameraDev& c, const SceneDev& s, int cur, const float4* pc, const float4* pm, const float4* smp, float4* col, float4* mom, cudaStream_t st);
@@ -35,7 +36,7 @@ bool launch_denoise_wavelet_tiled(const CameraDev& c, const SceneDev& s, u32 fra
 bool launch_denoise_variance_tiled(const CameraDev& c, const SceneDev& s, int cur, bool fast, u32* errors, cudaStream_t st);
 void launch_composition(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, cudaStream_t st);
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st);
-void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, cudaStream_t st);
+void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st);
 void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, cudaStream_t st);
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st);
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st);
@@ -97,7 +98,7 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, cudaStream_t st);
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
@@ -106,7 +107,7 @@ void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed,
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st);
 void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, cudaStream_t st);
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, cudaStream_t st);
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, cudaStream_t st);
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st);
 void launch_math_shading(int op, const float* a, const float* b, float* out, long n, cudaStream_t st);   // test hook: this build's sin/cos/exp/pow/sqrt/div

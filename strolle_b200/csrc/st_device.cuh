@@ -58,7 +58,9 @@ ST_DEV float ray_sphere(const Ray& r, float radius) {   // ray.rs:304-322
     else return -b - sqrtf(discr);
 }
 
-struct TriHit { float t; float3 point, normal; float2 uv; u32 material_id, triangle_id; };
+// bu, bv, inv_det: the Möller–Trumbore barycentrics and 1 / determinant of the closest hit (normal mapping reads them; set by
+// trace_closest only)
+struct TriHit { float t; float3 point, normal; float2 uv; u32 material_id, triangle_id; float bu, bv, inv_det; };
 ST_DEV TriHit trihit_none() { TriHit h; h.t = kF32Max; h.point = f3s(0.f); h.normal = f3s(0.f); h.uv = f2(0.f, 0.f); h.material_id = 0u; h.triangle_id = 0xffffffffu; return h; }
 ST_DEV bool trihit_some(const TriHit& h) { return h.t < kF32Max; }
 ST_DEV void trihit_pack(const TriHit& h, float4* d0, float4* d1) {   // hit.rs:112-120
@@ -116,17 +118,22 @@ ST_DEV void tri_shade(const float4* __restrict__ tri, float u, float v, float in
 // Material::sample_atlas (strolle-gpu/src/material.rs:76-104): repeat-wrap the hit uv, map it into the
 // image's atlas rect, nearest-texel fetch (wgpu default sampler, clamp-to-edge), sRGB decode of r,g,b.
 ST_DEV float wrap_uv(float t) { return (t > 0.0f) ? fmodf(t, 1.0f) : xsub(1.0f, fmodf(-t, 1.0f)); }
-ST_DEV float4 atlas_fetch(const SceneDev& sc, float2 uv) {
-    if (!sc.atlas) return f4zero();
+ST_DEV uchar4 atlas_texel(const SceneDev& sc, float2 uv) {   // the nearest texel's bytes; the caller checks sc.atlas
     int x = to_i32_sat(floorf(xmul(uv.x, (float)kAtlasSize))), y = to_i32_sat(floorf(xmul(uv.y, (float)kAtlasSize)));
     x = max(0, min(x, (int)kAtlasSize - 1)); y = max(0, min(y, (int)kAtlasSize - 1));
-    uchar4 t = __ldg(sc.atlas + (size_t)y * kAtlasSize + (size_t)x);
+    return __ldg(sc.atlas + (size_t)y * kAtlasSize + (size_t)x);
+}
+ST_DEV float2 atlas_uv(float2 hit_uv, float4 texture) {
+    return f2(xadd(texture.x, xmul(wrap_uv(hit_uv.x), texture.z)), xadd(texture.y, xmul(wrap_uv(hit_uv.y), texture.w)));
+}
+ST_DEV float4 atlas_fetch(const SceneDev& sc, float2 uv) {
+    if (!sc.atlas) return f4zero();
+    uchar4 t = atlas_texel(sc, uv);
     return f4(__ldg(sc.srgb_lut + t.x), __ldg(sc.srgb_lut + t.y), __ldg(sc.srgb_lut + t.z), xdiv((float)t.w, 255.0f));
 }
 ST_DEV float4 sample_atlas(const SceneDev& sc, float2 hit_uv, float4 multiplier, float4 texture) {
     if (all_zero(texture)) return multiplier;
-    float2 uv = f2(xadd(texture.x, xmul(wrap_uv(hit_uv.x), texture.z)), xadd(texture.y, xmul(wrap_uv(hit_uv.y), texture.w)));
-    float4 t = atlas_fetch(sc, uv);
+    float4 t = atlas_fetch(sc, atlas_uv(hit_uv, texture));
     return f4(xmul(multiplier.x, t.x), xmul(multiplier.y, t.y), xmul(multiplier.z, t.z), xmul(multiplier.w, t.w));
 }
 ST_DEV float4 mat_base_color(const SceneDev& sc, const GpuMaterial& m, float2 uv) { return sample_atlas(sc, uv, m.base_color, m.base_color_texture); }
@@ -140,6 +147,31 @@ ST_DEV float mat_alpha(const SceneDev& sc, u32 material_id, float2 uv) {
     const float4* m = reinterpret_cast<const float4*>(sc.materials + material_id);
     float4 base = ldg4(m), tex = ldg4(m + 1);
     return sample_atlas(sc, uv, base, tex).w;
+}
+// Normal mapping (ST_OPT_NORMAL_MAPS; DESIGN.md §2 "Normal maps"): the formula the reference keeps commented out in
+// strolle-gpu/src/material.rs:105-140, with Bevy's back-face convention and a fallback to the interpolated normal.
+//   N = tri_shade's normal before its sign flip, T4 = barycentric mix of the baked tangents (not renormalised), B = T4.w (N x T),
+//   Nt = 2 texel / 255 - 1 (linear: a normal map is data, not colour), n' = normalize((Nt.x T + Nt.y B) + Nt.z N),
+//   n' = N where n' is not finite or n'.N <= 0 (meshes without tangents bake NaN tangents), then the sign of inv_det.
+// Explicit round-to-nearest operations only, so that the strict and the fast-shading builds give the same bits.
+// `nmap` is the material's normal_map_texture rect; nothing beyond it is read for materials without a map.
+ST_DEV float3 nmap_normal(const SceneDev& sc, const TriHit& h, float4 nmap) {
+    if (all_zero(nmap) || !sc.atlas) return h.normal;
+    const float s = cpsign(1.0f, h.inv_det);
+    const float3 n = xscale(h.normal, s);   // exact: the factor is +-1
+    const float4* tri = sc.triangles + 9u * (size_t)h.triangle_id;
+    const float4 t0 = ldg4(tri + 2), t1 = ldg4(tri + 5), t2 = ldg4(tri + 8);
+    const float u = h.bu, v = h.bv, w = xsub(xsub(1.0f, u), v);
+    // same evaluation order as tri_shade's normal: (t1 u + t2 v) + t0 (1 - u - v)
+    const float3 t = xadd3(xadd3(xscale(xyz(t1), u), xscale(xyz(t2), v)), xscale(xyz(t0), w));
+    const float tw = xadd(xadd(xmul(t1.w, u), xmul(t2.w, v)), xmul(t0.w, w));
+    const float3 b = xscale(xcross(n, t), tw);
+    const uchar4 c = atlas_texel(sc, atlas_uv(h.uv, nmap));
+    const float nx = xsub(xmul(2.0f, xdiv((float)c.x, 255.0f)), 1.0f), ny = xsub(xmul(2.0f, xdiv((float)c.y, 255.0f)), 1.0f),
+                nz = xsub(xmul(2.0f, xdiv((float)c.z, 255.0f)), 1.0f);
+    const float3 m = xnorm(xadd3(xadd3(xscale(t, nx), xscale(b, ny)), xscale(n, nz)));
+    const bool ok = isfinite(m.x) && isfinite(m.y) && isfinite(m.z) && xdot(m, n) > 0.0f;
+    return xscale(ok ? m : n, s);
 }
 
 // Per-thread traversal stack: a column of a CTA-shared array, stack[level * ST_BLOCK + tid]
@@ -221,6 +253,7 @@ ST_DEV TriHit trace_closest(const Ray& ray, const SceneDev& sc, const TraceStack
     if (trihit_some(hit)) {
         tri_shade(sc.triangles + 9u * (size_t)hit.triangle_id, hu, hv, hid, &hit.normal, &hit.uv);
         hit.point = ray_at(ray, hit.t);
+        hit.bu = hu; hit.bv = hv; hit.inv_det = hid;
     }
     if (COUNT_MEMORY && used_memory) *used_memory = used;
     return hit;

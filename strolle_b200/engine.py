@@ -25,6 +25,7 @@ OPT_WAVELET_PAIRED = 13      # wide-stride a-trous iterations read {DI, GI} as i
 OPT_STRIP_DMA = 12           # strips: gi_reservoirs[1]/[2] halos by copy engine on side streams instead of in-kernel mirror stores
 OPT_STRIP_FUSED = 10         # strips: fused transport (mirror stores, neighbour flags, recompute) instead of push+barrier exchanges
 OPT_SHADING_FAST_MATH = 9  # ReSTIR kernels K5-K19 from the fast-shading build (FMA + SFU approximations; traversal unchanged)
+OPT_NORMAL_MAPS = 14         # shade with the materials' normal maps (off by default: the reference ignores them); from the next tick
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
 STAT_WAVELET_TILED_ERRORS = 2
@@ -33,6 +34,7 @@ STAT_VARIANCE_TILED_LAUNCHES = 4
 STAT_STRIP_PULLED_ROWS = 5
 STAT_LAST_FRAME_FUSED_STRIPS = 6
 STAT_STRIP_FIRST_TIMEOUT = 7
+STAT_NORMAL_MAP_LAUNCHES = 8   # launches of the normal-mapped kernel variants
 
 
 class StrolleError(RuntimeError):

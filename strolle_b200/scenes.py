@@ -283,16 +283,18 @@ def demo_level(width=1920, height=1080, mode=MODE_IMAGE, denoise=True, textures=
                 images=images, material_textures=material_textures)
 
 
-def _quad(p0, p1, p2, p3, normal, uv_lo=(0.0, 0.0), uv_hi=(1.0, 1.0)):
+def _quad(p0, p1, p2, p3, normal, uv_lo=(0.0, 0.0), uv_hi=(1.0, 1.0), tangents=None):
     """Two triangles wound so that the geometric normal agrees with `normal` (Triangle::hit flips the shading normal by
-    the sign of the determinant, strolle-gpu/src/triangle.rs:95-101, i.e. it trusts the winding)."""
+    the sign of the determinant, strolle-gpu/src/triangle.rs:95-101, i.e. it trusts the winding).  `tangents`: one
+    (x, y, z, handedness) for all four corners; None = zero tangents (a mesh without ATTRIBUTE_TANGENT)."""
     (u0, v0), (u1, v1) = uv_lo, uv_hi
     c = [np.asarray(p, np.float64) for p in (p0, p1, p2, p3)]
     uv = [[u0, v0], [u1, v0], [u1, v1], [u0, v1]]
     if np.dot(np.cross(c[1] - c[0], c[2] - c[0]), np.asarray(normal, np.float64)) < 0:
         c = [c[0], c[3], c[2], c[1]]
         uv = [uv[0], uv[3], uv[2], uv[1]]
-    return [tri36([c[0], c[1], c[2]], [normal] * 3, [uv[0], uv[1], uv[2]]), tri36([c[0], c[2], c[3]], [normal] * 3, [uv[0], uv[2], uv[3]])]
+    t = None if tangents is None else [tangents] * 3
+    return [tri36([c[0], c[1], c[2]], [normal] * 3, [uv[0], uv[1], uv[2]], t), tri36([c[0], c[2], c[3]], [normal] * 3, [uv[0], uv[2], uv[3]], t)]
 
 
 def textured_room(width=320, height=180, mode=MODE_IMAGE, denoise=True):
@@ -333,6 +335,101 @@ def textured_room(width=320, height=180, mode=MODE_IMAGE, denoise=True):
     cam = dict(mode=mode, denoise=denoise, ref_depth=1, w=width, h=height, transform=look_at_transform((0.3, 1.2, 4.0), (0.0, 0.9, 0.0)),
                projection=perspective_infinite_reverse_rh(math.pi / 4.0, width / height, 0.1))
     return dict(name="textured_room", meshes=meshes, materials=materials, instances=instances, lights=lights, sun=(1.0, 0.6), camera=cam,
+                images=images, material_textures=material_textures)
+
+
+def brick_normal_map(n=64, rows=4, cols=2, mortar=0.06, bevel=0.05, seed=11):
+    """A brick-wall tangent-space normal map (RGBA8, n x n, linear bytes 255 (t + 1) / 2): bevelled bricks in running bond,
+    flat mortar joints, a little per-brick tilt and grain, and one 6 x 6 patch whose texels point below the surface
+    (t.z < 0), which the shading rule falls back from."""
+    rng = np.random.RandomState(seed)
+    yy, xx = (np.mgrid[0:n, 0:n] + 0.5) / n
+    row = np.floor(yy * rows)
+    xs = xx * cols + 0.5 * (row % 2)
+    fx, fy = xs - np.floor(xs), yy * rows - row
+    brick = (row * 2 * cols + np.floor(xs)).astype(np.int64) % (2 * cols * rows)
+    tilt = rng.uniform(-0.15, 0.15, size=(2 * cols * rows, 2))
+    t = np.zeros((n, n, 3))
+    t[..., 0], t[..., 1] = tilt[brick, 0], tilt[brick, 1]
+    # bevels: the normal leans outwards over the last `bevel` of each brick edge
+    for f, k, s in ((fx, 0, 1.0), (fy, 1, 1.0)):
+        t[..., k] += np.where(f < mortar + bevel, -0.6 * s, 0.0) + np.where(f > 1.0 - bevel, 0.6 * s, 0.0)
+    joint = (fx < mortar) | (fy < mortar)
+    t[..., 0] = np.where(joint, 0.0, t[..., 0]); t[..., 1] = np.where(joint, 0.0, t[..., 1])
+    t[..., :2] += rng.normal(scale=0.04, size=(n, n, 2))
+    t[..., 2] = 1.0
+    t /= np.linalg.norm(t, axis=-1, keepdims=True)
+    t[n // 2:n // 2 + 6, n // 2:n // 2 + 6] = (0.1, -0.2, -0.97)
+    img = np.full((n, n, 4), 255, np.uint8)
+    img[..., :3] = np.clip(np.round((t + 1.0) * 127.5), 0, 255).astype(np.uint8)
+    return img
+
+
+def ripple_normal_map(n=32, waves=3):
+    """Sinusoidal ridges along u (RGBA8 tangent-space normal map)."""
+    u = (np.arange(n) + 0.5) / n
+    sx = 0.5 * np.sin(2 * np.pi * waves * u)
+    t = np.stack(np.broadcast_arrays(sx[None, :], np.zeros((n, 1)), np.ones((n, n))), axis=-1)
+    t /= np.linalg.norm(t, axis=-1, keepdims=True)
+    img = np.full((n, n, 4), 255, np.uint8)
+    img[..., :3] = np.clip(np.round((t + 1.0) * 127.5), 0, 255).astype(np.uint8)
+    return img
+
+
+def _tangent_torus(major=0.5, minor=0.2, nu=32, nv=16, tile=(4.0, 2.0)):
+    """A torus with per-vertex uvs and analytic tangents (dP/du, handedness from dP/dv): the tangent turns along the
+    surface, so the interpolated, not renormalised, tangent of a triangle is shorter than 1."""
+    tris = []
+    def vert(i, j):
+        a, b = 2 * math.pi * i / nu, 2 * math.pi * j / nv
+        ca, sa, cb, sb = math.cos(a), math.sin(a), math.cos(b), math.sin(b)
+        p = np.array([(major + minor * cb) * ca, minor * sb, (major + minor * cb) * sa])
+        n = np.array([cb * ca, sb, cb * sa])
+        t = np.array([-sa, 0.0, ca])
+        dv = np.array([-sb * ca, cb, -sb * sa])
+        w = 1.0 if np.dot(np.cross(n, t), dv) >= 0 else -1.0
+        return p, n, [tile[0] * i / nu, tile[1] * j / nv], list(t) + [w]
+    for i in range(nu):
+        for j in range(nv):
+            v00, v10, v01, v11 = vert(i, j), vert(i + 1, j), vert(i, j + 1), vert(i + 1, j + 1)
+            for a, b, c in ((v00, v01, v11), (v00, v11, v10)):
+                tris.append(tri36([a[0], b[0], c[0]], [a[1], b[1], c[1]], [a[2], b[2], c[2]], [a[3], b[3], c[3]]))
+    return tris
+
+
+def normal_mapped_room(width=224, height=126, mode=MODE_IMAGE, denoise=True, ref_depth=1):
+    """Normal maps (ST_OPT_NORMAL_MAPS): a brick-mapped floor and back wall, a ripple-mapped torus with analytic tangents and
+    a mirrored copy of it (negative determinant: the baked handedness flips), a brick-mapped two-sided panel seen from
+    behind, a brick-mapped box without tangents (NaN tangents: the interpolated normal stays) and an unmapped box.  All
+    dielectric with perceptual roughness >= 0.5, and the sun below the horizon: the fast-shading tier's drift from the strict tier on
+    sunlit direct light (2.7e-3 relative L2 on the textured room's first frame on an H100, maps or not) would blur the 1e-3
+    product-tier check.  Instance 304 (the torus) is the one the tests move."""
+    images = {710: brick_normal_map(), 711: ripple_normal_map()}
+    materials = {
+        100: (material((0.8, 0.7, 0.6, 1.0), perceptual_roughness=0.6), False),      # floor, brick map
+        101: (material((0.7, 0.45, 0.35, 1.0), perceptual_roughness=0.8), False),    # back wall / panel / box without tangents, brick map
+        102: (material((0.5, 0.6, 0.8, 1.0), perceptual_roughness=0.5), False),      # tori, ripple map
+        103: (material((0.6, 0.65, 0.6, 1.0), perceptual_roughness=0.9), False),     # no normal map
+    }
+    material_textures = {100: dict(normal_map=710), 101: dict(normal_map=710), 102: dict(normal_map=711)}
+    meshes = {
+        200: np.stack(_quad((-3, 0, -3), (3, 0, -3), (3, 0, 3), (-3, 0, 3), (0, 1, 0), (0, 0), (3, 3), tangents=(1, 0, 0, -1))),
+        201: np.stack(_quad((-3, 0, -3), (-3, 3, -3), (3, 3, -3), (3, 0, -3), (0, 0, 1), (0, 0), (3, 1.5), tangents=(1, 0, 0, 1))),
+        202: np.stack(_quad((-2.4, 0.2, 0.6), (-1.4, 0.2, 0.6), (-1.4, 1.4, 0.6), (-2.4, 1.4, 0.6), (0, 0, -1), (0, 0), (1, 1), tangents=(-1, 0, 0, 1))),
+        203: np.stack(_box((0.9, 0.0, -1.9), (1.7, 0.8, -1.1))),
+        204: np.stack(_tangent_torus()),
+        205: np.stack(_box((-1.8, 0.0, -2.2), (-1.1, 0.6, -1.5))),
+    }
+    instances = [(300, 200, 100, IDENTITY_AFFINE), (301, 201, 101, IDENTITY_AFFINE), (302, 202, 101, IDENTITY_AFFINE),
+                 (303, 203, 101, IDENTITY_AFFINE),
+                 (304, 204, 102, np.array([1, 0, 0, 0, 0, 1, 0, -1, 0, -0.3, 0.7, -0.6], np.float32)),     # stood up, facing the camera
+                 (305, 204, 102, np.array([-1, 0, 0, 0, 1, 0, 0, 0, 1, 1.6, 0.25, 0.2], np.float32)),     # mirrored in x, lying down
+                 (306, 205, 103, IDENTITY_AFFINE)]
+    lights = [(400, LIGHT_POINT, point_light((0.5, 2.4, 1.5), 0.1, (6.0, 6.0, 6.0), 20.0)),
+              (401, LIGHT_POINT, point_light((-1.5, 1.2, -0.5), 0.1, (2.0, 2.0, 3.0), 20.0))]
+    cam = dict(mode=mode, denoise=denoise, ref_depth=ref_depth, w=width, h=height, transform=look_at_transform((0.4, 1.5, 3.8), (0.0, 0.6, -0.5)),
+               projection=perspective_infinite_reverse_rh(math.pi / 4.0, width / height, 0.1))
+    return dict(name="normal_mapped_room", meshes=meshes, materials=materials, instances=instances, lights=lights, sun=(1.0, -1.0), camera=cam,
                 images=images, material_textures=material_textures)
 
 

@@ -1,0 +1,41 @@
+"""Compare per-kernel SASS of two libstrolle_b200.so builds: every kernel of the old build against the same kernel (for a kernel that
+gained a `bool NMAP` template parameter: its <false> instantiation) of the new one.  Compared: the full instruction text (opcodes,
+registers, immediates, constant-bank operands); normalised: the code-offset comments, branch targets and relocated symbol names."""
+import re, subprocess, sys
+
+def kernels(lib):
+    out = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
+    funcs, name, body = {}, None, []
+    for line in out.splitlines():
+        m = re.match(r"\s+Function : (\S+)", line)
+        if m:
+            if name: funcs[name] = body
+            name, body = m.group(1), []
+            continue
+        if name is None: continue
+        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?);", line)
+        if m:   # the instruction text without its code-offset comment; only branch targets and relocated names are normalised
+            ins = m.group(1)
+            if re.match(r"(@!?U?P\w+\s+)?(BRA|BSSY|CALL|JMP|JMX|BRX|BREAK|SSY|PBK|PCNT|WARPSYNC)\b", ins):
+                ins = re.sub(r"0x[0-9a-f]+", "TARGET", ins)
+            ins = re.sub(r"`\([^)]*\)", "SYM", ins)
+            body.append(ins)
+    if name: funcs[name] = body
+    dem = subprocess.run(["c++filt"], input="\n".join(funcs), capture_output=True, text=True).stdout.split("\n")
+    NM = ("k_prim_gbuffer", "k_gi_sampling_a", "k_gi_sampling_fused", "k_ref_tracing")
+    norm = lambda d: re.sub(r"^void (.*)<false>", r"\1", d) if any("::" + k + "<" in d for k in NM) else d
+    return {norm(d): funcs[m] for d, m in zip(dem, funcs)}, {d for d in dem if "<true>" in d and any("::" + k + "<" in d for k in NM)}
+
+old, _ = kernels(sys.argv[1])
+new, nmap = kernels(sys.argv[2])
+same = diff = 0
+for k, body in sorted(old.items()):
+    if k not in new: print("MISSING in new:", k); diff += 1; continue
+    if new[k] == body: same += 1
+    else:
+        diff += 1; print(f"DIFFERS: {k}: {len(body)} vs {len(new[k])} instructions")
+        if "-v" in sys.argv:
+            import difflib
+            print("\n".join(list(difflib.unified_diff(body, new[k], lineterm="", n=1))[:60]))
+print(f"{same} kernels identical, {diff} differ; {len(old)} kernels in the old build, {len(new)} (+{len(nmap)} NMAP instantiations) in the new")
+for k in sorted(nmap): print("  NMAP:", k)
