@@ -7,6 +7,10 @@ Written from the reference's definitions (paths relative to the reference tree),
                                           radiance, strolle-gpu/src/utils/vec3_ext.rs:56-58; `BlueNoise` strolle-gpu/src/noise/blue.rs
   * `Light::ray_bnoise`                   strolle-gpu/src/light.rs:217-239; glam 0.24 `any_orthonormal_pair` (Duff et al. 2017)
   * K6  `di_temporal_resampling::main`    strolle-shaders/src/di_temporal_resampling.rs:4-112
+  * K7  `di_spatial_resampling::pick`     strolle-shaders/src/di_spatial_resampling.rs:4-147; `resolve_checkerboard_alt` strolle-gpu/src/utils.rs:37;
+                                          `WhiteNoise::sample_disk` strolle-gpu/src/noise/white.rs:52-56; `Camera::contain`
+                                          strolle-gpu/src/camera.rs:57-77; `DiSample::ray` strolle-gpu/src/reservoir/di.rs:119-123;
+                                          `Normal::encode` strolle-gpu/src/normal.rs:9-23
   * K8  `di_spatial_resampling::trace`    strolle-shaders/src/di_spatial_resampling.rs:150-209
   * `Mis::di_temporal`                    strolle-gpu/src/reservoir/mis.rs:36-65
   * `DiSample::pdf` / `pdf_prev` / `pdf_ex`   strolle-gpu/src/reservoir/di.rs:95-117; `Light::contains` / slots / `rollback`
@@ -286,10 +290,12 @@ def ndc_to_world(transform16, projection16):
     return _hm_mul(t, _hm_inverse(p))
 
 
-def camera_ray(n2w, w, h, fast):
-    """Camera::ray for every pixel: (origin, dir) as Num (H, W, 3)."""
+def camera_ray(n2w, w, h, fast, xs=None, ys=None):
+    """Camera::ray for every pixel, or for the pixels (xs, ys): (origin, dir) as Num (H, W, 3) or (N, 3)."""
     m = np.asarray(n2w, np.float64).reshape(4, 4)          # m[c] = column c
-    ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+    if xs is None:
+        ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+    xs, ys = np.asarray(xs, np.float64), np.asarray(ys, np.float64)
     z = lambda a: Num(a, 0.0, fast)
     nx = (z(xs + 0.5) * 2.0) / float(w) - 1.0
     ny = -((z(ys + 0.5) * 2.0) / float(h) - 1.0)
@@ -297,7 +303,7 @@ def camera_ray(n2w, w, h, fast):
     def project(zc):
         r = [z(m[0][k]) * nx for k in range(4)]
         r = [r[k] + z(m[1][k]) * ny for k in range(4)]
-        r = [r[k] + z(np.full((h, w), m[2][k])) * zc for k in range(4)]
+        r = [r[k] + z(np.full(xs.shape, m[2][k])) * zc for k in range(4)]
         r = [r[k] + m[3][k] for k in range(4)]
         rw = 1.0 / r[3]
         return stack3(r[0] * rw, r[1] * rw, r[2] * rw)
@@ -336,9 +342,11 @@ def gbuffer(d0, d1, fast):
                 metallic_byte=mb, some=d0[..., 0] != 0)
 
 
-def hit(n2w, w, h, d0, d1, fast):
-    """Hit::new(camera.ray(pos), gbuffer): point = origin + dir * (depth - 0.01)."""
-    o, d = camera_ray(n2w, w, h, fast)
+def hit(n2w, w, h, d0, d1, fast, xs=None, ys=None):
+    """Hit::new(camera.ray(pos), gbuffer): point = origin + dir * (depth - 0.01), for every pixel or for the pixels (xs, ys)."""
+    o, d = camera_ray(n2w, w, h, fast, xs, ys)
+    if xs is not None:
+        d0, d1 = np.asarray(d0, np.float32)[ys, xs], np.asarray(d1, np.float32)[ys, xs]
     g = gbuffer(d0, d1, fast)
     t = Num(g["depth"], 0.0, fast) - _f32c(0.01)
     return dict(g=g, origin=o, dir=d, point=o + d * t.x3())
@@ -499,38 +507,58 @@ def _mis_eval(lm, rm, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, rpdf):
     return rm * mmin, lhs_mis, rhs_mis
 
 
-def di_spatial_sample(res_in, stash, seed, frame, w, h, fast):
-    """K9 on every checkerboard pair.  Returns dict(idx (P,), cands: list of dicts of expected (P, 8) words + bound on m / w, per-pair
-    `allowed` mask per candidate; decided (P,) bool; copies (Q,) indices of the pass-through pixels)."""
-    res_in = np.asarray(res_in, np.float32).reshape(-1, 8)
-    npx = w * h
-    stash = np.asarray(stash, np.float32).reshape(h, w, 4)
+def half_grid_pairs(w, h, frame, rows=None):
+    """The half-width dispatch grid of K7 / K9 (8 * ((ceil(w / 8)) / 2) columns, so with w = 67 the last columns are never reached):
+    (gx, gy, lhs x, other x) per pair, resolve_checkerboard_alt / resolve_checkerboard (utils.rs:33-39).  `rows`: only those rows."""
     hw = 8 * (((w + 7) // 8) // 2)
     gy, gx = np.mgrid[0:h, 0:hw]
     gx, gy = gx.reshape(-1), gy.reshape(-1)
+    if rows is not None:
+        keep = np.isin(gy, rows)
+        gx, gy = gx[keep], gy[keep]
     f2 = frame // 2
-    lx = gx * 2 + ((f2 + 1 + gy) % 2)
-    ox = gx * 2 + ((f2 + gy) % 2)
+    return gx, gy, gx * 2 + ((f2 + 1 + gy) % 2), gx * 2 + ((f2 + gy) % 2)
+
+
+def di_spatial_sample(res_in, stash, seed, frame, w, h, fast, rows=None, flips=0):
+    """K9 on every checkerboard pair (or those of `rows`).  `stash`: the (H, W, 4) visibility texels K8 left; or, for the fused
+    launch, K7's restatement composed with a visibility per ray (pick_stash), whose pdfs carry bounds and whose undecided pairs are
+    skipped.  `flips` is recorded in the candidates (how many visibility bits were flipped to build them).  Returns dict(idx (P,),
+    cands: list of dicts of expected (P, 8) words + bound on m / w / pdf, per-pair `allowed` mask per candidate; undecided, skip (P,)
+    bool; copies (Q,) indices of the pass-through pixels)."""
+    res_in = np.asarray(res_in, np.float32).reshape(-1, 8)
+    npx = w * h
+    gx, gy, lx, ox = half_grid_pairs(w, h, frame, rows)
     ok = lx < w
-    copies = (gy * w + ox)[(ox < w)]
+    # the other pixel of the pair is copied through only where the lhs is on the screen: the pass returns before the copy otherwise
+    # (di_spatial_resampling.rs:230)
+    copies = (gy * w + ox)[ok & (ox < w)]
     gx, gy, lx = gx[ok], gy[ok], lx[ok]
     lidx = gy * w + lx
-    ax, bx = gx * 2, gx * 2 + 1
-    tz = np.zeros((len(gx), 4), np.float32)
-    d0 = np.where((ax < w)[:, None], stash[gy, np.minimum(ax, w - 1)], tz)
-    d1 = np.where((bx < w)[:, None], stash[gy, np.minimum(bx, w - 1)], tz)
-    rhs_idx = d0[:, 1].view(np.uint32).astype(np.int64)
+    z = lambda a: Num(np.asarray(a, np.float64), 0.0, fast)
+    if isinstance(stash, dict):
+        rhs_idx, skip = stash["rhs_idx"][ok], stash["skip"][ok]
+        lhs_rhs_vis, rhs_lhs_vis = stash["vis_a"][ok].astype(np.float64), stash["vis_b"][ok].astype(np.float64)
+        pdf_lr, pdf_rl = stash["lhs_rhs_pdf"][ok], stash["rhs_lhs_pdf"][ok]
+    else:
+        stash = np.asarray(stash, np.float32).reshape(h, w, 4)
+        ax, bx = gx * 2, gx * 2 + 1
+        tz = np.zeros((len(gx), 4), np.float32)
+        d0 = np.where((ax < w)[:, None], stash[gy, np.minimum(ax, w - 1)], tz)
+        d1 = np.where((bx < w)[:, None], stash[gy, np.minimum(bx, w - 1)], tz)
+        rhs_idx, skip = d0[:, 1].view(np.uint32).astype(np.int64), np.zeros(len(gx), bool)
+        lhs_rhs_vis, rhs_lhs_vis = d0[:, 0].astype(np.float64), d1[:, 0].astype(np.float64)
+        pdf_lr, pdf_rl = z(d1[:, 1]), z(d1[:, 2])
     # K7 writes 0 (no neighbour) or screen index + 1; anything past the frame would make K9 read outside the reservoirs
     assert not ((rhs_idx > 0) & (rhs_idx - 1 >= npx)).any(), "K7 scratch texel holds a neighbour index outside the frame"
     merge = rhs_idx > 0
     lhs = res_in[lidx]
     rhs = res_in[np.where(merge, rhs_idx - 1, 0)]
-    z = lambda a: Num(np.asarray(a, np.float64), 0.0, fast)
     lm, lw, lpdf = z(lhs[:, 0]), z(lhs[:, 1]), z(lhs[:, 2])
     rm, rw, rpdf = z(rhs[:, 0]), z(rhs[:, 1]), z(rhs[:, 2])
-    lhs_rhs_vis, rhs_lhs_vis = d0[:, 0].astype(np.float64), d1[:, 0].astype(np.float64)
-    lhs_rhs_pdf = z(d1[:, 1]) * lhs_rhs_vis
-    rhs_lhs_pdf = z(d1[:, 2]) * rhs_lhs_vis
+    # pdf * vis with vis 0 or 1 (K8's texel layout) is exact
+    lhs_rhs_pdf = where(lhs_rhs_vis != 0, pdf_lr, z(np.zeros(len(gx))))
+    rhs_lhs_pdf = where(rhs_lhs_vis != 0, pdf_rl, z(np.zeros(len(gx))))
     with np.errstate(invalid="ignore", over="ignore"):
         mis_m, lhs_mis, rhs_mis = _mis_eval(lm, rm, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, rpdf)
         wl = (lhs_mis * lpdf) * lw
@@ -548,21 +576,22 @@ def di_spatial_sample(res_in, stash, seed, frame, w, h, fast):
             allowed = merge & np.where(dec1, acc1 == a1, True) & np.where(dec2, acc2 == a2, True)
             out = np.zeros((len(gx), 8), np.float32)
             src = rhs if a2 else (lhs if a1 else np.zeros_like(lhs))
-            pdf = (rhs_lhs_pdf.v if a2 else (lpdf.v if a1 else np.zeros(len(gx)))).astype(np.float32)
+            pdf = rhs_lhs_pdf if a2 else (lpdf if a1 else z(np.zeros(len(gx))))
             occ = (lhs_rhs_vis == 0) if a2 else ((src[:, 3].view(np.uint32) & 0xFF) > 0)
             conf = (src[:, 3].view(np.uint32) >> 8) & 0xFF
             with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
-                wn = W2 / Num(pdf.astype(np.float64), 0.0, fast)
-            wv = np.where(pdf == 0, 0.0, wn.v)
-            we = np.where(pdf == 0, 0.0, wn.e)
-            out[:, 2] = pdf
+                wn = W2 / pdf
+            # a pdf is either an exact zero or certainly nonzero (K7 decides `pdf > 0` before it builds a ray)
+            wv = np.where(pdf.v == 0, 0.0, wn.v)
+            we = np.where(pdf.v == 0, 0.0, wn.e)
+            out[:, 2] = pdf.v.astype(np.float32)
             out[:, 3] = (occ.astype(np.uint32) | (conf.astype(np.uint32) << 8)).view(np.float32)
             out[:, 4:8] = src[:, 4:8]
-            cands.append(dict(allowed=allowed, words=out, m=m_out.v, m_e=m_out.e, w=wv, w_e=we))
+            cands.append(dict(allowed=allowed, words=out, m=m_out.v, m_e=m_out.e, w=wv, w_e=we, pdf=pdf.v, pdf_e=pdf.e, flips=flips))
     # no merge: the lhs reservoir goes through as it is
     cands.append(dict(allowed=~merge, words=lhs.copy(), m=lhs[:, 0].astype(np.float64), m_e=np.zeros(len(gx)),
-                      w=lhs[:, 1].astype(np.float64), w_e=np.zeros(len(gx))))
-    return dict(idx=lidx, cands=cands, undecided=merge & ~(dec1 & dec2), merge=merge, copies=copies)
+                      w=lhs[:, 1].astype(np.float64), w_e=np.zeros(len(gx)), flips=flips))
+    return dict(idx=lidx, cands=cands, undecided=merge & ~(dec1 & dec2) & ~skip, skip=skip, merge=merge, copies=copies)
 
 
 # ---- K6: temporal resampling -------------------------------------------------------------------------------------------------
@@ -593,7 +622,7 @@ def di_pdf(L, ht, point):
     diff = (1.0 - g["metallic"]) / PI
     s = lr["radiance"] * (diff.x3() + lr["spec"])
     luma = (s.col(0) * LUMA[0] + s.col(1) * LUMA[1]) + s.col(2) * LUMA[2]
-    p = np.asarray(point, np.float32).astype(np.float64)
+    p = point if isinstance(point, Num) else np.asarray(point, np.float32).astype(np.float64)    # a Num: a bounded light point
     c = Num(L[:, 0:3].astype(np.float64), 0.0, fast) - p
     dist = dot3(c, c).sqrt()
     radius = L[:, 3].astype(np.float64)
@@ -610,10 +639,12 @@ def _round_u(x):
     return np.clip(np.nan_to_num(r, nan=0.0), 0, 2.0 ** 32 - 1).astype(np.int64)
 
 
-def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_prev, seed, fast):
+def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_prev, seed, fast, lhs=None, flips=0):
     """K6 di_temporal_resampling::main (di_temporal_resampling.rs:4-112) for every pixel with a surface.  gb / gb_prev: this and the
     previous frame's G-buffer (d0, d1); reproj: the reprojection map (Reprojection::deserialize, reprojection.rs:22-29); res_cur: what
-    K5 left in di_reservoirs[1]; res_prev: di_reservoirs[0].
+    K5 left in di_reservoirs[1]; res_prev: di_reservoirs[0].  For the fused K5 + K6 launch `lhs` replaces res_cur: K5's sample as
+    sampling_lhs restates it, with a bounded w and light point; its skipped pixels are not compared.  `flips` is recorded in the
+    candidates (1 where the lhs occluded bit was flipped).
       * lhs: K5's sample, its pdf recomputed with the current light (:47-51).
       * rhs: di_reservoirs[0] at prev_pos().round().as_uvec2() (reprojection.rs:46-48), M clamped to 64 (reservoir.rs:55-57), a killed
         slot zeroes w, a remapped one moves the id to slot - 1 (light.rs:107-129); its hit is rebuilt with the *previous* camera from
@@ -633,12 +664,19 @@ def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_p
     n = len(idx)
     zero = z(np.zeros(n))
     lh = _take(ht, idx)
-    cur, prv = di_fields(res_cur), di_fields(res_prev)
-    lm, lw, lid, lpoint = cur["m"][idx], cur["w"][idx], cur["id"][idx].astype(np.int64), cur["point"][idx]
+    prv = di_fields(res_prev)
+    if lhs is None:
+        cur = di_fields(res_cur)
+        lm, lw, lid, lpoint = cur["m"][idx], z(cur["w"][idx]), cur["id"][idx].astype(np.int64), cur["point"][idx]
+        locc, lpdf0, lskip = cur["occ"][idx], cur["pdf"][idx], np.zeros(n, bool)
+    else:
+        assert len(lhs["id"]) == n
+        lm, lid, lpoint, locc, lpdf0, lskip = lhs["m"], lhs["id"], lhs["point"], lhs["occ"], lhs["pdf"], lhs["skip"]
+        lw = where(locc, z(np.zeros(n)), lhs["w"])      # K5: w is exactly 0 where the shadow ray is occluded
     assert (lid[lm != 0] < nl).all(), "K6 lhs light id outside the light table"
     lid_c = np.minimum(lid, nl - 1)
     lp, und_c1, und_s1 = di_pdf(lights[lid_c], lh, lpoint)
-    lpdf = where(lm != 0, lp, z(cur["pdf"][idx]))
+    lpdf = where(lm != 0, lp, z(lpdf0))
     rp = np.asarray(reproj, f32).reshape(-1, 4)[idx]
     has_rp = rp[:, 2] > 0
     rx, ry = _round_u(rp[:, 0]), _round_u(rp[:, 1])
@@ -671,7 +709,8 @@ def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_p
     rhs_lhs_pdf = where(use_rl, rlp, zero)
     und = {"contains": (und_c1 & (lm != 0)) | (und_c2 & use_lr) | (und_c3 & use_rl),
            "specular": (und_s1 & (lm != 0)) | (und_s2 & use_lr) | (und_s3 & use_rl)}
-    skip = und["contains"] | und["specular"]
+    und["K5"] = lskip
+    skip = und["contains"] | und["specular"] | lskip
     with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
         lmN, rmN = z(lm), z(rm)
         mis_m, lhs_mis, rhs_mis = _mis_eval(lmN, rmN, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, z(rpdf))
@@ -682,7 +721,7 @@ def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_p
         # a recomputed pdf without a finite bound (GGX at minimum roughness on a normal along the view: the (n.h a^2 - n.h) n.h + 1
         # cancellation) leaves the pixel's m and w unbounded: counted
         und["unbounded"] = ~np.isfinite(m_e) | ~np.isfinite(lpdf.e) | ~np.isfinite(lhs_rhs_pdf.e) | ~np.isfinite(rhs_lhs_pdf.e)
-        wl = (lhs_mis * lpdf) * z(lw)
+        wl = (lhs_mis * lpdf) * lw
         wr = (rhs_mis * rhs_lhs_pdf) * z(rw)
         rng = WhiteNoise(seed, idx % w, idx // w)
         r1, r2 = rng.sample(), rng.sample()
@@ -699,7 +738,7 @@ def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_p
             if a2:
                 pdf, occ, point, lid_o = rhs_lhs_pdf, rocc, rpoint, rid
             elif a1:
-                pdf, occ, point, lid_o = lpdf, cur["occ"][idx], lpoint, lid
+                pdf, occ, point, lid_o = lpdf, locc, lpoint, lid
             else:
                 pdf, occ, point, lid_o = zero, np.zeros(n, bool), np.zeros((n, 3), f32), np.zeros(n, np.int64)
             with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
@@ -708,9 +747,12 @@ def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_p
             firm = pdf.v > pdf.e        # the f32 pdf is certainly nonzero
             out = np.zeros((n, 8), f32)
             out[:, 3] = (occ.astype(np.uint32) | (conf << 8)).view(f32)
-            out[:, 4:7] = point
+            point_e = point.e if isinstance(point, Num) else np.zeros((n, 3))
+            out[:, 4:7] = point.v if isinstance(point, Num) else point
             out[:, 7] = lid_o.astype(np.uint32).view(f32)
             cands.append(dict(allowed=allowed, words=out, m=m_out.v, m_e=m_e, pdf=pdf.v, pdf_e=pdf.e,
+                              point=point.v if isinstance(point, Num) else out[:, 4:7].astype(np.float64),
+                              point_e=point_e, flips=flips,
                               w=np.where(exact0 | ~firm, 0.0, wn.v), w_e=np.where(exact0, 0.0, np.where(firm, wn.e, np.inf))))
     return dict(idx=idx, cands=cands, undecided=und, skip=skip, surf=ht["g"]["some"].reshape(-1), killed=int(killed.sum()),
                 remapped=int(remap.sum()), reprojected=int(read.sum()))
@@ -718,8 +760,9 @@ def di_temporal(n2w, n2w_prev, w, h, gb, gb_prev, reproj, lights, res_cur, res_p
 
 def check_temporal(got, res_before, r, what):
     """K6's reservoirs: at every surface pixel without an undecided pdf, one admissible outcome with the discrete words (occluded,
-    confidence, light point, light id) bit for bit and m, w, pdf within their bounds; every other pixel untouched.  Returns (largest
-    error / bound ratio, undecided counts per decision type, pixels checked)."""
+    confidence, light id, and the light point where it is exact) bit for bit and m, w, pdf (and a bounded light point) within their
+    bounds; every other pixel untouched.  Returns (largest error / bound ratio, undecided counts per decision type, pixels checked,
+    pixels matched only by a candidate with a flipped lhs occluded bit)."""
     got = np.asarray(got, np.float32).reshape(-1, 8)
     before = np.asarray(res_before, np.float32).reshape(-1, 8)
     assert (got[~r["surf"]].view(np.uint32) == before[~r["surf"]].view(np.uint32)).all(), f"{what}: K6 wrote a sky pixel"
@@ -728,17 +771,24 @@ def check_temporal(got, res_before, r, what):
     ok = r["skip"].copy()
     best = np.zeros(len(g))
     found = np.zeros(len(g), bool)
+    flips = np.full(len(g), np.inf)
     for c in r["cands"]:
-        disc = (gb[:, 3:8] == c["words"].view(np.uint32)[:, 3:8]).all(1)
+        wb = c["words"].view(np.uint32)
+        disc = (gb[:, 3] == wb[:, 3]) & (gb[:, 7] == wb[:, 7])
         rat = []
         with np.errstate(invalid="ignore", divide="ignore"):
             for k, key in ((0, "m"), (1, "w"), (2, "pdf")):
                 err = np.abs(g[:, k].astype(np.float64) - c[key])
                 rk = np.where(err == 0, 0.0, err / c[key + "_e"])
                 rat.append(np.where(np.isnan(rk), np.inf, rk))
-        ratio = np.maximum(np.maximum(rat[0], rat[1]), rat[2])
+            err = np.abs(g[:, 4:7].astype(np.float64) - c["point"])
+            rk = np.where(err == 0, 0.0, err / c["point_e"])
+            rk = np.where(c["point_e"] == 0, np.where(gb[:, 4:7] == wb[:, 4:7], 0.0, np.inf), np.where(np.isnan(rk), np.inf, rk))
+            rat.append(rk.max(1))
+        ratio = np.maximum(np.maximum(rat[0], rat[1]), np.maximum(rat[2], rat[3]))
         good = c["allowed"] & disc & (ratio <= 1.0) & ~r["skip"]
         best = np.where(good & ~found, ratio, np.where(good, np.minimum(best, ratio), best))
+        flips = np.where(good, np.minimum(flips, c["flips"]), flips)
         found |= good
         ok |= good
     if not ok.all():
@@ -746,7 +796,35 @@ def check_temporal(got, res_before, r, what):
         raise AssertionError(f"{what}: {int((~ok).sum())}/{len(ok)} pixels match no admissible outcome; first pixels {r['idx'][i].tolist()}: "
                              f"got {g[i].tolist()}")
     und = {k: int(v.sum()) for k, v in r["undecided"].items()}
-    return float(best.max()) if len(best) else 0.0, und, len(g)
+    return float(best.max()) if len(best) else 0.0, und, len(g), int((np.isfinite(flips) & (flips > 0)).sum())
+
+
+def merge_temporal(rs):
+    """One K6 restatement whose candidates are those of all of `rs` (the same pixels under different lhs occluded bits)."""
+    return dict(rs[0], cands=[c for r in rs for c in r["cands"]], skip=np.logical_or.reduce([r["skip"] for r in rs]),
+                undecided={k: np.logical_or.reduce([r["undecided"][k] for r in rs]) for k in rs[0]["undecided"]})
+
+
+def sampling_lhs(r, sin, cos, trace_any):
+    """K5's sample of every surface pixel as k_di_sample_temporal hands it to K6 in registers (di_sampling_px): m 1, pdf 0, the
+    light id and w (Num) of the decided selection of `r` (di_sampling), the light point (Num) of Light::ray_bnoise under the decided
+    sign of any_orthonormal_pair, and the occluded bit of `trace_any` on the shadow ray rebuilt in strict f32.  Pixels whose selection
+    or sign is undecided are marked `skip`."""
+    n = len(r["idx"])
+    skip = r["undecided"].copy()
+    lid, w, we = np.zeros(n, np.int64), np.zeros(n), np.zeros(n)
+    for c in r["cands"]:
+        sel = c["allowed"] & ~skip      # exactly one candidate where the selection is decided
+        lid, w, we = np.where(sel, c["id"], lid), np.where(sel, c["w"], w), np.where(sel, c["w_e"], we)
+    L = r["lights"][lid]
+    p = r["hit"]["point"]
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        lz = norm3(Num(L[:, 0:3].astype(np.float64), 0.0, p.fast) - p).col(2)
+        skip |= ~(np.abs(lz.v) > lz.e)
+        point, _ = ray_bnoise(L, p, r["bn"], np.where(lz.v >= 0, 1.0, -1.0))
+    pt = hit_point_f32(r["n2w"], r["w"], r["h"], _depth_image(r)).reshape(-1, 3)[r["idx"]]
+    occ = np.asarray(trace_any(ray_bnoise_f32(L, pt, r["bn"], sin, cos)), np.uint32) != 0
+    return dict(m=np.ones(n), w=Num(w, we, p.fast), pdf=np.zeros(n), occ=occ, point=point, id=lid, skip=skip)
 
 
 def temporal_tight(r):
@@ -1054,31 +1132,337 @@ def _depth_image(r):
     return d.reshape(r["h"], r["w"])
 
 
+# ---- K7: DI spatial tap choice -------------------------------------------------------------------------------------------------
+
+K7_BRANCHES = ("self tap", "sky or outside", "depth", "normal", "radius floor", "exhausted", "empty neighbour")
+K7_UNDECIDED = ("truncation", "depth", "normal", "pdf", "fold")
+
+
+def _trunc_decided(x):
+    """as_ivec2 truncates toward zero: decided where trunc is the same over [v - e, v + e] (its steps are at the nonzero integers)."""
+    with np.errstate(invalid="ignore"):
+        return np.trunc(x.v - x.e) == np.trunc(x.v + x.e)
+
+
+def _contain(x, w):
+    """Camera::contain (camera.rs:57-77) on one coordinate: mirror below 0, then above the screen.  On screens smaller than the tap
+    radius the result can be negative; cast to u32 it lies outside the frame."""
+    x = np.where(x < 0, -x, x)
+    return np.where(x >= w, w - x + w - 1, x)
+
+
+def oct_encode(n):
+    """Normal::encode (normal.rs:9-23) of a Num direction (N, 3): (encoded Num (N, 2), decided).  The fold (n.z >= 0) and, below
+    the equator, the copysign of x and y are decisions, decided where the value is farther from 0 than its bound."""
+    s = (n.col(0).abs() + n.col(1).abs()) + n.col(2).abs()
+    q = n / s.x3()
+    x, y, zc = q.col(0), q.col(1), q.col(2)
+    up = zc.v >= 0
+    dec = np.abs(zc.v) > zc.e
+    dec &= up | ((np.abs(x.v) > x.e) & (np.abs(y.v) > y.e))
+    tx, ty = 1.0 - y.abs(), 1.0 - x.abs()
+    ex = where(up, x, Num(np.copysign(tx.v, x.v), tx.e, n.fast)) * 0.5 + 0.5
+    ey = where(up, y, Num(np.copysign(ty.v, y.v), ty.e, n.fast)) * 0.5 + 0.5
+    return Num(np.stack([ex.v, ey.v], -1), np.stack([ex.e, ey.e], -1), n.fast), dec
+
+
+def di_spatial_pick(n2w, w, h, d0, d1, lights, res, seed, frame, fast, rows=None):
+    """K7 di_spatial_resampling::pick (di_spatial_resampling.rs:4-147) on every pair of the half-width grid (or those of `rows`).
+      * lhs = resolve_checkerboard_alt(id, frame / 2) (utils.rs:37-39); off the screen: nothing is written (state 0); a sky lhs: the
+        two d1 texels are cleared (state 1; the reference leaves them stale, C-15).
+      * 8 tries: WhiteNoise::sample_disk (noise/white.rs:44-56: radius = sqrt(sample) first, then the angle sample * PI * 2, (cos, sin)
+        * radius) times max_radius, plus the lhs position; as_ivec2 truncates toward zero before Camera::contain mirrors.  A tap on the
+        lhs itself uses up its try.  A tap outside the frame reads zero and, like the sky, a depth off by more than 0.33 of the lhs
+        depth or a normal dot below 0.33 (both from GBufferEntry::unpack of the neighbour's texels), is rejected and halves
+        max_radius with a floor of 5; an accepted neighbour with an empty reservoir (M = 0) does not halve it.
+      * found: lhs_rhs_pdf = lhs.pdf(rhs_hit), rhs_lhs_pdf = rhs.pdf(lhs_hit) (DiSample::pdf, di.rs:95-117); a ray where the pdf is
+        > 0 (DiSample::ray, di.rs:119-123: origin the light point, dir = normalize(hit - light point), len = |hit - light point|),
+        else the zero ray (origin 0, len 0, Normal::encode(0) = NaN).  Texel a = (ray_a origin, len), (encode(dir_a), rhs_idx + 1, 0);
+        texel b = (ray_b origin, len), (encode(dir_b), lhs_rhs_pdf, rhs_lhs_pdf) (state 2); no neighbour: d1 texels cleared (state 1).
+    Every decision (truncation, the depth and normal tests, pdf > 0, the fold signs) is decided only where its margin exceeds its
+    bound; a pair with an undecided one is counted and skipped.  Returns dict(pairs (gx, gy, lx), state (P,), undecided (P,),
+    und (counts per decision), branches (counts per K7_BRANCHES), and for the found pairs: found (P,) mask and per-found-pair rhs_idx,
+    lhs / rhs light point, len_a / len_b / enc_a / enc_b (Num), zero_a / zero_b, lhs_rhs_pdf / rhs_lhs_pdf (Num))."""
+    d0 = np.asarray(d0, np.float32).reshape(h, w, 4)
+    d1 = np.asarray(d1, np.float32).reshape(h, w, 4)
+    lights = np.asarray(lights, np.float32).reshape(-1, 28)
+    nl = len(lights)
+    rf = di_fields(res)
+    gx, gy, lx, _ = half_grid_pairs(w, h, frame, rows)
+    npair = len(gx)
+    state = np.zeros(npair, np.int64)
+    on = lx < w
+    depth = d0[..., 0]
+    surf = on & (depth[gy, np.minimum(lx, w - 1)] != 0)
+    state[on] = 1
+    und = np.zeros(npair, bool)
+    und_n = dict.fromkeys(K7_UNDECIDED, 0)
+    br = dict.fromkeys(K7_BRANCHES, 0)
+    P = np.flatnonzero(surf)
+    n = len(P)
+    px, py = lx[P], gy[P]
+    z = lambda a: Num(np.asarray(a, np.float64), 0.0, fast)
+    dl = z(depth[py, px])
+    nrm_l = oct_decode(d0[py, px, 1:3], fast)
+    rng = WhiteNoise(seed, px, py)
+    radius = np.full(n, 128.0)
+    active = np.ones(n, bool)
+    u = np.zeros(n, bool)
+    found = np.zeros(n, bool)
+    floor = np.zeros(n, bool)
+    rx, ry = np.zeros(n, np.int64), np.zeros(n, np.int64)
+    thr = _f32c(0.33)
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        for _ in range(8):
+            r = z(rng.sample()).sqrt()
+            ang = (z(rng.sample()) * PI) * 2.0
+            sa, ca = sincos(ang)
+            fx = (ca * r) * radius + px.astype(np.float64)
+            fy = (sa * r) * radius + py.astype(np.float64)
+            dec = _trunc_decided(fx) & _trunc_decided(fy)
+            und_n["truncation"] += int((active & ~dec).sum())
+            u |= active & ~dec
+            active &= dec
+            tx = _contain(np.trunc(fx.v).astype(np.int64), w)
+            ty = _contain(np.trunc(fy.v).astype(np.int64), h)
+            self_ = active & (tx == px) & (ty == py)
+            br["self tap"] += int(self_.sum())
+            live = active & ~self_
+            inside = (tx >= 0) & (ty >= 0) & (tx < w) & (ty < h)
+            cx, cy = np.clip(tx, 0, w - 1), np.clip(ty, 0, h - 1)
+            dr = np.where(inside, depth[cy, cx], 0.0)
+            rej_sky = live & (dr == 0)
+            live &= ~rej_sky
+            diff = (z(dr) - dl).abs()
+            lim = dl * thr
+            margin, bound = diff.v - lim.v, diff.e + lim.e
+            dec = (np.abs(margin) > bound) | (bound == 0)
+            und_n["depth"] += int((live & ~dec).sum())
+            u |= live & ~dec
+            live &= dec
+            rej_depth = live & (margin > 0)
+            live &= ~rej_depth
+            dt = dot3(oct_decode(d0[cy, cx, 1:3], fast), nrm_l)
+            margin, bound = dt.v - thr, dt.e
+            dec = (np.abs(margin) > bound) | (bound == 0)
+            und_n["normal"] += int((live & ~dec).sum())
+            u |= live & ~dec
+            live &= dec
+            rej_normal = live & (margin < 0)
+            live &= ~rej_normal
+            br["sky or outside"] += int(rej_sky.sum()); br["depth"] += int(rej_depth.sum()); br["normal"] += int(rej_normal.sum())
+            rej = rej_sky | rej_depth | rej_normal
+            radius = np.where(rej, np.maximum(radius * 0.5, 5.0), radius)
+            floor |= rej & (radius == 5.0)
+            nonempty = rf["m"][np.where(live, cy * w + cx, 0)] != 0
+            br["empty neighbour"] += int((live & ~nonempty).sum())
+            hitn = live & nonempty
+            rx, ry = np.where(hitn, cx, rx), np.where(hitn, cy, ry)
+            found |= hitn
+            active &= ~u & ~hitn
+    br["radius floor"] = int((floor & ~u).sum())
+    br["exhausted"] = int((~found & ~u).sum())
+    F = np.flatnonzero(found)
+    lidx, ridx = py[F] * w + px[F], ry[F] * w + rx[F]
+    lid, rid = rf["id"][lidx].astype(np.int64), rf["id"][ridx].astype(np.int64)
+    assert (lid < nl).all() and (rid < nl).all(), "K7 light id outside the light table"
+    lp, rp = rf["point"][lidx], rf["point"][ridx]
+    lh = hit(n2w, w, h, d0, d1, fast, px[F], py[F])
+    rh = hit(n2w, w, h, d0, d1, fast, rx[F], ry[F])
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        pdf_lr, uc1, us1 = di_pdf(lights[lid], rh, lp)
+        pdf_rl, uc2, us2 = di_pdf(lights[rid], lh, rp)
+        pos_lr, pos_rl = pdf_lr.v > pdf_lr.e, pdf_rl.v > pdf_rl.e
+        zero_lr, zero_rl = (pdf_lr.v == 0) & (pdf_lr.e == 0), (pdf_rl.v == 0) & (pdf_rl.e == 0)
+        upd = uc1 | us1 | uc2 | us2 | ~(pos_lr | zero_lr) | ~(pos_rl | zero_rl)
+
+        def ray(point, ht):
+            d = ht["point"] - z(point)
+            ln = dot3(d, d).sqrt()
+            enc, dec = oct_encode(d * (1.0 / ln).x3())
+            return ln, enc, dec
+        len_a, enc_a, dec_a = ray(lp, rh)
+        len_b, enc_b, dec_b = ray(rp, lh)
+    ufold = ~upd & ((pos_lr & ~dec_a) | (pos_rl & ~dec_b))
+    und_n["pdf"] = int(upd.sum()); und_n["fold"] = int(ufold.sum())
+    u[F] |= upd | ufold
+    und[P] = u
+    st = np.where(found, 2, 1)
+    state[P] = st
+    return dict(pairs=(gx, gy, lx), state=state, undecided=und, und=und_n, branches=br, found=P[F], rhs_idx=ridx + 1,
+                lhs_point=lp, rhs_point=rp, len_a=len_a, len_b=len_b, enc_a=enc_a, enc_b=enc_b, zero_a=~pos_lr, zero_b=~pos_rl,
+                lhs_rhs_pdf=pdf_lr, rhs_lhs_pdf=pdf_rl, found_und=u[F], w=w, h=h, n2w=n2w, depth=depth)
+
+
+def check_spatial_pick(got_d0, got_d1, before_d0, before_d1, r, what):
+    """K7's scratch texels against the restatement, at every pair that is not undecided: state 0 pairs and the columns past the
+    grid untouched; state 1: both d1 texels zero, d0 as it was; state 2: rhs_idx + 1 exact, ray origins the light points' words
+    exactly (zero for a zero ray), lengths, encoded directions and pdfs within their bounds (a zero ray: length 0, NaN direction).
+    Texel b at x = w is dropped.  Returns dict(ratio, undecided, pairs, tight [bounded below 1e-3 relative, finite nonzero])."""
+    w, h = r["w"], r["h"]
+    gd0, gd1 = (np.asarray(a, np.float32).reshape(h * w, 4) for a in (got_d0, got_d1))
+    bd0, bd1 = (np.asarray(a, np.float32).reshape(h * w, 4) for a in (before_d0, before_d1))
+    gx, gy, lx = r["pairs"]
+    ax, bx = gx * 2, gx * 2 + 1
+    ia, ib = gy * w + ax, gy * w + np.minimum(bx, w - 1)
+    bin_ = bx < w
+    # the texels of the checked rows that no decided pair may write: both buffers as they were
+    keep = np.isin(np.arange(h * w) // w, gy)
+    und = r["undecided"]
+    skip = np.zeros(h * w, bool)
+    skip[ia[und]] = True; skip[ib[und & bin_]] = True
+    s0 = r["state"] == 0
+    for b, g, nm in ((bd0, gd0, "d0"), (bd1, gd1, "d1")):
+        untouched = keep & ~skip
+        for st in (1, 2):
+            sel = (r["state"] == st) & ~und
+            if st == 2 or nm == "d1":
+                untouched[ia[sel]] = False; untouched[ib[sel & bin_]] = False
+        assert (g[untouched].view(np.uint32) == b[untouched].view(np.uint32)).all(), f"{what}: K7 wrote a texel it should leave ({nm})"
+    s1 = (r["state"] == 1) & ~und
+    for i in (ia[s1], ib[s1 & bin_]):
+        assert (gd1[i].view(np.uint32) == 0).all(), f"{what}: K7 state-1 d1 texel is not zero"
+    assert not s0[und].any()
+    F = r["found"]
+    fu = r["found_und"]
+    F, sel = F[~fu], ~fu
+    a, b, inb = ia[F], ib[F], bin_[F]
+    out = dict(ratio=0.0, undecided=int(und.sum()), pairs=int((~s0).sum()), tight=[0, 0])
+    ba1, bb1 = gd1[a].view(np.uint32), gd1[b].view(np.uint32)
+    assert (ba1[:, 2] == r["rhs_idx"][sel].astype(np.uint32)).all(), f"{what}: K7 rhs_idx + 1"
+    assert (ba1[:, 3] == 0).all(), f"{what}: K7 texel a d1.w"
+    worst = [0.0]
+
+    def within(got, num, key, mask):
+        v, e = num.v[sel][mask], num.e[sel][mask]
+        gg = got[mask].astype(np.float64)
+        err = np.abs(gg - v)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            rk = np.where(err == 0, 0.0, err / e)
+        rk = np.where(np.isnan(rk), np.inf, rk)
+        if not (rk <= 1).all():
+            i = np.flatnonzero(~(rk <= 1).reshape(len(rk), -1).all(1))[:4]
+            raise AssertionError(f"{what}: K7 {key} outside its bound at pairs {F[mask][i].tolist()}: got {gg[i].tolist()} want "
+                                 f"{v[i].tolist()} bound {e[i].tolist()}")
+        worst[0] = max(worst[0], float(rk.max()) if rk.size else 0.0)
+        if key in ("len", "pdf"):
+            fin = np.isfinite(v) & (v != 0)
+            out["tight"][0] += int((e[fin] < 1e-3 * np.abs(v[fin])).sum()); out["tight"][1] += int(fin.sum())
+
+    for tex0, tex1, key, mask in ((gd0[a], gd1[a], "a", np.ones(len(F), bool)), (gd0[b], gd1[b], "b", inb)):
+        zr = r["zero_" + key][sel]
+        pt = r["lhs_point" if key == "a" else "rhs_point"][sel]
+        live = mask & ~zr
+        assert (tex0[live][:, 0:3].view(np.uint32) == pt[live].view(np.uint32)).all(), f"{what}: K7 ray {key} origin"
+        dead = mask & zr
+        assert (tex0[dead].view(np.uint32) == 0).all() and np.isnan(tex1[dead][:, 0:2]).all(), f"{what}: K7 zero ray {key}"
+        within(tex0[:, 3], r["len_" + key], "len", live)
+        within(tex1[:, 0:2], r["enc_" + key], "direction", live)
+    within(gd1[b][:, 2], r["lhs_rhs_pdf"], "pdf", inb)
+    within(gd1[b][:, 3], r["rhs_lhs_pdf"], "pdf", inb)
+    out["ratio"] = worst[0]
+    return out
+
+
+def di_ray_f32(point, hit_pt):
+    """DiSample::ray evaluated in f32 operation by operation, with the direction through the octahedral round trip (Normal::encode,
+    then Normal::decode as the trace pass does): the strict build's (N, 8) ray, exactly."""
+    f = np.float32
+    p, q = np.asarray(point, f), np.asarray(hit_pt, f)
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+        d = q - p
+        ln = np.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])
+        n = d * (f(1) / ln)[:, None]
+        n = n / ((np.abs(n[:, 0]) + np.abs(n[:, 1])) + np.abs(n[:, 2]))[:, None]
+        up = n[:, 2] >= 0
+        ex = np.where(up, n[:, 0], np.copysign(f(1) - np.abs(n[:, 1]), n[:, 0]))
+        ey = np.where(up, n[:, 1], np.copysign(f(1) - np.abs(n[:, 0]), n[:, 1]))
+        enc = np.stack([ex * f(0.5) + f(0.5), ey * f(0.5) + f(0.5)], -1).astype(f)
+    rays = np.zeros((len(p), 8), f)
+    rays[:, 0:3], rays[:, 3], rays[:, 4:7] = p, ln, oct_decode_f32(enc)
+    return rays
+
+
+def pick_stash(r, trace_any):
+    """K9's per-pair inputs as the fused launch makes them from K7's pairs: rhs_idx (0 without a neighbour), the two pdfs (Num; 0 at
+    texel b's x = w, which the launch does not trace) and the visibility of each ray from `trace_any` of the ray rebuilt in strict f32
+    (a zero ray is visible).  Returns the dict di_spatial_sample takes, plus `rays_b` (the pairs whose texel b is traced)."""
+    gx, gy, lx = r["pairs"]
+    w = r["w"]
+    npair = len(gx)
+    fast = r["len_a"].fast
+    rhs_idx = np.zeros(npair, np.int64)
+    vis_a, vis_b = np.zeros(npair), np.zeros(npair)
+    zero = Num(np.zeros(npair), 0.0, fast)
+    plr, prl = Num(zero.v.copy(), zero.e.copy(), fast), Num(zero.v.copy(), zero.e.copy(), fast)
+    F = r["found"]
+    inb = (gx[F] * 2 + 1) < w
+    rhs_idx[F] = r["rhs_idx"]
+    plr.v[F] = np.where(inb, r["lhs_rhs_pdf"].v, 0.0); plr.e[F] = np.where(inb, r["lhs_rhs_pdf"].e, 0.0)
+    prl.v[F] = np.where(inb, r["rhs_lhs_pdf"].v, 0.0); prl.e[F] = np.where(inb, r["rhs_lhs_pdf"].e, 0.0)
+    pts = hit_point_f32(r["n2w"], w, r["h"], r["depth"])
+    ra = di_ray_f32(r["lhs_point"], pts[(r["rhs_idx"] - 1) // w, (r["rhs_idx"] - 1) % w])
+    rb = di_ray_f32(r["rhs_point"], pts[gy[F], lx[F]])
+    va = np.where(r["zero_a"], 1.0, 1.0 - np.asarray(trace_any(ra), np.float64))
+    vb = np.where(r["zero_b"], 1.0, 1.0 - np.asarray(trace_any(rb), np.float64))
+    vis_a[F], vis_b[F] = va, np.where(inb, vb, 0.0)
+    skip = r["undecided"].copy()
+    traced_a = rhs_idx > 0
+    traced_b = traced_a & ((gx * 2 + 1) < w)
+    return dict(rhs_idx=rhs_idx, vis_a=vis_a, vis_b=vis_b, lhs_rhs_pdf=plr, rhs_lhs_pdf=prl, skip=skip, traced_a=traced_a & ~skip,
+                traced_b=traced_b & ~skip)
+
+
+def flip_visibility(st, a, b):
+    """The composed K9 inputs with the visibility of ray a and / or ray b flipped on every traced pair."""
+    out = dict(st)
+    if a:
+        out["vis_a"] = np.where(st["traced_a"], 1.0 - st["vis_a"], st["vis_a"])
+    if b:
+        out["vis_b"] = np.where(st["traced_b"], 1.0 - st["vis_b"], st["vis_b"])
+    return out
+
+
+def pick_tight_ok(acc):
+    """At least 99 % of K7's finite nonzero lengths and pdfs are bounded below 1e-3 relative."""
+    return acc[1] > 0 and acc[0] >= 0.99 * acc[1]
+
+
 # ---- checks shared by the CPU chain test and the GPU tests --------------------------------------------------------------------
 
+def merge_alternatives(rs):
+    """One K9 restatement whose candidates are those of all of `rs` (the same pairs under different visibility bits)."""
+    return dict(rs[0], cands=[c for r in rs for c in r["cands"]], undecided=np.logical_or.reduce([r["undecided"] for r in rs]))
+
+
 def check_spatial_sample(got, res_in, r, what):
-    """Every merged pair matches one of its admissible outcomes: the discrete words bit for bit, m and w within their bounds; the
-    pass-through pixels are copies.  Returns (largest error / bound ratio, undecided pairs, merged pairs)."""
+    """Every merged pair (but the skipped ones) matches one of its admissible outcomes: the discrete words bit for bit, m, w and a
+    bounded pdf within their bounds; the pass-through pixels are copies.  Returns (largest error / bound ratio, undecided pairs,
+    merged pairs, visibility bits flipped: the fewest flipped rays any matching candidate needs, summed over the pairs)."""
     got = np.asarray(got, np.float32).reshape(-1, 8)
     g = got[r["idx"]]
     gb = g.view(np.uint32)
-    ok = np.zeros(len(g), bool)
+    ok = r["skip"].copy()
     best = np.full(len(g), np.inf)
+    flips = np.full(len(g), np.inf)
     for c in r["cands"]:
         wb = c["words"].view(np.uint32)
-        disc = (gb[:, 2:8] == wb[:, 2:8]).all(1)
-        if c is r["cands"][-1]:          # pass-through: every word as read
+        disc = (gb[:, 3:8] == wb[:, 3:8]).all(1)
+        if "pdf" not in c:          # pass-through: every word as read
             ratio = np.where((gb == wb).all(1), 0.0, np.inf)
         else:
             with np.errstate(invalid="ignore", divide="ignore"):
                 rat = []
-                for k, key in ((0, "m"), (1, "w")):
+                for k, key in ((0, "m"), (1, "w"), (2, "pdf")):
                     err = np.abs(g[:, k].astype(np.float64) - c[key])
                     rk = np.where(err == 0, 0.0, err / c[key + "_e"])
                     rat.append(np.where(np.isnan(rk), np.inf, rk))
-                ratio = np.maximum(rat[0], rat[1])
-        good = c["allowed"] & disc & (ratio <= 1.0)
+                # an exact pdf (e = 0) is compared bit for bit
+                rat[2] = np.where(c["pdf_e"] == 0, np.where(gb[:, 2] == wb[:, 2], 0.0, np.inf), rat[2])
+                ratio = np.maximum(np.maximum(rat[0], rat[1]), rat[2])
+        good = c["allowed"] & disc & (ratio <= 1.0) & ~r["skip"]
         best = np.where(good, np.minimum(best, ratio), best)
+        flips = np.where(good, np.minimum(flips, c["flips"]), flips)
         ok |= good
     if not ok.all():
         i = np.flatnonzero(~ok)[:4]
@@ -1087,15 +1471,19 @@ def check_spatial_sample(got, res_in, r, what):
     cp = r["copies"]
     src = np.asarray(res_in, np.float32).reshape(-1, 8)[cp].view(np.uint32)
     assert (got[cp].view(np.uint32) == src).all(), f"{what}: pass-through reservoirs differ"
-    return float(best.max()) if len(best) else 0.0, int(r["undecided"].sum()), int(r["merge"].sum())
+    best = best[~r["skip"]]
+    flipped = np.where(np.isfinite(flips) & ~r["skip"], flips, 0)
+    return (float(best.max()) if len(best) else 0.0, int(r["undecided"].sum()), int((r["merge"] & ~r["skip"]).sum()), int(flipped.sum()))
 
 
 def spatial_sample_tight(r):
     """(fraction of the merged pairs' finite nonzero m and w whose bound is below 1e-3 of the value, count), over the outcome the f64
     decisions select (undecided pairs are left out)."""
     n = t = 0
-    for c in r["cands"][:-1]:
-        sel = c["allowed"] & ~r["undecided"]
+    for c in r["cands"]:
+        if "pdf" not in c or c["flips"]:
+            continue
+        sel = c["allowed"] & ~r["undecided"] & ~r["skip"]
         for key in ("m", "w"):
             v, e = c[key][sel], c[key + "_e"][sel]
             fin = np.isfinite(v) & (v != 0)

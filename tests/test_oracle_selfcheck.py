@@ -382,7 +382,8 @@ def test_transmittance_lut_is_physically_plausible(oracle, blue_noise):
 
 
 def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11), edge_lights=False, extra_lights=0, remove=9001):
-    """K6 (DI temporal resampling), K8 (the spatial visibility rays), K9 (DI spatial merge) and K10 (DI resolving) of the strict
+    """K5 (DI sampling), K6 (DI temporal resampling), K7 (the spatial tap choice), K8 (the spatial visibility rays), K9 (DI spatial
+    merge, and K7 + K8 + K9 composed as the fused launch is checked) and K10 (DI resolving) of the strict
     oracle against tests/ref64_restir.py, pass by pass: the frame is stepped with render_range, each pass's inputs are read right
     before it runs and its outputs right after.  `extra_lights` small point lights are added before the first frame; `remove` is
     the light taken out on frame 10 (9001, the last one, kills its slot; one from the middle of the list remaps the last slot)."""
@@ -395,7 +396,7 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
     t_prev = t.copy()          # the camera before the last update_camera: what the engine keeps as the previous camera
     stats = {"K6": [0.0, {}, 0], "K6 tight": {k: [0, 0] for k in ("m", "w", "pdf")}, "K6 branches": [0, 0, 0], "K8": [0, 0],
              "K9": [0.0, 0, 0], "K10": [0.0, 0], "K9 tight": [0, 0], "K5": [0.0, {}, 0, 0],
-             "K5 tight": {k: [0, 0] for k in ("w", "light_point")}}
+             "K5 tight": {k: [0, 0] for k in ("w", "light_point")}, "K7": [0.0, 0, 0], "K7 tight": [0, 0], "K7 branches": {}}
     if edge_lights:
         from tests.test_restir_reference import edge_lights as add_lights
         add_lights(e)
@@ -414,7 +415,7 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
             e.remove_light(remove)
         e.tick()
         sched = e.frame_schedule(cam)
-        k5, k6, k8, k9, k10 = sched.index(1), sched.index(2), sched.index(4), sched.index(5), sched.index(6)
+        k5, k6, k7, k8, k9, k10 = (sched.index(p) for p in (1, 2, 3, 4, 5, 6))
         rd = lambda n: e.read_buffer(cam, n)
         cur = "b" if f % 2 == 1 else "a"
         old = "a" if cur == "b" else "b"
@@ -440,13 +441,28 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
         k6r = Q.di_temporal(Q.ndc_to_world(t, c["projection"]), Q.ndc_to_world(t_prev, c["projection"]), w, h, gb, gb_prev,
                             rd("reprojection_map"), e.read_scene("lights"), r1, r0, Q.dispatch_seed(0xC0FFEE, f, 2), fast=False)
         e.render_range(cam, k6, k6)
-        ratio, und, npx = Q.check_temporal(rd("di_reservoirs_1"), r1, k6r, f"f{f} K6")
+        ratio, und, npx, _ = Q.check_temporal(rd("di_reservoirs_1"), r1, k6r, f"f{f} K6")
+        # the composition the fused K5 + K6 launch is checked against: K5's restated sample (bounded w and light point, the
+        # occluded bit from trace_any of the strict f32 rebuild) handed to K6's restatement; on the strict oracle every pixel matches
+        lhs = Q.sampling_lhs(k5r, lambda x: oracle.math("sin", x), lambda x: oracle.math("cos", x), e.trace_any)
+        kc6 = Q.di_temporal(Q.ndc_to_world(t, c["projection"]), Q.ndc_to_world(t_prev, c["projection"]), w, h, gb, gb_prev,
+                            rd("reprojection_map"), e.read_scene("lights"), None, r0, Q.dispatch_seed(0xC0FFEE, f, 2), fast=False, lhs=lhs)
+        Q.check_temporal(rd("di_reservoirs_1"), r1, kc6, f"f{f} K5-K6 composed")
         s = stats["K6"]
         stats["K6"] = [max(s[0], ratio), {k: s[1].get(k, 0) + v for k, v in und.items()}, s[2] + npx]
         for k, (tt, nn) in Q.temporal_tight(k6r).items():
             stats["K6 tight"][k][0] += tt; stats["K6 tight"][k][1] += nn
         stats["K6 branches"] = [a + k6r[b] for a, b in zip(stats["K6 branches"], ("reprojected", "killed", "remapped"))]
-        e.render_range(cam, k6 + 1, k8 - 1)
+        e.render_range(cam, k6 + 1, k7 - 1)
+        p0, p1, r1 = rd("di_diff_samples"), rd("di_diff_curr_colors"), rd("di_reservoirs_1")
+        k7r = Q.di_spatial_pick(Q.ndc_to_world(t, c["projection"]), w, h, rd(f"prim_gbuffer_d0_{cur}"), rd(f"prim_gbuffer_d1_{cur}"),
+                                e.read_scene("lights"), r1, Q.dispatch_seed(0xC0FFEE, f, 3), f, fast=False)
+        e.render_range(cam, k7, k7)
+        s7 = Q.check_spatial_pick(rd("di_diff_samples"), rd("di_diff_curr_colors"), p0, p1, k7r, f"f{f} K7")
+        stats["K7"] = [max(stats["K7"][0], s7["ratio"]), stats["K7"][1] + s7["undecided"], stats["K7"][2] + s7["pairs"]]
+        stats["K7 tight"] = [a + b for a, b in zip(stats["K7 tight"], s7["tight"])]
+        stats["K7 branches"] = {k: stats["K7 branches"].get(k, 0) + v for k, v in k7r["branches"].items()}
+        e.render_range(cam, k7 + 1, k8 - 1)
         b0, b1 = rd("di_diff_samples"), rd("di_diff_curr_colors")
         e.render_range(cam, k8, k8)
         traced, bad = Q.check_spatial_trace(b0, b1, rd("di_diff_stash"), e.trace_any, f"f{f} K8")
@@ -457,7 +473,11 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
         e.render_range(cam, k9, k9)
         r2 = rd("di_reservoirs_2")
         k9r = Q.di_spatial_sample(r1, stash, Q.dispatch_seed(0xC0FFEE, f, 5), f, w, h, fast=False)
-        ratio, und, merged = Q.check_spatial_sample(r2, r1, k9r, f"f{f} K9")
+        ratio, und, merged, _ = Q.check_spatial_sample(r2, r1, k9r, f"f{f} K9")
+        # the composition the fused K7 + K8 + K9 launch is checked against: K7's restatement, trace_any of its rays rebuilt in strict
+        # f32, K9's restatement with bounded pdfs; on the strict oracle every pair must match with each visibility bit as traced
+        kc = Q.di_spatial_sample(r1, Q.pick_stash(k7r, e.trace_any), Q.dispatch_seed(0xC0FFEE, f, 5), f, w, h, fast=False)
+        Q.check_spatial_sample(r2, r1, kc, f"f{f} K7-K9 composed")
         stats["K9"] = [max(stats["K9"][0], ratio), stats["K9"][1] + und, stats["K9"][2] + merged]
         frac, n = Q.spatial_sample_tight(k9r)
         stats["K9 tight"] = [stats["K9 tight"][0] + round(frac * n), stats["K9 tight"][1] + n]
@@ -516,7 +536,9 @@ def test_restir_float64_chain_matches_oracle(oracle, blue_noise, which):
     print(f"\n{which}: K5 ratio {k5[0]:.3g} over {k5[2]} pixels, undecided {k5[1]}, {k5[3]} shadow rays, tight {stats['K5 tight']}; "
           f"K6 ratio {k6[0]:.3g} over {k6[2]} pixels, undecided {k6[1]}, reprojected / killed / remapped "
           f"{stats['K6 branches']}; K8 {stats['K8'][0]} rays traced, {stats['K8'][1]} differ; K9 ratio {stats['K9'][0]:.3g}, "
-          f"undecided {stats['K9'][1]} of {stats['K9'][2]} merges; K10 ratio {stats['K10'][0]:.3g}, undecided specular {stats['K10'][1]}")
+          f"undecided {stats['K9'][1]} of {stats['K9'][2]} merges; K10 ratio {stats['K10'][0]:.3g}, undecided specular {stats['K10'][1]}; "
+          f"K7 ratio {stats['K7'][0]:.3g}, undecided {stats['K7'][1]} of {stats['K7'][2]} pairs, tight {stats['K7 tight']}, "
+          f"branches {stats['K7 branches']}")
     assert stats["K9"][2] > 0 and stats["K9"][1] <= 0.01 * stats["K9"][2]
     assert 1e-3 < stats["K10"][0] <= 1 and 1e-3 < stats["K9"][0] <= 1 and 1e-3 < k6[0] <= 1
     assert stats["K9 tight"][0] >= 0.99 * stats["K9 tight"][1] > 0, stats["K9 tight"]
@@ -527,6 +549,8 @@ def test_restir_float64_chain_matches_oracle(oracle, blue_noise, which):
     assert stats["K6 branches"][0] > 0 and stats["K8"][0] > 0
     assert 1e-3 < k5[0] <= 1 and k5[3] > 0 and Q.sampling_tight_ok(stats["K5 tight"]), stats["K5 tight"]
     assert all(v <= 0.01 * k5[2] for v in k5[1].values()), k5[1]
+    k7 = stats["K7"]
+    assert 1e-3 < k7[0] <= 1 and k7[1] <= 0.01 * k7[2] and Q.pick_tight_ok(stats["K7 tight"]), (k7, stats["K7 tight"])
     if which.startswith("cornell"):     # a reprojected reservoir named light 9001 (or the light removed) after its removal
         assert stats["K6 branches"][1] > 0
     if which == "cornell_remap":

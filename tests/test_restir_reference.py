@@ -15,10 +15,12 @@ from tests.util import Frame, check_within, write_buffer
 
 pytestmark = pytest.mark.gpu
 
-P_DI_SAMPLING, P_DI_TEMPORAL, P_DI_SPATIAL_TRACE, P_DI_SPATIAL_SAMPLE, P_DI_RESOLVING = 1, 2, 4, 5, 6
+P_DI_SAMPLING, P_DI_TEMPORAL, P_DI_SPATIAL_PICK, P_DI_SPATIAL_TRACE, P_DI_SPATIAL_SAMPLE, P_DI_RESOLVING = 1, 2, 3, 4, 5, 6
+SCRATCH = ("di_diff_samples", "di_diff_curr_colors", "di_diff_stash")
 SEED_BASE = 0xC0FFEE
 SCENES = {"cornell": scenes.cornell, "demo_level": scenes.demo_level, "textured_room": scenes.textured_room,
-          "cornell_spots": lambda w, h: scenes.cornell_spots(w, h), "cornell_many_lights": scenes.cornell, "cornell_remap": scenes.cornell}
+          "cornell_spots": lambda w, h: scenes.cornell_spots(w, h), "cornell_many_lights": scenes.cornell, "cornell_remap": scenes.cornell,
+          "normal_mapped_room": scenes.normal_mapped_room}
 # undecided decisions allowed per pass, as a fraction of the values checked.  None were seen in the scene runs on an H100 (24 runs, both
 # tiers); the injected M = 1e6 / w = 1e6 reservoirs put 3.6 % of K9's merges inside the bound of `rng W < weight` (W dominated by the
 # huge weight, the other weight below its rounding), hence the looser limit there.
@@ -27,8 +29,20 @@ UNDECIDED_MAX_EDGES = 0.1
 # K8's visibility bit against trace_any of the ray decoded in strict f32, as a fraction of the rays traced.  The strict build must
 # agree on every ray; the fast build decodes the octahedral direction with FMA contraction, so a ray grazing an edge may differ.
 # Worst seen in the fast scene runs on an H100: 3 of 29164 rays (1.0e-4, textured room 67x45); the cap is 1e-3 of the rays traced.
+# The fused K7-K9 launch, against the rays of K7's restatement rebuilt in strict f32: 55 of 238198 rays (2.3e-4, textured room
+# 224x126, fast build), 0 in the strict build.
 K8_DISAGREE_MAX = 1e-3
 K5_EVERY_FRAME_PX = 67 * 45     # screens up to this size check K5 on every frame, larger ones on every third (Chain.frame)
+# K7 pairs with an undecided decision (a tap coordinate within its bound of an integer, a depth or normal test or `pdf > 0` within
+# its bound, an octahedral fold sign), as a fraction of the pairs checked, for K7 alone and for the fused K7-K9 launch (plus K9's
+# undecided merges there).  Worst seen on an H100 (every run of this file, both tiers): 1.3e-3 (fused K7-K9, textured room 67x45, fast
+# build, with empty reservoirs injected); K7 alone 9.1e-4.  The cap is 1.5 times the worst.
+K7_UNDECIDED_MAX = 0.002
+# The fused K5 + K6 launch against K5 composed into K6, per decision type, as a fraction of the pixels checked.  K6's lhs light point
+# now carries K5's bound, and Light::ray_bnoise puts it near the light's sphere, so `Light::contains` (|center - point| <= radius) is
+# often decided inside that bound.  Worst seen on an H100 (fast build): contains 5.4e-3 (textured room 224x126), K6's updates 2.3e-3
+# (Cornell with spot lights, 67x45), K5's selection or sign 7.4e-4; the cap is about twice the worst.
+FUSED_K6_UNDECIDED_MAX = 0.01
 
 
 @pytest.fixture(scope="module")
@@ -37,18 +51,21 @@ def gpu():
     return strolle_b200
 
 
-def _engine(gpu, blue_noise, strict, fused):
-    from strolle_b200.engine import OPT_FUSED_PASSES
+def _engine(gpu, blue_noise, strict, fused, nmap=False):
+    from strolle_b200.engine import OPT_FUSED_PASSES, OPT_NORMAL_MAPS
     e = gpu.Engine(blue_noise=blue_noise, exact=strict)
     e.set_option(OPT_FUSED_PASSES, int(fused))
+    e.set_option(OPT_NORMAL_MAPS, int(nmap))
     return e
 
 
 class Chain:
-    """Drives one camera frame by frame and checks K5, K6, K8, K9 (these four in the unfused schedule) and K10 as they run."""
+    """Drives one camera frame by frame and checks K5, K6, K7, K8, K9 (these five in the unfused schedule), the fused K7 + K8 + K9
+    launch against K7, K8 and K9 composed, and K10 as they run.  `rows`: the fused launch is checked on these rows only."""
 
-    def __init__(self, gpu, blue_noise, scene, strict, fused):
-        self.e = _engine(gpu, blue_noise, strict, fused)
+    def __init__(self, gpu, blue_noise, scene, strict, fused, nmap=False, rows=None):
+        self.e = _engine(gpu, blue_noise, strict, fused, nmap)
+        self.rows = rows
         self.scene = scene
         self.cam = scenes.apply(self.e, scene)
         c = scene["camera"]
@@ -57,7 +74,11 @@ class Chain:
         self.t_prev = self.t.copy()     # the camera before the last update_camera: the engine's previous camera
         self.fast = not strict
         self.blue_noise = blue_noise
-        self.stats = {"K9": [0.0, 0, 0], "K10": [0.0, 0, 0], "K6": [0.0, {}, 0], "K8": [0, 0], "K5": [0.0, {}, 0, 0, 0]}
+        self.stats = {"K9": [0.0, 0, 0], "K10": [0.0, 0, 0], "K6": [0.0, {}, 0], "K8": [0, 0], "K5": [0.0, {}, 0, 0, 0],
+                      "K7": [0.0, 0, 0], "K7-K9": [0.0, 0, 0, 0, 0],   # K7-K9: K9 ratio, undecided, merges, rays, disagreements
+                      "K5-K6": [0.0, {}, 0, 0]}    # ratio, undecided per decision type, pixels (one shadow ray each), disagreements
+        self.k7_tight = [0, 0]
+        self.k7_branches = dict.fromkeys(Q.K7_BRANCHES, 0)
         self.k5_tight = {k: [0, 0] for k in ("w", "light_point")}
         self.k6_tight = {k: [0, 0] for k in ("m", "w", "pdf")}
         self.k6_branches = [0, 0, 0]    # reprojected, killed, remapped
@@ -92,7 +113,78 @@ class Chain:
         for k, (tt, nn) in s5["tight"].items():
             self.k5_tight[k][0] += tt; self.k5_tight[k][1] += nn
 
-    def frame(self, inject_k9=None, inject_k10=None, inject_k6=None):
+    def _pick(self, fr, cur, inject_k7, rows=None):
+        """Runs to the launch before K7 (or the fused K7 + K8 + K9), injects, and restates K7 on what the launch will read: returns
+        (restatement, di_reservoirs[1], the three scratch buffers as they were)."""
+        e, f = self.e, self.f
+        k7 = fr.steps(P_DI_SPATIAL_PICK)[0]
+        fr.run_to(k7 - 1)
+        if inject_k7:
+            inject_k7(fr)
+        r1 = e.read_buffer(self.cam, "di_reservoirs_1")
+        scratch = [fr.read(n).copy() for n in SCRATCH]
+        r = Q.di_spatial_pick(Q.ndc_to_world(self.t, self.scene["camera"]["projection"]), self.w, self.h, fr.read(f"prim_gbuffer_d0_{cur}"),
+                              fr.read(f"prim_gbuffer_d1_{cur}"), e.read_scene("lights"), r1, Q.dispatch_seed(SEED_BASE, f, P_DI_SPATIAL_PICK),
+                              f, self.fast, rows)
+        self.k7_branches = {k: self.k7_branches[k] + v for k, v in r["branches"].items()}
+        fr.run_to(k7)
+        return r, r1, scratch
+
+    def _check_fused_spatial(self, fr, cur, inject_k7):
+        """k_di_spatial_fused against K7, K8 (trace_any of each ray rebuilt in strict f32) and K9 composed, on self.rows.  The strict
+        build must agree with every rebuilt ray; in the fast build a pair matched only with a flipped visibility bit counts as a
+        disagreement.  The scratch textures are left as they were."""
+        e, f = self.e, self.f
+        r7, r1, scratch = self._pick(fr, cur, inject_k7, self.rows)
+        for n, a in zip(SCRATCH, scratch):
+            assert (fr.read(n).view(np.uint32) == a.view(np.uint32)).all(), f"f{f} fused K7-K9 wrote {n}"
+        st = Q.pick_stash(r7, e.trace_any)
+        seed = Q.dispatch_seed(SEED_BASE, f, P_DI_SPATIAL_SAMPLE)
+        flips = [(False, False)] if not self.fast else [(False, False), (True, False), (False, True), (True, True)]
+        r = Q.merge_alternatives([Q.di_spatial_sample(r1, Q.flip_visibility(st, a, b), seed, f, self.w, self.h, self.fast, self.rows, a + b)
+                                  for a, b in flips])
+        ratio, und, merged, flipped = Q.check_spatial_sample(e.read_buffer(self.cam, "di_reservoirs_2"), r1, r, f"f{f} fused K7-K9")
+        s = self.stats["K7-K9"]
+        self.stats["K7-K9"] = [max(s[0], ratio), s[1] + und + int(r7["undecided"].sum()), s[2] + merged,
+                               s[3] + int(st["traced_a"].sum() + st["traced_b"].sum()), s[4] + flipped]
+
+    def _check_fused_temporal(self, fr, cur, old, restate):
+        """k_di_sample_temporal against K5 composed into K6 (sampling_lhs into di_temporal), inputs read just before the launch.  The
+        strict build must agree with trace_any of every shadow ray rebuilt in strict f32; in the fast build a pixel matched only with
+        its occluded bit flipped counts as a disagreement.  Without `restate` only the scratch textures are checked (left alone)."""
+        e, cam, w, h, f = self.e, self.cam, self.w, self.h, self.f
+        kt = fr.steps(P_DI_TEMPORAL)[0]
+        fr.run_to(kt - 1)
+        scratch = [fr.read(n).copy() for n in SCRATCH]
+        if restate:
+            proj = self.scene["camera"]["projection"]
+            n2w = Q.ndc_to_world(self.t, proj)
+            gb = [fr.read(f"prim_gbuffer_d{k}_{cur}") for k in (0, 1)]
+            gb_prev = [fr.read(f"prim_gbuffer_d{k}_{old}") for k in (0, 1)]
+            r1, r0, lights = e.read_buffer(cam, "di_reservoirs_1"), e.read_buffer(cam, "di_reservoirs_0"), e.read_scene("lights")
+            k5 = Q.di_sampling(n2w, w, h, gb[0], gb[1], lights, e.read_scene("world")[:1].view(np.uint32)[0], self.blue_noise,
+                               Q.dispatch_seed(SEED_BASE, f, P_DI_SAMPLING), f, self.fast)
+            lhs = Q.sampling_lhs(k5, lambda x: e.device_math("sin", x), lambda x: e.device_math("cos", x), e.trace_any)
+            args = (n2w, Q.ndc_to_world(self.t_prev, proj), w, h, gb, gb_prev, fr.read("reprojection_map"), lights, None, r0,
+                    Q.dispatch_seed(SEED_BASE, f, P_DI_TEMPORAL), self.fast)
+            rs = [Q.di_temporal(*args, lhs=lhs)]
+            if self.fast:
+                rs.append(Q.di_temporal(*args, lhs=dict(lhs, occ=~lhs["occ"]), flips=1))
+            r = Q.merge_temporal(rs)
+        fr.run_to(kt)
+        for n, a in zip(SCRATCH, scratch):
+            assert (fr.read(n).view(np.uint32) == a.view(np.uint32)).all(), f"f{f} fused K5-K6 wrote {n}"
+        if restate:
+            ratio, und, n, flipped = Q.check_temporal(e.read_buffer(cam, "di_reservoirs_1"), r1, r, f"f{f} fused K5-K6")
+            s = self.stats["K5-K6"]
+            self.stats["K5-K6"] = [max(s[0], ratio), {k: s[1].get(k, 0) + v for k, v in und.items()}, s[2] + n, s[3] + flipped]
+
+    def _k7_stats(self, s7):
+        s = self.stats["K7"]
+        self.stats["K7"] = [max(s[0], s7["ratio"]), s[1] + s7["undecided"], s[2] + s7["pairs"]]
+        self.k7_tight = [a + b for a, b in zip(self.k7_tight, s7["tight"])]
+
+    def frame(self, inject_k9=None, inject_k10=None, inject_k6=None, inject_k7=None):
         e, cam, w, h = self.e, self.cam, self.w, self.h
         self.f += 1
         f = self.f
@@ -101,6 +193,10 @@ class Chain:
         cur = "b" if f % 2 == 1 else "a"
         old = "a" if cur == "b" else "b"
         k9 = fr.steps(P_DI_SPATIAL_SAMPLE)
+        if not k9:   # fused schedule: k_di_sample_temporal (pass 2), then k_di_spatial_fused (pass 3)
+            # as for K5 in the unfused schedule, screens above K5_EVERY_FRAME_PX check pass 2 on every third frame
+            self._check_fused_temporal(fr, cur, old, self.rows is None and (w * h <= K5_EVERY_FRAME_PX or f % 3 == 1))
+            self._check_fused_spatial(fr, cur, inject_k7)
         if k9:   # unfused schedule: K5 writes its samples to di_reservoirs[1], K6 reads them from there
             # K5 carries no state from frame to frame, so above K5_EVERY_FRAME_PX pixels it is checked on every third frame (1, 4, 7,
             # 10, 13: the frames that insert, move and remove a light); its f64 restatement is the costliest of the chain
@@ -117,12 +213,16 @@ class Chain:
             r = Q.di_temporal(Q.ndc_to_world(self.t, proj), Q.ndc_to_world(self.t_prev, proj), w, h, gb, gb_prev, fr.read("reprojection_map"),
                               e.read_scene("lights"), r1, r0, Q.dispatch_seed(SEED_BASE, f, P_DI_TEMPORAL), self.fast)
             fr.run_to(k6)
-            ratio, und, n = Q.check_temporal(e.read_buffer(cam, "di_reservoirs_1"), r1, r, f"f{f} K6")
+            ratio, und, n, _ = Q.check_temporal(e.read_buffer(cam, "di_reservoirs_1"), r1, r, f"f{f} K6")
             s = self.stats["K6"]
             self.stats["K6"] = [max(s[0], ratio), {k: s[1].get(k, 0) + v for k, v in und.items()}, s[2] + n]
             for k, (tt, nn) in Q.temporal_tight(r).items():
                 self.k6_tight[k][0] += tt; self.k6_tight[k][1] += nn
             self.k6_branches = [a + r[b] for a, b in zip(self.k6_branches, ("reprojected", "killed", "remapped"))]
+            # K7 too carries no state from frame to frame: above K5_EVERY_FRAME_PX pixels it is checked on K5's frames
+            if w * h <= K5_EVERY_FRAME_PX or f % 3 == 1:
+                r7, _, (p0, p1, _) = self._pick(fr, cur, inject_k7)
+                self._k7_stats(Q.check_spatial_pick(fr.read("di_diff_samples"), fr.read("di_diff_curr_colors"), p0, p1, r7, f"f{f} K7"))
             k8 = fr.steps(P_DI_SPATIAL_TRACE)[0]
             fr.run_to(k8 - 1)
             b0, b1 = fr.read("di_diff_samples"), fr.read("di_diff_curr_colors")
@@ -138,7 +238,7 @@ class Chain:
             r1, stash = e.read_buffer(cam, "di_reservoirs_1"), fr.read("di_diff_stash")
             fr.run_to(k9[0])
             r = Q.di_spatial_sample(r1, stash, Q.dispatch_seed(SEED_BASE, f, P_DI_SPATIAL_SAMPLE), f, w, h, self.fast)
-            ratio, und, merged = Q.check_spatial_sample(e.read_buffer(cam, "di_reservoirs_2"), r1, r, f"f{f} K9")
+            ratio, und, merged, _ = Q.check_spatial_sample(e.read_buffer(cam, "di_reservoirs_2"), r1, r, f"f{f} K9")
             s = self.stats["K9"]
             self.stats["K9"] = [max(s[0], ratio), s[1] + und, s[2] + merged]
             frac, n = Q.spatial_sample_tight(r)
@@ -161,10 +261,18 @@ class Chain:
 
     def report(self, tag, limit=UNDECIDED_MAX):
         s9, s10, s6, s8, s5 = self.stats["K9"], self.stats["K10"], self.stats["K6"], self.stats["K8"], self.stats["K5"]
+        s7, sf, st = self.stats["K7"], self.stats["K7-K9"], self.stats["K5-K6"]
         print(f"\n{tag}: K5 ratio {s5[0]:.3g} undecided {s5[1]} of {s5[2]}, shadow rays differ {s5[4]}/{s5[3]}, tight {self.k5_tight}; "
               f"K6 ratio {s6[0]:.3g} undecided {s6[1]} of {s6[2]}, reprojected / killed / remapped {self.k6_branches}; "
               f"K8 visibility differs {s8[1]}/{s8[0]}; K9 ratio {s9[0]:.3g} undecided {s9[1]}/{s9[2]}; "
-              f"K10 ratio {s10[0]:.3g} undecided specular {s10[1]}/{s10[2]}")
+              f"K10 ratio {s10[0]:.3g} undecided specular {s10[1]}/{s10[2]}; "
+              f"K7 ratio {s7[0]:.3g} undecided {s7[1]}/{s7[2]} tight {self.k7_tight} branches {self.k7_branches}; "
+              f"fused K7-K9 ratio {sf[0]:.3g} undecided {sf[1]}/{sf[2]} rays differ {sf[4]}/{sf[3]}; "
+              f"fused K5-K6 ratio {st[0]:.3g} undecided {st[1]} of {st[2]}, shadow rays differ {st[3]}/{st[2]}")
+        assert all(v <= max(limit, FUSED_K6_UNDECIDED_MAX) * max(st[2], 1) for v in st[1].values()), st
+        assert st[3] <= (0 if not self.fast else K8_DISAGREE_MAX * st[2]), st
+        assert s7[1] <= K7_UNDECIDED_MAX * max(s7[2], 1) and sf[1] <= K7_UNDECIDED_MAX * max(sf[2], 1), (s7, sf)
+        assert sf[4] <= (0 if not self.fast else K8_DISAGREE_MAX * sf[3]), sf
         assert s9[1] <= limit * max(s9[2], 1) and s10[1] <= limit * max(s10[2], 1)
         assert all(v <= limit * max(s6[2], 1) for v in s6[1].values()), s6[1]
         assert s8[1] <= K8_DISAGREE_MAX * s8[0], s8
@@ -172,8 +280,9 @@ class Chain:
         assert s5[4] <= K8_DISAGREE_MAX * s5[3], s5
 
 
-def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11), extra_lights=0, remove=9001):
-    ch = Chain(gpu, blue_noise, scene, strict, fused)
+def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11), extra_lights=0, remove=9001, nmap=False, rows=None,
+         inject_k7=None):
+    ch = Chain(gpu, blue_noise, scene, strict, fused, nmap, rows)
     many_lights(ch.e, extra_lights)
     for f in range(1, frames + 1):
         if f in moves:
@@ -184,20 +293,25 @@ def _run(gpu, blue_noise, scene, strict, fused, frames=13, moves=(3, 5, 8, 11), 
             ch.e.insert_light(9001, scenes.LIGHT_POINT, scenes.point_light((-0.3, 0.8, 0.1), 0.08, (3.0, 2.0, 1.0), 6.0))
         if f == 10:
             ch.e.remove_light(remove)
-        ch.frame()
+        ch.frame(inject_k7=inject_k7 and inject_k7(f))
     return ch
 
 
-@pytest.mark.parametrize("size", [(224, 126), (67, 45), (37, 29)])
-@pytest.mark.parametrize("scene_name", ["cornell", "demo_level", "textured_room", "cornell_spots", "cornell_many_lights", "cornell_remap"])
+@pytest.mark.parametrize("size", [(224, 126), (67, 45), (37, 29), (63, 45)])
+@pytest.mark.parametrize("scene_name", ["cornell", "demo_level", "textured_room", "cornell_spots", "cornell_many_lights", "cornell_remap",
+                                        "normal_mapped_room"])
 @pytest.mark.parametrize("strict", [True, False], ids=["strict", "fast"])
 def test_di_merge_and_resolve_within_float64_bound(gpu, blue_noise, strict, scene_name, size):
-    """K5, K6, K8, K9 and K10 in the unfused schedule, every pixel / texel / pair, frames 1-13 (both GI cycles) with the camera moving
-    and a light inserted, moved and removed; 67x45 leaves columns outside the half grid, 37x29 is smaller than the 128 px tap radius.
-    Many lights: 23, so K5 draws 16 of them; remap: the light removed is from the middle of the list, so K6 meets a remapped slot."""
+    """K5, K6, K7, K8, K9 and K10 in the unfused schedule, every pixel / texel / pair, frames 1-13 (both GI cycles) with the camera
+    moving and a light inserted, moved and removed; 67x45 leaves columns outside the half grid; the half grid of 63x45 is 64 wide, so
+    on alternate rows the last pair's lhs is off the screen (nothing written, no copy through) and its texel b lies at x = 63 (dropped);
+    37x29 is smaller than the 128 px tap radius (K7's mirrored taps land outside the frame).  Many lights: 23, so K5 draws 16 of them; remap: the light removed is from the
+    middle of the list, so K6 meets a remapped slot; the normal-mapped room shades with ST_OPT_NORMAL_MAPS, so the mapped normals feed
+    K7's normal test and every pdf."""
     many = scene_name in ("cornell_many_lights", "cornell_remap")
     ch = _run(gpu, blue_noise, SCENES[scene_name](*size), strict, fused=False, extra_lights=MANY_LIGHTS if many else 0,
-              remove=REMAP_REMOVED if scene_name == "cornell_remap" else 9001)
+              remove=REMAP_REMOVED if scene_name == "cornell_remap" else 9001, nmap=scene_name == "normal_mapped_room")
+    assert 1e-3 < ch.stats["K7"][0] <= 1 and Q.pick_tight_ok(ch.k7_tight), (ch.stats["K7"], ch.k7_tight)
     assert ch.stats["K9"][2] > 0 and 0 < ch.stats["K10"][0] <= 1 and 0 < ch.stats["K6"][0] <= 1 and ch.stats["K8"][0] > 0
     assert ch.k6_branches[0] > 0 and Q.tight_ok(ch.k6_tight), (ch.k6_branches, ch.k6_tight)
     if scene_name == "cornell_remap":
@@ -214,16 +328,44 @@ def test_di_merge_and_resolve_within_float64_bound(gpu, blue_noise, strict, scen
 
 
 
-@pytest.mark.parametrize("scene_name", ["cornell", "demo_level"])
-def test_di_resolve_product_default_within_bound(gpu, blue_noise, scene_name):
-    """The product default (fast build, fused passes): K10 still runs as its own launch and is checked against the bound."""
-    ch = _run(gpu, blue_noise, SCENES[scene_name](224, 126), strict=False, fused=True)
+def _empty_reservoirs(seed):
+    """Sets M = 0 on half of di_reservoirs[1]'s pixels before K7 (or the fused K7 + K8 + K9): long walks, walks that reach the radius
+    floor, accepted neighbours with an empty reservoir, and pairs whose lhs is empty while the rhs is not."""
+    def inject(fr):
+        rng = np.random.RandomState(seed)
+        r = fr.e.read_buffer(fr.cam, "di_reservoirs_1").reshape(-1, 8).copy()
+        r[rng.rand(len(r)) < 0.5, 0] = 0
+        write_buffer(fr.e, fr.cam, "di_reservoirs_1", r.astype(np.float32))
+    return inject
+
+
+FUSED_CASES = [(s, size, False) for s in ("cornell", "demo_level", "textured_room", "cornell_spots")
+               for size in ((224, 126), (67, 45), (63, 45))] + [("cornell", (67, 45), True)]
+
+
+@pytest.mark.parametrize("scene_name,size,strict", FUSED_CASES,
+                         ids=[f"{s}-{w}x{h}-{'strict' if t else 'fast'}" for s, (w, h), t in FUSED_CASES])
+def test_di_resolve_product_default_within_bound(gpu, blue_noise, scene_name, size, strict):
+    """The product default (fast build, fused passes): k_di_sample_temporal against K5 composed into K6 (every pixel; every third
+    frame at 224x126), k_di_spatial_fused against K7, K8 and K9 composed (every pair), inputs read just before each launch, K10
+    against its bound, and neither fused DI launch touches the scratch textures.  The small screens get empty reservoirs injected
+    before the fused K7-K9 launch on every other frame; 63x45 has pairs whose lhs is off the screen and texel b at x = 63, which the
+    launch does not trace.  The strict-build case calibrates the compositions: there every rebuilt shadow ray must agree."""
+    w, h = size
+    inject = (lambda f: _empty_reservoirs(f) if f % 2 == 0 else None) if w < 224 else None
+    ch = _run(gpu, blue_noise, SCENES[scene_name](w, h), strict=strict, fused=True, inject_k7=inject)
     assert ch.stats["K9"][2] == 0 and ch.stats["K10"][2] > 0
-    ch.report(f"{scene_name} product default")
+    sf, st = ch.stats["K7-K9"], ch.stats["K5-K6"]
+    assert sf[2] > 0 and sf[3] > 0 and 1e-3 < sf[0] <= 1, sf
+    assert st[2] > 0 and 1e-3 < st[0] <= 1, st
+    ch.report(f"{scene_name} {w}x{h} product default{' (strict)' if strict else ''}")
 
 
 def test_di_resolve_1080p_product_default(gpu, blue_noise):
-    ch = _run(gpu, blue_noise, scenes.cornell(1920, 1080), strict=False, fused=True, frames=2, moves=())
+    """Two product-default frames at 1080p: K10 on every pixel, the fused K7 + K8 + K9 launch on a band of 32 rows (the fused K5 + K6
+    launch is checked at the smaller sizes above; here only that it leaves the scratch textures alone)."""
+    ch = _run(gpu, blue_noise, scenes.cornell(1920, 1080), strict=False, fused=True, frames=2, moves=(), rows=np.arange(524, 556))
+    assert ch.stats["K7-K9"][2] > 0
     ch.report("1080p product default")
 
 
@@ -329,9 +471,11 @@ def test_di_edge_inputs_within_bound(gpu, blue_noise, strict, scene_name):
     for f in range(1, 6):
         if f in (2, 4):
             ch.move(f)
-        ch.frame(_reservoir_edges(10 * f), _gbuffer_edges(10 * f + 1, ch), _temporal_edges(10 * f + 2))
+        ch.frame(_reservoir_edges(10 * f), _gbuffer_edges(10 * f + 1, ch), _temporal_edges(10 * f + 2), _empty_reservoirs(10 * f + 3))
         assert ch.e.read_scene("world")[:1].view(np.uint32)[0] == want
     assert 0 < ch.stats["K5"][0] <= 1 and ch.stats["K5"][2] > 0
+    # with half the reservoirs empty every branch of K7's walk is taken
+    assert all(v > 0 for v in ch.k7_branches.values()), ch.k7_branches
     ch.report(f"edges {scene_name} {want} lights {'strict' if strict else 'fast'}", UNDECIDED_MAX_EDGES)
 
 
