@@ -173,7 +173,15 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15 };
+/* ST_OPT_BVH_REFIT (default 0): N > 0 allows up to N refit ticks in a row.  A refit tick is an st_tick whose only scene change is new
+ * transforms of existing instances (same mesh, same material, nothing inserted or removed, no material's alpha mode changed): the moved
+ * instances' triangles are baked on the device (bit-identical to the host bake) and the BVH boxes are recomputed bottom-up on the device
+ * over the kept topology, with no host BVH build, no full upload and no stream synchronisation.  The next qualifying tick after N of
+ * them, and every other instance change, rebuilds on the host as with 0.  After a refit the tree is no longer the one the reference
+ * would build: closest hits stay the true closest hits (only equal-distance ties may resolve differently), any-hit answers are
+ * unchanged, and CameraMode::BvhHeatmap / used_memory show the refit tree.  0 = every tick that changed an instance rebuilds, as the
+ * reference does.  Takes effect at the next st_tick (DESIGN.md §2). */
 /* ST_OPT_NORMAL_MAPS (default 0): materials with a normal map shade with the mapped normal, n' = normalize((t.x T + t.y B) + t.z N) with
  * t = 2 texel / 255 - 1, T the interpolated mesh tangent (not renormalised), B = w (N x T), w its handedness (mirrored instances flip
  * it); where n' is not finite (meshes without tangents) or n'.N <= 0 the interpolated normal N stays.  Back faces flip the result as
@@ -242,7 +250,8 @@ int st_set_option(st_engine* e, int option, int value);
 enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_STAT_BVH_GRAFTED_SUBTREES = 3, ST_STAT_VARIANCE_TILED_LAUNCHES = 4,
        ST_STAT_STRIP_PULLED_ROWS = 5 /* rows x buffers fetched from other ranks by the temporal pull since linking */, ST_STAT_LAST_FRAME_FUSED_STRIPS = 6 /* 1 = the last strip frame used the fused transport */,
        ST_STAT_STRIP_FIRST_TIMEOUT = 7 /* 0, or 0x80000000 | slot << 16 | awaited rank << 8 | sequence & 0xff of the first strip flag wait that gave up */,
-       ST_STAT_NORMAL_MAP_LAUNCHES = 8 /* launches of the normal-mapped kernel variants (ST_OPT_NORMAL_MAPS) since creation */ };
+       ST_STAT_NORMAL_MAP_LAUNCHES = 8 /* launches of the normal-mapped kernel variants (ST_OPT_NORMAL_MAPS) since creation */,
+       ST_STAT_BVH_REFITS = 9 /* refit ticks (ST_OPT_BVH_REFIT) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,

@@ -43,9 +43,12 @@ pub struct StrolleSun {
 /// Engine-wide settings, read once when the plugin finishes building; insert the resource before `StrollePlugin` to change them.
 /// `normal_maps`: shade with `StandardMaterial::normal_map_texture` and the mesh's `ATTRIBUTE_TANGENT` (off by default, as in the
 /// reference, which ignores normal maps).
+/// `bvh_refit_ticks`: up to this many frames in a row that only move entities refit the BVH on the GPU instead of rebuilding it
+/// (0, the default, rebuilds every time, as the reference does).
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
+    pub bvh_refit_ticks: u32,
 }
 
 #[derive(Clone, Debug)]
@@ -87,6 +90,7 @@ impl Plugin for StrollePlugin {
             .unwrap_or_else(|| vec![0]);
         let mut engine = st::Engine::new(&devices).expect("strolle_b200: no usable CUDA device (this engine has no CPU fallback)");
         engine.set_normal_maps(settings.normal_maps).expect("strolle_b200: ST_OPT_NORMAL_MAPS");
+        engine.set_bvh_refit(settings.bvh_refit_ticks).expect("strolle_b200: ST_OPT_BVH_REFIT");
         render_app.insert_resource(EngineResource(engine));
     }
 }

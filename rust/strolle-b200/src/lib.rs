@@ -427,6 +427,12 @@ impl<P: Params> Engine<P> {
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_NORMAL_MAPS, on as c_int) })
     }
 
+    /// Lets up to `ticks` frames in a row that only move instances refit the BVH on the GPU instead of rebuilding it on the host
+    /// (`ST_OPT_BVH_REFIT`; 0, the default, rebuilds every time, as the reference does).  Takes effect with the next frame's scene update.
+    pub fn set_bvh_refit(&mut self, ticks: u32) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_BVH_REFIT, ticks.min(c_int::MAX as u32) as c_int) })
+    }
+
     /// Creates or updates a mesh (`lib.rs:161-164`).
     pub fn insert_mesh(&mut self, handle: P::MeshHandle, item: Mesh) {
         let id = self.meshes.id(handle);

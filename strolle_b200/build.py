@@ -17,6 +17,7 @@ LIB = os.path.join(OUT_DIR, "libstrolle_b200.so")
 # ReSTIR kernels (namespace stf: FMA contraction, approximate div/sqrt, SFU transcendentals; traversal stays bit-exact, st_math.cuh)
 UNITS = [("kernels.cu", "kernels", ["-fmad=false"]),
          ("kernels.cu", "kernels_fast", ["-DST_FAST=1", "-fmad=true", "-prec-div=false", "-prec-sqrt=false"]),
+         ("refit.cu", "refit", ["-fmad=false"]),
          ("engine.cu", "engine", ["-fmad=false"])]
 HEADERS = ["st_math.cuh", "st_device.cuh", "st_types.h", "kernels.h", os.path.join("..", "..", "include", "strolle_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

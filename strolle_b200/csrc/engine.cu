@@ -181,6 +181,13 @@ struct SlotAllocator {
 // ---- BVH: binned SAH build + DFS flatten (strolle/src/bvh/builder.rs, serializer.rs) ---------------------
 struct Prim { uint32_t tri, mat; H3 center; Box box; };
 struct BvhOut { std::vector<float4> buf; int depth = 0; };
+// ST_OPT_BVH_REFIT: what the refit kernels need of a flattened stream.  runs = {parent slot, first leaf entry, entry count, 0} per
+// leaf child; levels[d] = {ptr, parent slot} of every internal node at depth d (the root, which has no parent slot, excluded).
+// A child slot is the float4 index of its lo corner: ptr for the left child, ptr + 2 for the right one.
+struct RefitPlan {
+    std::vector<uint4> runs; std::vector<std::vector<uint2>> levels;
+    void clear() { runs.clear(); levels.clear(); }
+};
 class BvhBuild {
 public:
     static const int kBins = 12;   // builder.rs:15
@@ -228,7 +235,11 @@ public:
             if (rgraft) graft(ri, rdonor); else work.push_back(Item{ri, rdonor});
         }
     }
-    void flatten(const std::vector<uint8_t>& alpha_blend, BvhOut* out) const { out->buf.clear(); out->depth = 0; emit(0, 1, alpha_blend, out); }
+    void flatten(const std::vector<uint8_t>& alpha_blend, BvhOut* out, RefitPlan* plan = nullptr) const {
+        out->buf.clear(); out->depth = 0;
+        if (plan) plan->clear();
+        emit(0, 1, alpha_blend, out, plan);
+    }
 
 private:
     static float comp(H3 v, int a) { return a == 0 ? v.x : (a == 1 ? v.y : v.z); }
@@ -310,14 +321,22 @@ private:
             nodes[pr.dst] = n;
         }
     }
-    uint32_t emit(int id, int depth, const std::vector<uint8_t>& alpha, BvhOut* out) const {   // serializer.rs:20-110
+    void plan_child(RefitPlan* plan, int child, uint32_t ptr, uint32_t slot, int depth) const {
+        const Node& c = nodes[child];
+        if (c.left >= 0) {
+            if ((int)plan->levels.size() <= depth) plan->levels.resize(depth + 1);
+            plan->levels[depth].push_back(make_uint2(ptr, slot));
+        } else plan->runs.push_back(make_uint4(slot, ptr, c.e - c.b, 0u));
+    }
+    uint32_t emit(int id, int depth, const std::vector<uint8_t>& alpha, BvhOut* out, RefitPlan* plan) const {   // serializer.rs:20-110
         uint32_t at = (uint32_t)out->buf.size();
         if (depth > out->depth) out->depth = depth;
         const Node& nd = nodes[id];
         if (nd.left >= 0) {
             out->buf.resize(out->buf.size() + 4, make_float4(0, 0, 0, 0));
-            emit(nd.left, depth + 1, alpha, out);
-            uint32_t rp = emit(nd.right, depth + 1, alpha, out);
+            uint32_t lp = emit(nd.left, depth + 1, alpha, out, plan);
+            uint32_t rp = emit(nd.right, depth + 1, alpha, out, plan);
+            if (plan) { plan_child(plan, nd.left, lp, at, depth + 1); plan_child(plan, nd.right, rp, at + 2, depth + 1); }
             const Box& lb = nodes[nd.left].box; const Box& rb = nodes[nd.right].box;
             out->buf[at] = make_float4(lb.lo.x, lb.lo.y, lb.lo.z, bits2f(0u));
             out->buf[at + 1] = make_float4(lb.hi.x, lb.hi.y, lb.hi.z, bits2f(rp));
@@ -409,7 +428,12 @@ struct st_engine {
     DevMem d_atlas, d_srgb, d_tri_instance, d_instance_xforms;
     bool motion_dirty = true;
     bool moved_last_tick = false;   // an instance was inserted / moved / removed in the tick that prepared the current frame
-    struct Inst { st_handle handle, mesh, material; Affine3 xf, xf_inv, prev_xf; bool dirty; };
+    // baked_mesh / baked_material: what the instance's triangles were last baked from.  host_stale: the last bake ran on the device
+    // (ST_OPT_BVH_REFIT) with dev_xf, so h_triangles / prims still hold an older one until rebake_host.
+    struct Inst {
+        st_handle handle, mesh, material; Affine3 xf, xf_inv, prev_xf; bool dirty;
+        st_handle baked_mesh = ~(st_handle)0, baked_material = ~(st_handle)0; bool host_stale = false; Affine3 dev_xf, dev_xf_inv;
+    };
     std::vector<Inst> instances; bool instances_dirty = false;
     struct Range { st_handle handle; size_t b, e; };
     std::vector<Range> tri_ranges; SlotAllocator tri_alloc;
@@ -445,6 +469,15 @@ struct st_engine {
     // ST_OPT_NORMAL_MAPS: `normal_maps` is the option, `any_normal_map` whether some material has a normal-map rect (set when materials
     // are uploaded), `nmap_frame` their conjunction taken at st_tick: the frame's hit-shading kernels run their NMAP instantiation
     bool normal_maps = false, any_normal_map = false, nmap_frame = false; uint64_t normal_map_launches = 0;
+    // ST_OPT_BVH_REFIT: `bvh_refit` = the option (refit ticks allowed in a row), `refit_run` = refit ticks since the last rebuild.
+    // `structure_changed`: an instance was inserted or removed, or changed mesh or material, since the last tick.  The plan of the
+    // last rebuild (`plan_ready` = taken with the option on and uploaded to d_plan: runs, then nodes deepest level first, split at
+    // `plan_levels`), the alpha flags it was flattened with, the meshes' object-space triangles on the device, and two pinned staging
+    // slots for the bake records + instance transforms (`staging_ev[k]` = slot k's copies done).
+    int bvh_refit = 0; uint32_t refit_run = 0; uint64_t bvh_refits = 0; bool structure_changed = false;
+    RefitPlan plan; bool plan_ready = false; std::vector<uint32_t> plan_levels; std::vector<uint8_t> plan_alpha; DevMem d_plan, d_bake;
+    std::unordered_map<st_handle, DevMem> d_meshes;
+    void* staging[2] = {nullptr, nullptr}; size_t staging_cap[2] = {0, 0}; cudaEvent_t staging_ev[2] = {nullptr, nullptr}; int staging_slot = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -568,6 +601,7 @@ static bool refresh_instances(st_engine* e) {
             p.tri = (uint32_t)(b + i); p.mat = mat_id;
             bake_triangle(tris[i], in.xf, in.xf_inv, &e->h_triangles[9 * (b + i)], &p);
         }
+        in.baked_mesh = in.mesh; in.baked_material = in.material; in.host_stale = false;
         e->triangles_dirty = true;
     }
     return true;
@@ -576,6 +610,122 @@ static bool refresh_instances(st_engine* e) {
 static int upload(st_engine* e, DevMem& d, const void* src, size_t bytes) {
     int rc = d.ensure(bytes); if (rc) return rc;
     if (bytes) CK(cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, e->stream));
+    return ST_OK;
+}
+
+// ---- ST_OPT_BVH_REFIT ------------------------------------------------------------------------------------
+static const st_engine::Range* range_of(const st_engine* e, st_handle inst) {
+    for (const auto& r : e->tri_ranges) if (r.handle == inst) return &r;
+    return nullptr;
+}
+
+// The host mirror of an instance the device baked: the same bake on the host (bit-identical), so that a rebuild sees the primitives
+// it would have seen with the option off.
+static void rebake_host(st_engine* e, st_engine::Inst& in) {
+    if (!in.host_stale) return;
+    in.host_stale = false;
+    auto mesh = e->meshes.find(in.baked_mesh);
+    const st_engine::Range* r = range_of(e, in.handle);
+    if (mesh == e->meshes.end() || !r) return;   // the mesh verbs and st_remove_instance rebake first, so neither happens
+    for (size_t i = 0; i < r->e - r->b; i++) bake_triangle(mesh->second[i], in.dev_xf, in.dev_xf_inv, &e->h_triangles[9 * (r->b + i)], &e->prims[r->b + i]);
+}
+static void rebake_host_mesh(st_engine* e, st_handle mesh) { for (auto& in : e->instances) if (in.host_stale && in.baked_mesh == mesh) rebake_host(e, in); }
+
+static std::vector<uint8_t> alpha_flags(const st_engine* e) {
+    std::vector<uint8_t> alpha(e->materials.size());
+    for (size_t i = 0; i < alpha.size(); i++) alpha[i] = e->materials[i].alpha_blend ? 1 : 0;
+    return alpha;
+}
+
+// A refit tick: the option allows one more, the last rebuild left a plan, and the only instance changes are new transforms of
+// instances that keep the mesh and material their triangles were baked from (and the material table's alpha flags are unchanged).
+static bool refit_qualifies(const st_engine* e) {
+    if (e->bvh_refit <= 0 || (int)e->refit_run >= e->bvh_refit || !e->plan_ready || !e->instances_dirty || e->structure_changed) return false;
+    if (alpha_flags(e) != e->plan_alpha) return false;
+    for (const auto& in : e->instances) {
+        if (!in.dirty) continue;
+        if (in.mesh != in.baked_mesh || in.material != in.baked_material) return false;
+        auto mesh = e->meshes.find(in.mesh);
+        const st_engine::Range* r = range_of(e, in.handle);
+        if (mesh == e->meshes.end() || !r || r->e - r->b != mesh->second.size()) return false;
+        if (std::find(e->material_handles.begin(), e->material_handles.end(), in.material) == e->material_handles.end()) return false;
+    }
+    return true;
+}
+
+static int upload_plan(st_engine* e) {
+    const RefitPlan& p = e->plan;
+    size_t nodes = 0;
+    for (const auto& l : p.levels) nodes += l.size();
+    std::vector<char> blob(p.runs.size() * sizeof(uint4) + nodes * sizeof(uint2));
+    if (!p.runs.empty()) std::memcpy(blob.data(), p.runs.data(), p.runs.size() * sizeof(uint4));
+    e->plan_levels.assign(1, 0u);
+    uint2* dst = (uint2*)(blob.data() + p.runs.size() * sizeof(uint4));
+    for (size_t d = p.levels.size(); d-- > 0;) {   // deepest level first
+        if (p.levels[d].empty()) continue;
+        std::memcpy(dst, p.levels[d].data(), p.levels[d].size() * sizeof(uint2)); dst += p.levels[d].size();
+        e->plan_levels.push_back(e->plan_levels.back() + (uint32_t)p.levels[d].size());
+    }
+    int rc = upload(e, e->d_plan, blob.data(), blob.size()); if (rc) return rc;
+    CK(cudaStreamSynchronize(e->stream));   // `blob` goes out of scope; rebuild ticks synchronise anyway
+    return ST_OK;
+}
+
+// The moved instances' bake records and every instance's velocity-map transforms go through a pinned staging slot, copied on the
+// engine stream; the slot is reused two refit ticks later, after its copies are done.  No stream synchronisation.
+static int refit_tick(st_engine* e, const std::vector<float4>& xf) {
+    std::vector<BakeRecord> recs;
+    uint32_t total = 0;
+    for (auto& in : e->instances) {
+        if (!in.dirty) continue;
+        in.dirty = false;
+        const st_engine::Range* r = range_of(e, in.handle);
+        const std::vector<st_mesh_triangle>& tris = e->meshes[in.mesh];
+        DevMem& dm = e->d_meshes[in.mesh];
+        if (!dm.p) {   // first refit of an instance of this mesh: its object-space triangles go to the device
+            const size_t bytes = std::max<size_t>(tris.size(), 1) * sizeof(st_mesh_triangle);
+            CK(cudaMalloc(&dm.p, bytes)); dm.cap = bytes;
+            if (!tris.empty()) CK(cudaMemcpyAsync(dm.p, tris.data(), tris.size() * sizeof(st_mesh_triangle), cudaMemcpyHostToDevice, e->stream));
+        }
+        BakeRecord rec; std::memset(&rec, 0, sizeof rec);
+        const Affine3& a = in.xf; const Affine3& inv = in.xf_inv;   // bake_triangle's values before its per-vertex loop
+        const float xfv[12] = {a.x.x, a.x.y, a.x.z, a.y.x, a.y.y, a.y.z, a.z.x, a.z.y, a.z.z, a.t.x, a.t.y, a.t.z};
+        const float ntv[9] = {inv.x.x, inv.y.x, inv.z.x, inv.x.y, inv.y.y, inv.z.y, inv.x.z, inv.y.z, inv.z.z};
+        std::memcpy(rec.xf, xfv, sizeof xfv); std::memcpy(rec.nt, ntv, sizeof ntv);
+        const float det = hdot(a.z, hcross(a.x, a.y));
+        rec.sign = (f2bits(det) >> 31) ? -1.0f : 1.0f;
+        rec.b = (uint32_t)r->b; rec.e = (uint32_t)r->e; rec.first = total; rec.tris = (unsigned long long)(uintptr_t)dm.p;
+        total += rec.e - rec.b;
+        recs.push_back(rec);
+        in.host_stale = true; in.dev_xf = in.xf; in.dev_xf_inv = in.xf_inv;
+    }
+    e->instances_dirty = false;
+    const size_t rec_bytes = (recs.size() * sizeof(BakeRecord) + 15) & ~(size_t)15, xf_bytes = xf.size() * sizeof(float4);
+    const int k = e->staging_slot; e->staging_slot ^= 1;
+    if (!e->staging_ev[k]) CK(cudaEventCreateWithFlags(&e->staging_ev[k], cudaEventDisableTiming));
+    else CK(cudaEventSynchronize(e->staging_ev[k]));   // slot k's copies of two refit ticks ago
+    if (e->staging_cap[k] < rec_bytes + xf_bytes) {
+        if (e->staging[k]) CK(cudaFreeHost(e->staging[k]));
+        e->staging[k] = nullptr; e->staging_cap[k] = 0;
+        CK(cudaMallocHost(&e->staging[k], 2 * (rec_bytes + xf_bytes)));
+        e->staging_cap[k] = 2 * (rec_bytes + xf_bytes);
+    }
+    char* s = (char*)e->staging[k];
+    if (!recs.empty()) std::memcpy(s, recs.data(), recs.size() * sizeof(BakeRecord));
+    std::memcpy(s + rec_bytes, xf.data(), xf_bytes);
+    int rc;
+    if ((rc = e->d_bake.ensure(rec_bytes)) || (rc = e->d_instance_xforms.ensure(xf_bytes))) return rc;
+    if (rec_bytes) CK(cudaMemcpyAsync(e->d_bake.p, s, rec_bytes, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(e->d_instance_xforms.p, s + rec_bytes, xf_bytes, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaEventRecord(e->staging_ev[k], e->stream));
+    launch_bake_instances((const BakeRecord*)e->d_bake.p, (uint32_t)recs.size(), total, (float4*)e->d_triangles.p, e->stream);
+    if (!e->bvh_out.buf.empty()) {
+        const uint32_t nruns = (uint32_t)e->plan.runs.size();
+        launch_refit((const uint4*)e->d_plan.p, nruns, (const uint2*)((const char*)e->d_plan.p + nruns * sizeof(uint4)), e->plan_levels.data(),
+                     (int)e->plan_levels.size() - 1, (const float4*)e->d_triangles.p, (float4*)e->d_bvh.p, e->stream);
+    }
+    CK(cudaGetLastError());
+    e->refit_run++; e->bvh_refits++;
     return ST_OK;
 }
 
@@ -1155,8 +1305,10 @@ void st_engine_destroy(st_engine* e) {
     if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
     for (CameraSlot* c : e->cameras) { for (int k = 0; k < 2; k++) { if (c->side[k]) { cudaStreamSynchronize(c->side[k]); cudaStreamDestroy(c->side[k]); } if (c->ev_pushed[k]) cudaEventDestroy(c->ev_pushed[k]); } if (c->ev_produced) cudaEventDestroy(c->ev_produced);
         c->arena.release(); c->svgf_pairs.release(); c->rgba8.release(); for (int k = 0; k < 2; k++) { if (c->ev_ready[k]) cudaEventDestroy(c->ev_ready[k]); if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]); } delete c; }
-    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors};
+    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake};
     for (DevMem* d : all) d->release();
+    for (auto& m : e->d_meshes) m.second.release();
+    for (int k = 0; k < 2; k++) { if (e->staging[k]) cudaFreeHost(e->staging[k]); if (e->staging_ev[k]) cudaEventDestroy(e->staging_ev[k]); }
     for (auto& t : e->pending) { cudaEventDestroy(t.a); cudaEventDestroy(t.b); }
     for (cudaEvent_t ev : e->event_pool) cudaEventDestroy(ev);
     if (e->comm) g_nccl.CommDestroy(e->comm);
@@ -1167,10 +1319,20 @@ void st_engine_destroy(st_engine* e) {
 
 int st_insert_mesh(st_engine* e, st_handle mesh, const st_mesh_triangle* tris, size_t count) {
     if (!e || (!tris && count)) return fail(ST_ERR_INVALID, "null argument");
+    rebake_host_mesh(e, mesh);   // device-baked instances of the old triangles: their host mirror from the old ones
+    auto dm = e->d_meshes.find(mesh);
+    if (dm != e->d_meshes.end()) { cudaSetDevice(e->device); dm->second.release(); e->d_meshes.erase(dm); }   // uploaded again at the next refit that needs it
     e->meshes[mesh].assign(tris, tris + count);
     return ST_OK;
 }
-int st_remove_mesh(st_engine* e, st_handle mesh) { if (!e) return fail(ST_ERR_INVALID, "null engine"); e->meshes.erase(mesh); return ST_OK; }
+int st_remove_mesh(st_engine* e, st_handle mesh) {
+    if (!e) return fail(ST_ERR_INVALID, "null engine");
+    rebake_host_mesh(e, mesh);
+    auto dm = e->d_meshes.find(mesh);
+    if (dm != e->d_meshes.end()) { cudaSetDevice(e->device); dm->second.release(); e->d_meshes.erase(dm); }
+    e->meshes.erase(mesh);
+    return ST_OK;
+}
 
 int st_insert_material(st_engine* e, st_handle h, const st_material* m) {   // Materials::insert (materials.rs:36-55)
     if (!e || !m) return fail(ST_ERR_INVALID, "null argument");
@@ -1232,13 +1394,18 @@ int st_set_material_textures(st_engine* e, st_handle material, const st_material
 int st_insert_instance(st_engine* e, st_handle h, st_handle mesh, st_handle material, const float a[12]) {   // Instances::insert (instances.rs:29-50)
     if (!e || !a) return fail(ST_ERR_INVALID, "null argument");
     Affine3 xf; xf.x = h3(a[0], a[1], a[2]); xf.y = h3(a[3], a[4], a[5]); xf.z = h3(a[6], a[7], a[8]); xf.t = h3(a[9], a[10], a[11]);
-    for (auto& in : e->instances) if (in.handle == h) { in.prev_xf = in.xf; in.mesh = mesh; in.material = material; in.xf = xf; in.xf_inv = aff_inverse(xf); in.dirty = true; e->instances_dirty = true; e->motion_dirty = true; return ST_OK; }
+    for (auto& in : e->instances) if (in.handle == h) {
+        if (in.mesh != mesh || in.material != material) e->structure_changed = true;
+        in.prev_xf = in.xf; in.mesh = mesh; in.material = material; in.xf = xf; in.xf_inv = aff_inverse(xf); in.dirty = true; e->instances_dirty = true; e->motion_dirty = true; return ST_OK;
+    }
     st_engine::Inst in; in.handle = h; in.mesh = mesh; in.material = material; in.xf = xf; in.xf_inv = aff_inverse(xf); in.prev_xf = xf; in.dirty = true;
-    e->instances.push_back(in); e->instances_dirty = true; e->motion_dirty = true;
+    e->instances.push_back(in); e->instances_dirty = true; e->motion_dirty = true; e->structure_changed = true;
     return ST_OK;
 }
 int st_remove_instance(st_engine* e, st_handle h) {   // Engine::remove_instance (lib.rs:226-229)
     if (!e) return fail(ST_ERR_INVALID, "null engine");
+    for (auto& in : e->instances) if (in.handle == h) rebake_host(e, in);   // its freed triangle slots keep the option-off bytes
+    e->structure_changed = true;
     size_t before = e->instances.size();
     e->instances.erase(std::remove_if(e->instances.begin(), e->instances.end(), [&](const st_engine::Inst& i) { return i.handle == h; }), e->instances.end());
     if (e->instances.size() != before) e->instances_dirty = true;
@@ -1371,21 +1538,8 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
         if ((rc = e->d_matpacked.ensure(e->h_materials.size() * 4))) return rc;
         launch_material_derive((const GpuMaterial*)e->d_materials.p, (uint32_t)e->h_materials.size(), (uint32_t*)e->d_matpacked.p, e->stream);
     }
-    if (refresh_instances(e)) {   // Bvh::refresh (bvh.rs:48-70)
-        e->bvh.build(e->prims, e->bvh_reuse);
-        std::vector<uint8_t> alpha(e->materials.size());
-        for (size_t i = 0; i < alpha.size(); i++) alpha[i] = e->materials[i].alpha_blend ? 1 : 0;
-        e->bvh.flatten(alpha, &e->bvh_out);
-        // A tree deeper than the traversal stack cannot be walked (the reference silently corrupts a neighbour's stack,
-        // strolle-gpu/src/lib.rs:72-76).  The tick still completes — with an EMPTY tree, so that the device never pairs the
-        // new triangles with the old BVH — and reports ST_ERR_LIMIT at its end; nothing is drawn until the scene changes.
-        if (e->bvh_out.depth - 1 > 24) { e->bvh_out.buf.clear(); too_deep = true; }
-        if ((rc = upload(e, e->d_bvh, e->bvh_out.buf.data(), e->bvh_out.buf.size() * 16))) return rc;
-    }
-    e->moved_last_tick = e->motion_dirty;
-    if (e->motion_dirty) {   // per-instance curr_xform_inv / prev_transform for the velocity map (passes/prim_raster.rs:198-223)
-        e->motion_dirty = false;
-        std::vector<uint32_t> tri_inst(e->h_triangles.size() / 9, 0u);
+    // per-instance curr_xform_inv / prev_transform for the velocity map (passes/prim_raster.rs:198-223)
+    auto instance_xforms = [&]() {
         std::vector<float4> xf(6 * std::max<size_t>(e->instances.size(), 1), make_float4(0, 0, 0, 0));
         for (size_t k = 0; k < e->instances.size(); k++) {
             const st_engine::Inst& in = e->instances[k];
@@ -1395,8 +1549,38 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
                 xf[6 * k + 3 * j + 1] = make_float4(a[j]->y.x, a[j]->y.y, a[j]->y.z, a[j]->t.y);
                 xf[6 * k + 3 * j + 2] = make_float4(a[j]->z.x, a[j]->z.y, a[j]->z.z, a[j]->t.z);
             }
-            for (const auto& r : e->tri_ranges) if (r.handle == in.handle) for (size_t t = r.b; t < r.e; t++) tri_inst[t] = (uint32_t)k;
         }
+        return xf;
+    };
+    const bool refit = refit_qualifies(e);
+    e->structure_changed = false;
+    if (refit) {   // ST_OPT_BVH_REFIT: device bake + refit over the last rebuild's topology
+        e->moved_last_tick = true;
+        e->motion_dirty = false;
+        if ((rc = refit_tick(e, instance_xforms()))) return rc;
+    } else {
+        if (e->instances_dirty) for (auto& in : e->instances) rebake_host(e, in);   // the rebuild below sees the option-off primitives
+        if (refresh_instances(e)) {   // Bvh::refresh (bvh.rs:48-70)
+            e->bvh.build(e->prims, e->bvh_reuse);
+            std::vector<uint8_t> alpha = alpha_flags(e);
+            e->bvh.flatten(alpha, &e->bvh_out, e->bvh_refit > 0 ? &e->plan : nullptr);
+            // A tree deeper than the traversal stack cannot be walked (the reference silently corrupts a neighbour's stack,
+            // strolle-gpu/src/lib.rs:72-76).  The tick still completes — with an EMPTY tree, so that the device never pairs the
+            // new triangles with the old BVH — and reports ST_ERR_LIMIT at its end; nothing is drawn until the scene changes.
+            if (e->bvh_out.depth - 1 > 24) { e->bvh_out.buf.clear(); too_deep = true; }
+            if ((rc = upload(e, e->d_bvh, e->bvh_out.buf.data(), e->bvh_out.buf.size() * 16))) return rc;
+            e->refit_run = 0;
+            e->plan_ready = e->bvh_refit > 0 && !too_deep;   // a tree rejected as too deep is never refit
+            if (e->plan_ready) { e->plan_alpha = alpha; if ((rc = upload_plan(e))) return rc; }
+        }
+        e->moved_last_tick = e->motion_dirty;
+    }
+    if (e->motion_dirty) {
+        e->motion_dirty = false;
+        std::vector<uint32_t> tri_inst(e->h_triangles.size() / 9, 0u);
+        std::vector<float4> xf = instance_xforms();
+        for (size_t k = 0; k < e->instances.size(); k++)
+            for (const auto& r : e->tri_ranges) if (r.handle == e->instances[k].handle) for (size_t t = r.b; t < r.e; t++) tri_inst[t] = (uint32_t)k;
         if ((rc = upload(e, e->d_tri_instance, tri_inst.data(), tri_inst.size() * 4))) return rc;
         if ((rc = upload(e, e->d_instance_xforms, xf.data(), xf.size() * 16))) return rc;
         CK(cudaStreamSynchronize(e->stream));   // host staging vectors go out of scope
@@ -1599,6 +1783,7 @@ int st_set_option(st_engine* e, int option, int value) {
     if (option == ST_OPT_FUSE_REPROJECT) { e->fuse_reproject = value != 0; return ST_OK; }
     if (option == ST_OPT_WAVELET_TILE_CFG) { e->wavelet_cfg = value & 0xfffff; return ST_OK; }
     if (option == ST_OPT_NORMAL_MAPS) { e->normal_maps = value != 0; return ST_OK; }   // takes effect at the next st_tick
+    if (option == ST_OPT_BVH_REFIT) { if (value < 0) return fail(ST_ERR_INVALID, "ST_OPT_BVH_REFIT: 0 or a positive budget"); e->bvh_refit = value; return ST_OK; }
     return fail(ST_ERR_INVALID, "unknown option");
 }
 // ---- host-side BVH builder without a device (test / tool hook; strolle/src/bvh/builder.rs, serializer.rs) ----
@@ -1640,6 +1825,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_VARIANCE_TILED_LAUNCHES) { *value = e->variance_tiled_launches; return ST_OK; }
     if (stat == ST_STAT_BVH_GRAFTED_SUBTREES) { *value = e->bvh.grafted; return ST_OK; }
     if (stat == ST_STAT_NORMAL_MAP_LAUNCHES) { *value = e->normal_map_launches; return ST_OK; }
+    if (stat == ST_STAT_BVH_REFITS) { *value = e->bvh_refits; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
         CK(cudaSetDevice(e->device)); CK(cudaStreamSynchronize(e->stream));
         uint64_t total = 0;

@@ -84,6 +84,15 @@ void launch_strip_signal_wait(const StripSync& s, int sig_slot, u32 seq, u32 dst
 void launch_strip_pull(const StripPull& p, cudaStream_t st);
 void launch_atm_sun_color(float4* out2, const GpuWorld& world, cudaStream_t st);
 
+// ST_OPT_BVH_REFIT (refit.cu).  One record per moved instance: its affine (x, y, z columns then translation), the transpose of the
+// inverse's 3x3 (columns), the determinant's sign, its triangle range [b, e) in the triangle array, `first` = the thread index of
+// its first triangle (prefix sum of the ranges), `tris` = its mesh's object-space st_mesh_triangles on the device.
+struct BakeRecord { float xf[12]; float nt[9]; float sign; u32 b, e, first, pad; unsigned long long tris; };
+void launch_bake_instances(const BakeRecord* recs, u32 nrec, u32 total, float4* triangles, cudaStream_t st);
+// runs: {parent slot, first leaf entry, entry count, 0}; nodes: {ptr, parent slot} of every internal node but the root, grouped by level
+// (deepest first, level l = [level_begin[l], level_begin[l + 1]))
+void launch_refit(const uint4* runs, u32 nruns, const uint2* nodes, const u32* level_begin, int levels, const float4* triangles, float4* bvh, cudaStream_t st);
+
 }  // namespace st
 
 // The ReSTIR kernels K5-K19 built a second time with FMA contraction and SFU approximations (kernels.cu compiled with

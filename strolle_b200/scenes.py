@@ -283,6 +283,87 @@ def demo_level(width=1920, height=1080, mode=MODE_IMAGE, denoise=True, textures=
                 images=images, material_textures=material_textures)
 
 
+DEMO_TORI = (6000, 6001, 6002)   # demo_level's torus instances
+_DEMO_TORUS_AT = [(-0.5, 0.33, -5.5), (-11.0, 0.33, 28.0), (-11.5, 0.33, 13.5)]
+
+
+def _quat_mul(a, b):
+    (aw, ax, ay, az), (bw, bx, by, bz) = a, b
+    return (aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+            aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw)
+
+
+def _affine_trs(q, scale, t):
+    """Transform::from_translation(t).with_rotation(q).with_scale(scale) as 12 floats (matrix columns x, y, z, translation)."""
+    w, x, y, z = q
+    cols = [(1 - 2 * (y * y + z * z), 2 * (x * y + w * z), 2 * (x * z - w * y)),
+            (2 * (x * y - w * z), 1 - 2 * (x * x + z * z), 2 * (y * z + w * x)),
+            (2 * (x * z + w * y), 2 * (y * z - w * x), 1 - 2 * (x * x + y * y))]
+    return np.array([c * s for col, s in zip(cols, scale) for c in col] + list(t), np.float32)
+
+
+def demo_level_animated(t):
+    """The tori of demo_level at time `t` (seconds) as bevy-strolle/examples/demo.rs `animate_toruses` turns them:
+    rotation = Quat::from_rotation_z(t) * Quat::from_rotation_x(t + 1), scale 0.5, translation unchanged.  Returns
+    (instance, mesh, material, affine12) tuples to re-insert; every other instance of demo_level stays where it is."""
+    rz = (math.cos(0.5 * t), 0.0, 0.0, math.sin(0.5 * t))
+    rx = (math.cos(0.5 * (t + 1.0)), math.sin(0.5 * (t + 1.0)), 0.0, 0.0)
+    q = _quat_mul(rz, rx)
+    return [(h, 2000, 160 + k, _affine_trs(q, (0.5, 0.5, 0.5), at)) for k, (h, at) in enumerate(zip(DEMO_TORI, _DEMO_TORUS_AT))]
+
+
+def _icosphere(subdivisions=1):
+    """A unit icosphere (20 * 4^subdivisions triangles, flat-free vertex normals = positions)."""
+    p = (1 + 5 ** 0.5) / 2
+    v = [np.array(a, np.float64) for a in ((-1, p, 0), (1, p, 0), (-1, -p, 0), (1, -p, 0), (0, -1, p), (0, 1, p), (0, -1, -p), (0, 1, -p),
+                                            (p, 0, -1), (p, 0, 1), (-p, 0, -1), (-p, 0, 1))]
+    v = [a / np.linalg.norm(a) for a in v]
+    faces = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2), (10, 7, 6), (7, 1, 8),
+             (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11), (6, 2, 10), (8, 6, 7), (9, 8, 1)]
+    tris = [tuple(v[i] for i in f) for f in faces]
+    for _ in range(subdivisions):
+        nxt = []
+        for a, b, c in tris:
+            ab, bc, ca = [m / np.linalg.norm(m) for m in ((a + b) / 2, (b + c) / 2, (c + a) / 2)]
+            nxt += [(a, ab, ca), (b, bc, ab), (c, ca, bc), (ab, bc, ca)]
+        tris = nxt
+    return [tri36([a, b, c], [a, b, c]) for a, b, c in tris]
+
+
+STRESS_FLOOR = 7000   # stress_bvh's floor instance; its objects are 7001 .. 7000 + n
+
+
+def stress_bvh_instances(n, t):
+    """The `n` objects of stress_bvh at time `t`: object k (a unit box for even k, an icosphere of radius 0.5 for odd k) circles
+    its own spot on the floor, bounces and tumbles on a scripted path (no physics, fully deterministic)."""
+    out = []
+    for k in range(n):
+        r = 3.0 + 40.0 * ((k * 0.6180339887) % 1.0)
+        a0 = 2.0 * math.pi * ((k * 0.7548776662) % 1.0)
+        a = a0 + 0.3 * t / (1.0 + 0.05 * r)
+        y = 1.0 + 0.5 * (k % 7) + 2.0 * abs(math.sin(1.3 * t + k))
+        spin = 0.9 * t + k
+        q = _quat_mul((math.cos(0.5 * spin), 0.0, math.sin(0.5 * spin), 0.0), (math.cos(0.25 * spin), math.sin(0.25 * spin), 0.0, 0.0))
+        s = 1.0 if k % 2 == 0 else 0.5
+        out.append((STRESS_FLOOR + 1 + k, 201 if k % 2 == 0 else 202, 101 + k % 3, _affine_trs(q, (s, s, s), (r * math.cos(a), y, r * math.sin(a)))))
+    return out
+
+
+def stress_bvh(n=2000, width=1920, height=1080, mode=MODE_IMAGE, denoise=True, t=0.0):
+    """A scene shaped like bevy-strolle/examples/stress-bvh.rs: a 100 x 1 x 100 floor box and `n` unit boxes and icospheres
+    (20 triangles, where the example's shape::Icosphere::default() has 20480) that move every tick along the
+    scripted paths of stress_bvh_instances instead of the example's physics."""
+    meshes = {200: np.stack(_box((-50.0, -1.0, -50.0), (50.0, 0.0, 50.0))), 201: np.stack(_box((-0.5, -0.5, -0.5), (0.5, 0.5, 0.5))),
+              202: np.stack(_icosphere(0))}
+    materials = {100: (material((0.6, 0.6, 0.6, 1.0)), False), 101: (material((0.8, 0.3, 0.2, 1.0)), False),
+                 102: (material((0.2, 0.5, 0.8, 1.0)), False), 103: (material((0.3, 0.7, 0.3, 1.0), perceptual_roughness=0.5), False)}
+    instances = [(STRESS_FLOOR, 200, 100, IDENTITY_AFFINE)] + stress_bvh_instances(n, t)
+    lights = [(400, LIGHT_POINT, point_light((0.0, 12.0, 0.0), 0.3, (400.0, 400.0, 400.0), 60.0))]
+    cam = dict(mode=mode, denoise=denoise, ref_depth=1, w=width, h=height, transform=look_at_transform((0.0, 22.0, 48.0), (0.0, 0.0, 0.0)),
+               projection=perspective_infinite_reverse_rh(math.pi / 4.0, width / height, 0.1))
+    return dict(name="stress_bvh", meshes=meshes, materials=materials, instances=instances, lights=lights, sun=(1.0, 0.6), camera=cam)
+
+
 def _quad(p0, p1, p2, p3, normal, uv_lo=(0.0, 0.0), uv_hi=(1.0, 1.0), tangents=None):
     """Two triangles wound so that the geometric normal agrees with `normal` (Triangle::hit flips the shading normal by
     the sign of the determinant, strolle-gpu/src/triangle.rs:95-101, i.e. it trusts the winding).  `tangents`: one
