@@ -145,7 +145,10 @@ int st_set_blue_noise(st_engine* e, const uint8_t* rgba8_256x256);
  * *count; copies min(cap, count). */
 int st_read_buffer(st_engine* e, st_camera_handle camera, const char* name, float* dst, size_t cap_floats, size_t* count);
 /* Scene buffers as uploaded: "triangles", "bvh", "materials", "lights", "world", "transmittance_lut",
- * "scattering_lut", "sky_lut". */
+ * "scattering_lut", "sky_lut"; and, while ST_OPT_LIGHT_GRID is on and a tick has built it, "light_grid" as 32-bit words: a 21-word
+ * header {dims x, y, z, K = 64, light_count, cells, lo[3], cell[3], inv_cell[3], band[3], margin[3]} (the last 15 are f32 bits), the
+ * count of every cell then of the outside list (0xffffffff = overflow: every slot), then K slots per cell and K for the outside list
+ * (0xffffffff past the count).  Cell (x, y, z) is index (z dims.y + y) dims.x + x. */
 int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap_floats, size_t* count);
 int st_bvh_depth(st_engine* e, int* depth);
 uint32_t st_frame(st_engine* e);
@@ -173,7 +176,18 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16 };
+/* ST_OPT_LIGHT_GRID (default 0 = off; 1..64, anything else is ST_ERR_INVALID): the light candidates of ReSTIR DI sampling, of the GI
+ * bounce's next-event estimate and of Reference mode are drawn uniformly from a per-cell list of the light slots that can reach the
+ * point's cell, instead of from every slot.  N is the cell count along the longest axis of the grid box, the AABB of the range spheres of
+ * the cullable lights (point lights with a finite position and colour and a range in [2^-60, 2^60]); the other axes get
+ * max(1, ceil(N extent / longest)) cells.  A list holds, in ascending slot order, every non-cullable slot (the sun, spot lights, empty
+ * slots) and every cullable light within range of the cell box grown by cell/64 + 8 ulp; outside the box a point samples the
+ * non-cullable slots, and a non-finite point or a cell with more than 64 entries samples every slot, as with 0.  A dropped light's
+ * radiance at any point of the cell is exactly zero, so the estimates stay unbiased: only the candidate count M and the noise change.
+ * The lists are rebuilt on the device at st_tick whenever the lights were uploaded or the option changed (ST_STAT_LIGHT_GRID_BUILDS);
+ * st_read_scene("light_grid") returns them.  The reference samples every slot, so the default keeps parity with it.  Takes effect at
+ * the next st_tick (DESIGN.md §2). */
 /* ST_OPT_BVH_REFIT (default 0): N > 0 allows up to N refit ticks in a row.  A refit tick is an st_tick whose only scene change is new
  * transforms of existing instances (same mesh, same material, nothing inserted or removed, no material's alpha mode changed): the moved
  * instances' triangles are baked on the device (bit-identical to the host bake) and the BVH boxes are recomputed bottom-up on the device
@@ -251,7 +265,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_STRIP_PULLED_ROWS = 5 /* rows x buffers fetched from other ranks by the temporal pull since linking */, ST_STAT_LAST_FRAME_FUSED_STRIPS = 6 /* 1 = the last strip frame used the fused transport */,
        ST_STAT_STRIP_FIRST_TIMEOUT = 7 /* 0, or 0x80000000 | slot << 16 | awaited rank << 8 | sequence & 0xff of the first strip flag wait that gave up */,
        ST_STAT_NORMAL_MAP_LAUNCHES = 8 /* launches of the normal-mapped kernel variants (ST_OPT_NORMAL_MAPS) since creation */,
-       ST_STAT_BVH_REFITS = 9 /* refit ticks (ST_OPT_BVH_REFIT) since creation */ };
+       ST_STAT_BVH_REFITS = 9 /* refit ticks (ST_OPT_BVH_REFIT) since creation */,
+       ST_STAT_LIGHT_GRID_BUILDS = 10 /* light grid builds (ST_OPT_LIGHT_GRID) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,

@@ -45,10 +45,13 @@ pub struct StrolleSun {
 /// reference, which ignores normal maps).
 /// `bvh_refit_ticks`: up to this many frames in a row that only move entities refit the BVH on the GPU instead of rebuilding it
 /// (0, the default, rebuilds every time, as the reference does).
+/// `light_grid`: sample light candidates from a grid of the point lights that can reach each cell, this many cells along its
+/// longest axis (1..=64; 0, the default, samples every light, as the reference does) - for scenes with many short-range lights.
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
     pub bvh_refit_ticks: u32,
+    pub light_grid: u32,
 }
 
 #[derive(Clone, Debug)]
@@ -91,6 +94,7 @@ impl Plugin for StrollePlugin {
         let mut engine = st::Engine::new(&devices).expect("strolle_b200: no usable CUDA device (this engine has no CPU fallback)");
         engine.set_normal_maps(settings.normal_maps).expect("strolle_b200: ST_OPT_NORMAL_MAPS");
         engine.set_bvh_refit(settings.bvh_refit_ticks).expect("strolle_b200: ST_OPT_BVH_REFIT");
+        engine.set_light_grid(settings.light_grid).expect("strolle_b200: ST_OPT_LIGHT_GRID");
         render_app.insert_resource(EngineResource(engine));
     }
 }

@@ -433,6 +433,13 @@ impl<P: Params> Engine<P> {
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_BVH_REFIT, ticks.min(c_int::MAX as u32) as c_int) })
     }
 
+    /// Draws the light candidates from a world-space grid of the lights that can reach each cell, `cells` cells along its longest
+    /// axis (`ST_OPT_LIGHT_GRID`, 1..=64; 0, the default, draws from every light, as the reference does).  Takes effect with the next
+    /// frame's scene update.
+    pub fn set_light_grid(&mut self, cells: u32) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_LIGHT_GRID, cells.min(c_int::MAX as u32) as c_int) })
+    }
+
     /// Creates or updates a mesh (`lib.rs:161-164`).
     pub fn insert_mesh(&mut self, handle: P::MeshHandle, item: Mesh) {
         let id = self.meshes.id(handle);

@@ -478,6 +478,10 @@ struct st_engine {
     RefitPlan plan; bool plan_ready = false; std::vector<uint32_t> plan_levels; std::vector<uint8_t> plan_alpha; DevMem d_plan, d_bake;
     std::unordered_map<st_handle, DevMem> d_meshes;
     void* staging[2] = {nullptr, nullptr}; size_t staging_cap[2] = {0, 0}; cudaEvent_t staging_ev[2] = {nullptr, nullptr}; int staging_slot = 0;
+    // ST_OPT_LIGHT_GRID: `light_grid` = the option (cells along the longest axis, 0 = off), `lgrid_built` = the option value the grid
+    // on the device was built for (0 = none, or stale), `lgrid` = its header with the pointers into d_lgrid, `lgrid_frame` = the
+    // frame's candidate-sampling kernels run their LGRID instantiation (taken at st_tick)
+    int light_grid = 0, lgrid_built = 0; bool lgrid_frame = false; LightGridDev lgrid{}; DevMem d_lgrid; uint64_t light_grid_builds = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -530,6 +534,56 @@ static void light_overwrite(st_engine* e, uint32_t slot, st_handle h, GpuLight n
     nl.prev_d0 = old.d0; nl.prev_d1 = old.d1; nl.prev_d2 = old.d2;
     uniq_add(e->lights_updated, h);
     e->h_lights[slot] = nl; e->lights_dirty = true;
+}
+
+// ---- ST_OPT_LIGHT_GRID (DESIGN.md §2 "Light grid") --------------------------------------------------------------------------
+// lgrid_cullable (st_device.cuh) on the host: a point light with a finite position and colour and 2^-60 <= range <= 2^60
+static bool lgrid_cullable_host(const GpuLight& l) {
+    const float big = 0x1p60f, tiny = 0x1p-60f;
+    uint32_t kind; std::memcpy(&kind, &l.d2.x, 4);
+    if (kind != 1u) return false;
+    if (!(std::fabs(l.d0.x) <= big && std::fabs(l.d0.y) <= big && std::fabs(l.d0.z) <= big)) return false;
+    if (!(std::isfinite(l.d1.x) && std::isfinite(l.d1.y) && std::isfinite(l.d1.z))) return false;
+    return l.d1.w >= tiny && l.d1.w <= big;
+}
+// The grid's box, dims, cell size, margins and index bands, in f32 in this operation order (oracle_lightgrid restates it).  No
+// cullable light: dims 0, only the outside list.
+static LightGridDev light_grid_header(const std::vector<GpuLight>& lights, uint32_t light_count, int n) {
+    LightGridDev g; std::memset(&g, 0, sizeof g);
+    g.light_count = light_count;
+    const float inf = std::numeric_limits<float>::infinity();
+    float lo[3] = {inf, inf, inf}, hi[3] = {-inf, -inf, -inf};
+    bool any = false;
+    for (uint32_t i = 0; i < light_count && i < lights.size(); i++) {
+        const GpuLight& l = lights[i];
+        if (!lgrid_cullable_host(l)) continue;
+        any = true;
+        const float c[3] = {l.d0.x, l.d0.y, l.d0.z}, r = l.d1.w;
+        for (int a = 0; a < 3; a++) { lo[a] = std::min(lo[a], c[a] - r); hi[a] = std::max(hi[a], c[a] + r); }
+    }
+    if (!any) return g;
+    float ext[3], longest = 0.0f, m = 0.0f;
+    for (int a = 0; a < 3; a++) { ext[a] = hi[a] - lo[a]; longest = std::max(longest, ext[a]); m = std::max(m, std::max(std::fabs(lo[a]), std::fabs(hi[a]))); }
+    const float ulp = std::nextafter(m, inf) - m;   // spacing of the largest bound coordinate
+    for (int a = 0; a < 3; a++) {
+        const float q = std::ceil(((float)n * ext[a]) / longest);
+        const uint32_t d = q < 1.0f ? 1u : (q > (float)n ? (uint32_t)n : (uint32_t)q);
+        g.dims[a] = d; g.lo[a] = lo[a];
+        g.cell[a] = ext[a] / (float)d; g.inv_cell[a] = (float)d / ext[a];
+        g.margin[a] = g.cell[a] * 0.015625f + 8.0f * ulp;                // cell / 64 + 8 ulp
+        g.band[a] = 0.0078125f + (2.0f * ulp) * g.inv_cell[a];           // 1/128 cell + 2 ulp, in cells
+    }
+    return g;
+}
+static int build_light_grid(st_engine* e) {
+    LightGridDev g = light_grid_header(e->h_lights, e->world.light_count, e->light_grid);
+    const size_t cells = (size_t)g.dims[0] * g.dims[1] * g.dims[2] + 1;   // + the outside list
+    const size_t count_words = (cells + 3) & ~(size_t)3;
+    int rc = e->d_lgrid.ensure((count_words + cells * kLightGridK) * 4); if (rc) return rc;
+    g.counts = (const uint32_t*)e->d_lgrid.p; g.lists = g.counts + count_words;
+    launch_light_grid_build(g, (const GpuLight*)e->d_lights.p, e->stream);
+    e->lgrid = g; e->lgrid_built = e->light_grid; e->light_grid_builds++;
+    return ST_OK;
 }
 
 static float2 oct_encode_host(H3 n) {   // strolle-gpu/src/normal.rs:9-23 (spot light direction)
@@ -812,6 +866,8 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     const st_camera& d = cs->desc;
     const bool fs = e->shading_fast;   // ReSTIR kernels from the fast-shading build (ST_OPT_SHADING_FAST_MATH)
     const bool nm = e->nmap_frame;     // normal-mapped shading normals (ST_OPT_NORMAL_MAPS)
+    const bool lgon = e->lgrid_frame;  // light-grid candidate lists (ST_OPT_LIGHT_GRID)
+    const LightGridDev lgd = e->lgrid;
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
     auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
@@ -825,9 +881,9 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         for (uint32_t depth = 0; depth <= (uint32_t)d.ref_depth; depth++) {
             uint32_t sd = seed(P_REF_SHADING_SEED + depth);
             add(P_REF_TRACING, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_ref_tracing(cam, sc, depth, nm, s); });
-            add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, sd, depth, s); });
+            add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, sd, depth, lgon ? &lgd : nullptr, s); });
         }
-        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, s); });
+        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, s); });
         add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, 6u, di_final, gi_final, s); });
         return;
     }
@@ -845,10 +901,10 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         if (needs_di) {
             uint32_t s1 = seed(P_DI_SAMPLING), s2 = seed(P_DI_TEMPORAL), s3 = seed(P_DI_SPATIAL_PICK), s5 = seed(P_DI_SPATIAL_SAMPLE);
             if (fp) {
-                add(P_DI_TEMPORAL, [=](cudaStream_t s) { (fs ? stf::launch_di_sample_temporal : st::launch_di_sample_temporal)(cam, sc, cur, s1, s2, f, s); });
+                add(P_DI_TEMPORAL, [=](cudaStream_t s) { (fs ? stf::launch_di_sample_temporal : st::launch_di_sample_temporal)(cam, sc, cur, s1, s2, f, lgon ? &lgd : nullptr, s); });
                 add(P_DI_SPATIAL_PICK, [=](cudaStream_t s) { (fs ? stf::launch_di_spatial_fused : st::launch_di_spatial_fused)(cam, sc, cur, s3, s5, f, s); });
             } else {
-                add(P_DI_SAMPLING, [=](cudaStream_t s) { (fs ? stf::launch_di_sampling : st::launch_di_sampling)(cam, sc, cur, s1, f, s); });
+                add(P_DI_SAMPLING, [=](cudaStream_t s) { (fs ? stf::launch_di_sampling : st::launch_di_sampling)(cam, sc, cur, s1, f, lgon ? &lgd : nullptr, s); });
                 add(P_DI_TEMPORAL, [=](cudaStream_t s) { (fs ? stf::launch_di_temporal : st::launch_di_temporal)(cam, sc, cur, s2, s); });
                 add(P_DI_SPATIAL_PICK, [=](cudaStream_t s) { (fs ? stf::launch_di_spatial_pick : st::launch_di_spatial_pick)(cam, sc, cur, s3, f, s); });
                 add(P_DI_SPATIAL_TRACE, [=](cudaStream_t s) { (fs ? stf::launch_spatial_trace : st::launch_spatial_trace)(cam, sc, cam.di_diff_samples, cam.di_diff_curr_colors, cam.di_diff_stash, s); });
@@ -863,9 +919,9 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
             const int inline_rp = (fp && tracing) ? 1 : 0;   // K11 inside K14; validation frames keep K11 (K12 / K13 read its output)
             if (!inline_rp) add(P_GI_REPROJECTION, [=](cudaStream_t s) { (fs ? stf::launch_gi_reprojection : st::launch_gi_reprojection)(cam, sc, cur, s); });
             auto sampling = [&]() {
-                if (fp) { add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, nm, s); }); return; }
+                if (fp) { add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, nm, lgon ? &lgd : nullptr, s); }); return; }
                 add(P_GI_SAMPLING_A, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, nm, s); });
-                add(P_GI_SAMPLING_B, [=](cudaStream_t s) { (fs ? stf::launch_gi_sampling_b : st::launch_gi_sampling_b)(cam, sc, cur, sb, f, s); });
+                add(P_GI_SAMPLING_B, [=](cudaStream_t s) { (fs ? stf::launch_gi_sampling_b : st::launch_gi_sampling_b)(cam, sc, cur, sb, f, lgon ? &lgd : nullptr, s); });
             };
             if (tracing) {
                 if (f % 2u == 0u) sampling();
@@ -1305,7 +1361,7 @@ void st_engine_destroy(st_engine* e) {
     if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
     for (CameraSlot* c : e->cameras) { for (int k = 0; k < 2; k++) { if (c->side[k]) { cudaStreamSynchronize(c->side[k]); cudaStreamDestroy(c->side[k]); } if (c->ev_pushed[k]) cudaEventDestroy(c->ev_pushed[k]); } if (c->ev_produced) cudaEventDestroy(c->ev_produced);
         c->arena.release(); c->svgf_pairs.release(); c->rgba8.release(); for (int k = 0; k < 2; k++) { if (c->ev_ready[k]) cudaEventDestroy(c->ev_ready[k]); if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]); } delete c; }
-    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake};
+    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake, &e->d_lgrid};
     for (DevMem* d : all) d->release();
     for (auto& m : e->d_meshes) m.second.release();
     for (int k = 0; k < 2; k++) { if (e->staging[k]) cudaFreeHost(e->staging[k]); if (e->staging_ev[k]) cudaEventDestroy(e->staging_ev[k]); }
@@ -1596,6 +1652,7 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
         CK(cudaStreamSynchronize(e->stream));
         light_overwrite(e, 0, st_engine::kSun, make_sun(sun[0], sun[1]));
     }
+    const bool lights_uploaded = e->lights_dirty;
     if (e->lights_dirty) {   // Lights::flush (lights.rs:133-162)
         for (uint32_t id : e->lights_killed) e->h_lights[id].d3.x = bits2f(0xcafebabeu);
         for (auto& r : e->lights_remapped) e->h_lights[r.second].d3.x = bits2f(*e->light_slot(r.first) + 1u);
@@ -1609,6 +1666,10 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
         e->lights_created.clear(); e->lights_updated.clear(); e->lights_remapped.clear(); e->lights_killed.clear();
         e->lights_dirty = again;   // commit()/clear_slot() re-dirty the mirror: uploaded on the next tick (mapped_storage_buffer.rs:167-168)
     }
+    // ST_OPT_LIGHT_GRID: the lists follow the lights just uploaded (the build reads d_lights on the stream, behind the upload)
+    if (e->light_grid == 0) e->lgrid_built = 0;
+    else if (lights_uploaded || e->lgrid_built != e->light_grid) { if ((rc = build_light_grid(e))) return rc; }
+    e->lgrid_frame = e->light_grid > 0;
     for (CameraSlot* c : e->cameras) if (c->alive) c->frame = e->frame;   // CameraController::flush (camera_controller.rs:81-85)
     e->nmap_frame = e->normal_maps && e->any_normal_map;
     e->frame += 1;
@@ -1709,6 +1770,21 @@ int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap, size_t
     std::string s(name);
     const void* dev = nullptr; size_t n = 0;
     if (s == "world") { *count = 4; if (dst) std::memcpy(dst, &e->world, 4 * std::min<size_t>(cap, 4)); return ST_OK; }
+    if (s == "light_grid") {   // header, counts, lists (include/strolle_b200.h)
+        if (!e->lgrid_built) return fail(ST_ERR_NOT_FOUND, "no light grid: ST_OPT_LIGHT_GRID is off or no st_tick has built it");
+        const LightGridDev& g = e->lgrid;
+        const size_t cells = (size_t)g.dims[0] * g.dims[1] * g.dims[2] + 1;
+        std::vector<uint32_t> w = {g.dims[0], g.dims[1], g.dims[2], kLightGridK, g.light_count, (uint32_t)(cells - 1)};
+        for (const float* v : {g.lo, g.cell, g.inv_cell, g.band, g.margin}) for (int a = 0; a < 3; a++) { uint32_t b; std::memcpy(&b, v + a, 4); w.push_back(b); }
+        const size_t head = w.size();
+        w.resize(head + cells + cells * kLightGridK);
+        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaMemcpy(w.data() + head, g.counts, cells * 4, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(w.data() + head + cells, g.lists, cells * kLightGridK * 4, cudaMemcpyDeviceToHost));
+        *count = w.size();
+        if (dst) std::memcpy(dst, w.data(), 4 * std::min(cap, w.size()));
+        return ST_OK;
+    }
     if (s == "triangles") { dev = e->d_triangles.p; n = e->h_triangles.size() * 4; }
     else if (s == "bvh") { dev = e->d_bvh.p; n = e->bvh_out.buf.size() * 4; }
     else if (s == "materials") { dev = e->d_materials.p; n = e->h_materials.size() * 28; }
@@ -1783,6 +1859,10 @@ int st_set_option(st_engine* e, int option, int value) {
     if (option == ST_OPT_FUSE_REPROJECT) { e->fuse_reproject = value != 0; return ST_OK; }
     if (option == ST_OPT_WAVELET_TILE_CFG) { e->wavelet_cfg = value & 0xfffff; return ST_OK; }
     if (option == ST_OPT_NORMAL_MAPS) { e->normal_maps = value != 0; return ST_OK; }   // takes effect at the next st_tick
+    if (option == ST_OPT_LIGHT_GRID) {   // takes effect at the next st_tick
+        if (value < 0 || value > 64) return fail(ST_ERR_INVALID, "ST_OPT_LIGHT_GRID: 0 (off) or 1..64 cells along the longest axis");
+        e->light_grid = value; return ST_OK;
+    }
     if (option == ST_OPT_BVH_REFIT) { if (value < 0) return fail(ST_ERR_INVALID, "ST_OPT_BVH_REFIT: 0 or a positive budget"); e->bvh_refit = value; return ST_OK; }
     return fail(ST_ERR_INVALID, "unknown option");
 }
@@ -1826,6 +1906,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_BVH_GRAFTED_SUBTREES) { *value = e->bvh.grafted; return ST_OK; }
     if (stat == ST_STAT_NORMAL_MAP_LAUNCHES) { *value = e->normal_map_launches; return ST_OK; }
     if (stat == ST_STAT_BVH_REFITS) { *value = e->bvh_refits; return ST_OK; }
+    if (stat == ST_STAT_LIGHT_GRID_BUILDS) { *value = e->light_grid_builds; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
         CK(cudaSetDevice(e->device)); CK(cudaStreamSynchronize(e->stream));
         uint64_t total = 0;

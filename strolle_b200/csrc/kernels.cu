@@ -231,9 +231,11 @@ __global__ void __launch_bounds__(ST_BLOCK) k_frame_reprojection(KPARAMS, int cu
 #endif   // ST_EXACT_ONLY
 
 // K5 di_sampling::main (di_sampling.rs:4-94): the initial sample of a pixel whose primary hit is `hit`
-ST_DEV DiRes di_sampling_px(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, const Hit& hit, u32 seed, u32 frame, Px p) {
+// LGRID (ST_OPT_LIGHT_GRID): the candidates are drawn from the light grid's list for hit.point instead of from every slot
+template <bool LGRID>
+ST_DEV DiRes di_sampling_px(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, const Hit& hit, u32 seed, u32 frame, Px p, const LightGridDev& lg) {
     Rng rng = rng_make(seed, p.x, p.y);
-    EphRes res = ephemeral_build(rng, sc, hit);
+    EphRes res = LGRID ? ephemeral_build_list(rng, sc, hit, lgrid_list(lg, hit.point)) : ephemeral_build(rng, sc, hit);
     DiRes out = di_zero();
     if (res.m > 0.0f) {
         float4 bn = blue_noise(sc, p.x, p.y, frame);
@@ -244,13 +246,14 @@ ST_DEV DiRes di_sampling_px(const CameraDev& cam, const SceneDev& sc, const Trac
     }
     return out;
 }
-__global__ void ST_LB_DI_SAMPLING k_di_sampling(KPARAMS, int cur, u32 seed, u32 frame) {
+template <bool LGRID>
+__global__ void ST_LB_DI_SAMPLING k_di_sampling(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ LightGridDev lg) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
     Hit hit = load_hit_lut(sc, cam.curr, cam.prim_gbuffer_d0[cur], cam.prim_gbuffer_d1[cur], cam, p.x, p.y);
     if (!hit_some(hit)) return;
-    di_store(di_sampling_px(cam, sc, stk, hit, seed, frame, p), cam.di_reservoirs[1], screen_idx(cam, p.x, p.y));
+    di_store(di_sampling_px<LGRID>(cam, sc, stk, hit, seed, frame, p, lg), cam.di_reservoirs[1], screen_idx(cam, p.x, p.y));
 }
 
 // K6 di_temporal_resampling::main (di_temporal_resampling.rs:4-112): merges this frame's sample `lhs` with last frame's reservoir at
@@ -302,13 +305,14 @@ __global__ void ST_LB_DI_TEMPORAL k_di_temporal(KPARAMS, int cur, u32 seed) {
 // K5 + K6 in one launch (ST_OPT_FUSED_PASSES): the pixel's fresh sample goes from K5 to K6 in registers instead of through di_reservoirs[1]
 // (the hit is decoded once).  What di_store / di_load would do to the sample on the way (confidence -> byte) is the identity for K5's
 // output (confidence 0), so the result is the two-launch result bit for bit.
-__global__ void ST_LB_DI_SAMPLING k_di_sample_temporal(KPARAMS, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame) {
+template <bool LGRID>
+__global__ void ST_LB_DI_SAMPLING k_di_sample_temporal(KPARAMS, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, const __grid_constant__ LightGridDev lg) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
     Hit hit = load_hit_lut(sc, cam.curr, cam.prim_gbuffer_d0[cur], cam.prim_gbuffer_d1[cur], cam, p.x, p.y);
     if (!hit_some(hit)) return;
-    DiRes fresh = di_sampling_px(cam, sc, stk, hit, seed_sampling, frame, p);
+    DiRes fresh = di_sampling_px<LGRID>(cam, sc, stk, hit, seed_sampling, frame, p, lg);
     di_store_m(cam, di_temporal_px(cam, sc, cur, seed_temporal, p, hit, fresh), cam.di_reservoirs[1], screen_idx(cam, p.x, p.y), p.y, cam.di_mirror_reach);
 }
 
@@ -540,8 +544,10 @@ __global__ void ST_LB_GI_SAMPLING_A k_gi_sampling_a(KPARAMS, int cur, u32 seed, 
     cam.gi_d0[gi] = t0; cam.gi_d1[gi] = t1; cam.gi_d2[gi] = t2;
 }
 
-// K13 gi_sampling_b::main (gi_sampling_b.rs:4-235)
-ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4 d0, float4 d1, float4 d2) {
+// K13 gi_sampling_b::main (gi_sampling_b.rs:4-235); LGRID: the light candidates come from the light grid's list for the bounce hit
+// (the sky-or-light draw still tests the global light count, so the RNG sequence keeps its shape)
+template <bool LGRID>
+ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4 d0, float4 d1, float4 d2, const LightGridDev& lg) {
     bool tracing = gi_tracing_frame(frame);
     uint2 sp = tracing ? checker(g.x, g.y, frame / 2u) : checker(g.x, g.y, frame);
     if (!cam_contains_u(cam.curr, sp.x, sp.y)) return;
@@ -572,7 +578,7 @@ ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const T
             light_dir = rng_hemisphere(rng, gh.g.normal);
             light_rad = atmosphere_sample(sc, sun_dir, light_dir) * dot(gh.g.normal, light_dir);
         } else {
-            EphRes er = ephemeral_build(rng, sc, gh);
+            EphRes er = LGRID ? ephemeral_build_list(rng, sc, gh, lgrid_list(lg, gh.point)) : ephemeral_build(rng, sc, gh);
             if (er.w > 0.0f) { light_id = er.light_id; light_pdf = (1.0f / er.w) * (1.0f - atm_pdf); light_rad = er.rad.radiance * (f3s(1.0f) + er.rad.spec); }
             else { light_id = 0u; light_pdf = 1.0f; light_rad = f3s(0.f); }
         }
@@ -598,23 +604,24 @@ ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const T
     }
     gi_store(res, cam.gi_reservoirs[1], idx);
 }
-__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, u32 frame) {
+template <bool LGRID>
+__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ LightGridDev lg) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     size_t gi = pix(cam, g.x, g.y);
-    gi_sampling_b_pair(cam, sc, stk, cur, seed, frame, g, cam.gi_d0[gi], cam.gi_d1[gi], cam.gi_d2[gi]);
+    gi_sampling_b_pair<LGRID>(cam, sc, stk, cur, seed, frame, g, cam.gi_d0[gi], cam.gi_d1[gi], cam.gi_d2[gi], lg);
 }
 // K12 + K13 in one launch (ST_OPT_FUSED_PASSES): the bounce ray is traced and shaded by the same thread; the hit still goes through
 // GBufferEntry's pack / unpack (its 8-bit quantisation is part of the result), just not through memory.
-template <bool NMAP>
-__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_fused(KPARAMS, int cur, u32 seed_a, u32 seed_b, u32 frame) {
+template <bool NMAP, bool LGRID>
+__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_fused(KPARAMS, int cur, u32 seed_a, u32 seed_b, u32 frame, const __grid_constant__ LightGridDev lg) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
     if (!gi_sampling_a_pair<NMAP>(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2)) return;
-    gi_sampling_b_pair(cam, sc, stk, cur, seed_b, frame, g, t0, t1, t2);
+    gi_sampling_b_pair<LGRID>(cam, sc, stk, cur, seed_b, frame, g, t0, t1, t2, lg);
 }
 
 // K14 gi_temporal_resampling::main (gi_temporal_resampling.rs:4-156)
@@ -1270,8 +1277,9 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
     cam.ref_hits[2 * idx] = h0; cam.ref_hits[2 * idx + 1] = h1;
 }
 
-// K2 ref_shading::main (ref_shading.rs:4-177)
-__global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32 depth) {
+// K2 ref_shading::main (ref_shading.rs:4-177); LGRID: the one light is drawn from the light grid's list for the nudged hit point
+template <bool LGRID>
+__global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32 depth, const __grid_constant__ LightGridDev lg) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
@@ -1304,9 +1312,10 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32
     hit.g.base_color = mat_base_color(sc, m, th.uv); hit.g.normal = th.normal; hit.g.metallic = m.metallic; hit.g.emissive = mat_emissive(sc, m, th.uv);
     hit.g.roughness = m.roughness; hit.g.reflectance = m.reflectance; hit.g.depth = 0.0f;
     color = color + thr * hit.g.emissive;
-    if (sc.world.light_count > 0u) {
-        u32 lid = rng_u32(rng) % sc.world.light_count;
-        float lpdf = 1.0f / (float)sc.world.light_count;
+    const LgList list = LGRID ? lgrid_list(lg, hit.point) : LgList{nullptr, sc.world.light_count};
+    if (list.n > 0u) {
+        u32 lid = lgrid_pick(list, rng_u32(rng) % list.n);
+        float lpdf = 1.0f / (float)list.n;
         GpuLight light = light_load(sc, lid);
         bool occ = trace_any(light_ray_wnoise(light, rng, hit.point), sc, stk);
         if (!occ) color = color + thr * lightrad_sum(light_radiance(light, hit)) / lpdf;
@@ -1374,6 +1383,49 @@ __global__ void k_math(int op, const float* __restrict__ a, const float* __restr
         case 6: r = acos_approx_glam(a[i]); break;
     }
     out[i] = r;
+}
+
+// ST_OPT_LIGHT_GRID: the candidate lists (DESIGN.md §2 "Light grid").  One warp per cell, the outside list last (cell == ncell: no
+// cell box, so only the non-cullable slots).  The warp tests 32 slots at a time and compacts the kept ones with ballot / popc in
+// ascending slot order: deterministic with no sort and no atomics.  A cullable light is dropped when the squared distance from its
+// centre to the cell box grown by `margin` exceeds range^2 (1 + 2^-8); the entries past the count are 0xffffffff.
+__global__ void __launch_bounds__(128) k_light_grid_build(const __grid_constant__ LightGridDev lg, const GpuLight* __restrict__ lights, u32 ncell,
+                                                          u32* __restrict__ counts, u32* __restrict__ lists) {
+    const u32 lane = threadIdx.x & 31u, cell = blockIdx.x * 4u + (threadIdx.x >> 5);
+    if (cell > ncell) return;   // whole warps
+    const bool outside = cell == ncell;
+    float bmin[3] = {0.f, 0.f, 0.f}, bmax[3] = {0.f, 0.f, 0.f};
+    if (!outside) {
+        const u32 idx[3] = {cell % lg.dims[0], (cell / lg.dims[0]) % lg.dims[1], cell / (lg.dims[0] * lg.dims[1])};
+        for (int a = 0; a < 3; a++) {
+            bmin[a] = xsub(xadd(lg.lo[a], xmul((float)idx[a], lg.cell[a])), lg.margin[a]);
+            bmax[a] = xadd(xadd(lg.lo[a], xmul((float)(idx[a] + 1u), lg.cell[a])), lg.margin[a]);
+        }
+    }
+    u32* out = lists + (size_t)cell * kLightGridK;
+    u32 n = 0u;
+    for (u32 base = 0u; base < lg.light_count; base += 32u) {
+        const u32 slot = base + lane;
+        bool keep = false;
+        if (slot < lg.light_count) {
+            const float4* p = reinterpret_cast<const float4*>(lights + slot);
+            GpuLight l; l.d0 = ldg4(p); l.d1 = ldg4(p + 1); l.d2 = ldg4(p + 2);
+            if (!lgrid_cullable(l)) keep = true;
+            else if (!outside) {
+                const float c[3] = {l.d0.x, l.d0.y, l.d0.z};
+                float d[3];
+                for (int a = 0; a < 3; a++) d[a] = fmaxf(fmaxf(xsub(bmin[a], c[a]), xsub(c[a], bmax[a])), 0.0f);
+                const float d2 = xadd(xadd(xmul(d[0], d[0]), xmul(d[1], d[1])), xmul(d[2], d[2]));
+                keep = !(d2 > xmul(xmul(l.d1.w, l.d1.w), 1.00390625f));
+            }
+        }
+        const u32 mask = __ballot_sync(0xffffffffu, keep);
+        const u32 pos = n + __popc(mask & ((1u << lane) - 1u));
+        if (keep && pos < kLightGridK) out[pos] = slot;
+        n += __popc(mask);
+    }
+    for (u32 k = min(n, kLightGridK) + lane; k < kLightGridK; k += 32u) out[k] = 0xffffffffu;
+    if (lane == 0u) counts[cell] = n > kLightGridK ? kLightGridOverflow : n;
 }
 
 // derived tables: packed gamma colour per material, byte -> linear table for GBufferEntry::unpack
@@ -1563,7 +1615,9 @@ static dim3 grid_full(const CameraDev& cam) { return dim3((cam.w + TILE_W - 1) /
 static dim3 grid_half(const CameraDev& cam) { int hw = 8 * (((cam.w + 7) / 8) / 2); return dim3((hw + TILE_W - 1) / TILE_W, (cam.y1 - cam.y0 + TILE_H - 1) / TILE_H); }
 #define HALF_LAUNCH(kernel, c, st, ...) do { dim3 g_ = grid_half(c); if (g_.x > 0 && g_.y > 0) kernel<<<g_, ST_BLOCK, 0, st>>>(__VA_ARGS__); } while (0)
 
-void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { k_di_sampling<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, frame); }
+void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st) {
+    if (lg) k_di_sampling<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, frame, *lg); else k_di_sampling<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, frame, LightGridDev{});
+}
 void launch_di_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, cudaStream_t st) { k_di_temporal<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed); }
 void launch_di_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_pick, c, st, c, s, cur, seed, frame); }
 void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d0, const float4* d1, float4* d2, cudaStream_t st) { k_spatial_trace<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, d0, d1, d2); }
@@ -1573,16 +1627,26 @@ void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cuda
 void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, cudaStream_t st) {
     if (nmap) HALF_LAUNCH(k_gi_sampling_a<true>, c, st, c, s, cur, seed, frame); else HALF_LAUNCH(k_gi_sampling_a<false>, c, st, c, s, cur, seed, frame);
 }
-void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_sampling_b, c, st, c, s, cur, seed, frame); }
+void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st) {
+    if (lg) HALF_LAUNCH(k_gi_sampling_b<true>, c, st, c, s, cur, seed, frame, *lg); else HALF_LAUNCH(k_gi_sampling_b<false>, c, st, c, s, cur, seed, frame, LightGridDev{});
+}
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st) { k_gi_temporal<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, frame, inline_reprojection); }
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_pick, c, st, c, s, cur, seed, frame); }
 void launch_gi_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_sample, c, st, c, s, seed, frame); }
 void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 nth, const float4* in, float4* out, int mirror_reach, cudaStream_t st) { k_gi_preview<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, nth, in, out, mirror_reach); }
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st) { k_gi_resolving<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, in); }
-void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, cudaStream_t st) { k_di_sample_temporal<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed_sampling, seed_temporal, frame); }
+void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, const LightGridDev* lg, cudaStream_t st) {
+    if (lg) k_di_sample_temporal<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed_sampling, seed_temporal, frame, *lg);
+    else k_di_sample_temporal<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed_sampling, seed_temporal, frame, LightGridDev{});
+}
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, cudaStream_t st) {
-    if (nmap) HALF_LAUNCH(k_gi_sampling_fused<true>, c, st, c, s, cur, seed_a, seed_b, frame); else HALF_LAUNCH(k_gi_sampling_fused<false>, c, st, c, s, cur, seed_a, seed_b, frame);
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, cudaStream_t st) {
+    const LightGridDev none{};
+    if (lg) {
+        if (nmap) HALF_LAUNCH((k_gi_sampling_fused<true, true>), c, st, c, s, cur, seed_a, seed_b, frame, *lg); else HALF_LAUNCH((k_gi_sampling_fused<false, true>), c, st, c, s, cur, seed_a, seed_b, frame, *lg);
+    } else {
+        if (nmap) HALF_LAUNCH((k_gi_sampling_fused<true, false>), c, st, c, s, cur, seed_a, seed_b, frame, none); else HALF_LAUNCH((k_gi_sampling_fused<false, false>), c, st, c, s, cur, seed_a, seed_b, frame, none);
+    }
 }
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st) { k_gi_preview_resolve<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, in, source); }
@@ -1794,11 +1858,17 @@ void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cud
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {
     if (nmap) k_ref_tracing<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); else k_ref_tracing<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth);
 }
-void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, cudaStream_t st) { k_ref_shading<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth); }
+void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, cudaStream_t st) {
+    if (lg) k_ref_shading<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, *lg); else k_ref_shading<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, LightGridDev{});
+}
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st) { k_bvh_heatmap<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s); }
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st) { k_trace_stream_closest<<<(unsigned)((n + ST_BLOCK - 1) / ST_BLOCK), ST_BLOCK, 0, st>>>(s, rays, n, out); }
 void launch_trace_stream_any(const SceneDev& s, const float4* rays, long n, u32* out, cudaStream_t st) { k_trace_stream_any<<<(unsigned)((n + ST_BLOCK - 1) / ST_BLOCK), ST_BLOCK, 0, st>>>(s, rays, n, out); }
 void launch_math(int op, const float* a, const float* b, float* out, long n, cudaStream_t st) { k_math<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n); }
+void launch_light_grid_build(const LightGridDev& lg, const GpuLight* lights, cudaStream_t st) {
+    const u32 ncell = lg.dims[0] * lg.dims[1] * lg.dims[2];
+    k_light_grid_build<<<(ncell + 1u + 3u) / 4u, 128, 0, st>>>(lg, lights, ncell, const_cast<u32*>(lg.counts), const_cast<u32*>(lg.lists));
+}
 void launch_material_derive(const GpuMaterial* mats, u32 n, u32* packed, cudaStream_t st) { if (n) k_material_derive<<<(n + 127) / 128, 128, 0, st>>>(mats, n, packed); }
 void launch_srgb_lut(float* lut, cudaStream_t st) { k_srgb_lut<<<1, 256, 0, st>>>(lut); }
 void launch_unpack_lut(float* lut, cudaStream_t st) { k_unpack_lut<<<1, 256, 0, st>>>(lut); }
@@ -1941,7 +2011,7 @@ int preload_kernels() {
     cudaGetLastError();
     if (!get_module || !get_count || !enumerate || !load) return state = 1;
     cudaFunction_t anchor = nullptr;
-    if (cudaGetFuncBySymbol(&anchor, (const void*)k_di_sample_temporal) != cudaSuccess) { cudaGetLastError(); return state = 2; }
+    if (cudaGetFuncBySymbol(&anchor, (const void*)k_di_sample_temporal<false>) != cudaSuccess) { cudaGetLastError(); return state = 2; }
     CUmodule mod = nullptr; unsigned int n = 0;
     if (get_module(&mod, (CUfunction)anchor) != CUDA_SUCCESS || get_count(&n, mod) != CUDA_SUCCESS || n == 0u) return state = 3;
     std::vector<CUfunction> fns(n);

@@ -800,6 +800,61 @@ ST_DEV EphRes ephemeral_build(Rng& rng, const SceneDev& sc, const Hit& hit) {
     return res;
 }
 
+// ---- Light grid (ST_OPT_LIGHT_GRID; DESIGN.md §2 "Light grid") -----------------------------------------------------------
+// A slot is cullable when its radiance is provably zero outside its range sphere: a point light (kind 1) with a finite position and
+// colour and 2^-60 <= range <= 2^60 (|position| <= 2^60: no squared distance the test or light_radiance forms overflows or flushes).
+// Spot lights stay in every list: their f_angle is NaN where the cone axis or the offset degenerates, and sat() keeps NaN.
+ST_DEV bool lgrid_cullable(const GpuLight& l) {
+    const float big = 1.152921504606846976e18f, tiny = 8.673617379884035472e-19f;   // 2^60, 2^-60
+    if (fbits(l.d2.x) != 1u) return false;
+    if (!(fabsf(l.d0.x) <= big && fabsf(l.d0.y) <= big && fabsf(l.d0.z) <= big)) return false;
+    if (!(isfinite(l.d1.x) && isfinite(l.d1.y) && isfinite(l.d1.z))) return false;
+    return l.d1.w >= tiny && l.d1.w <= big;
+}
+// The list a point samples from: `ids` = nullptr means every slot (identity), as with the option off.
+struct LgList { const u32* ids; u32 n; };
+ST_DEV LgList lgrid_list(const LightGridDev& lg, float3 p) {
+    LgList all; all.ids = nullptr; all.n = lg.light_count;
+    if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) return all;
+    const u32 ncell = lg.dims[0] * lg.dims[1] * lg.dims[2];
+    u32 cell = ncell;   // the outside list
+    if (ncell > 0u) {
+        const float pc[3] = {p.x, p.y, p.z};
+        u32 idx[3]; bool inside = true;
+#pragma unroll
+        for (int a = 0; a < 3; a++) {
+            const float t = xmul(xsub(pc[a], lg.lo[a]), lg.inv_cell[a]);
+            if (!(t >= -lg.band[a]) || !(t < xadd((float)lg.dims[a], lg.band[a]))) inside = false;
+            const int i = (int)floorf(fminf(fmaxf(t, 0.0f), (float)(lg.dims[a] - 1u)));
+            idx[a] = (u32)i;
+        }
+        if (inside) cell = (idx[2] * lg.dims[1] + idx[1]) * lg.dims[0] + idx[0];
+    }
+    const u32 c = __ldg(lg.counts + cell);
+    if (c == kLightGridOverflow) return all;
+    LgList l; l.ids = lg.lists + (size_t)cell * kLightGridK; l.n = c;
+    return l;
+}
+ST_DEV u32 lgrid_pick(const LgList& l, u32 r) { return l.ids ? __ldg(l.ids + r) : r; }
+// ephemeral_build over a list of n slots: min(n, 16) uniform draws from the list at ipdf = n (the option off: the list of every slot)
+ST_DEV EphRes ephemeral_build_list(Rng& rng, const SceneDev& sc, const Hit& hit, const LgList& list) {
+    EphRes res; res.m = 0.f; res.w = 0.f; res.light_id = 0u; res.rad = lightrad_zero();
+    float res_pdf = 0.0f;
+    u32 lc = list.n;
+    u32 max_samples = lc < 16u ? lc : 16u;
+    float ipdf = (float)lc;
+    for (u32 nth = 0u; nth < max_samples; nth++) {
+        u32 id = lgrid_pick(list, rng_u32(rng) % lc);
+        LightRad lr = light_radiance(light_load(sc, id), hit);
+        float pdf = sqrtf(luma(lr.radiance));
+        float weight = pdf * ipdf;
+        res.m += 1.0f; res.w += weight;
+        if (rng_f(rng) * res.w < weight) { res.light_id = id; res.rad = lr; res_pdf = pdf; }
+    }
+    res.w = res_norm(res.w, res_pdf, 1.0f, res.m);
+    return res;
+}
+
 // Mis (mis.rs:12-155)
 struct MisIn { float lhs_m, rhs_m, rhs_jacobian, lhs_lhs_pdf, lhs_rhs_pdf, rhs_lhs_pdf, rhs_rhs_pdf; };
 struct MisOut { float m, lhs_pdf, lhs_mis, rhs_pdf, rhs_mis; };

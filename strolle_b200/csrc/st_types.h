@@ -48,6 +48,22 @@ struct SceneDev {
     unsigned long long* ray_counter;   // optional: counts executed Ray::trace / Ray::intersect calls (Mrays/s)
 };
 
+// ST_OPT_LIGHT_GRID (DESIGN.md §2 "Light grid"): the per-cell candidate lists of the light slots that can reach the cell.  Built on
+// the device at st_tick (k_light_grid_build); passed by value to the LGRID instantiations of the candidate-sampling kernels only.
+static const uint32_t kLightGridK = 64;                   // list capacity per cell
+static const uint32_t kLightGridOverflow = 0xffffffffu;   // a count that marks an overflowing list: the cell samples every slot
+struct LightGridDev {
+    float lo[3];         // grid box minimum: the AABB of the cullable lights' spheres
+    float cell[3];       // cell size per axis (extent / dims)
+    float inv_cell[3];   // dims / extent: point -> cell index
+    float band[3];       // in cells: points outside the box by less than this clamp to the edge cell instead of taking the outside list
+    float margin[3];     // world units each cell box is grown by before the reach test
+    uint32_t dims[3];
+    uint32_t light_count;            // the slots the lists were built over
+    const uint32_t* counts;          // dims.x * dims.y * dims.z cells + 1 (the outside list last); kLightGridOverflow = every slot
+    const uint32_t* lists;           // kLightGridK slots per cell, the outside list last
+};
+
 // Per-camera device buffers: the logical buffers of
 // strolle/src/camera_controller/buffers.rs:53-339 as linear row-major float4
 // arrays indexed by full-frame coordinates (each GPU of a strip-partitioned run

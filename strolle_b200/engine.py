@@ -27,6 +27,7 @@ OPT_STRIP_FUSED = 10         # strips: fused transport (mirror stores, neighbour
 OPT_SHADING_FAST_MATH = 9  # ReSTIR kernels K5-K19 from the fast-shading build (FMA + SFU approximations; traversal unchanged)
 OPT_NORMAL_MAPS = 14         # shade with the materials' normal maps (off by default: the reference ignores them); from the next tick
 OPT_BVH_REFIT = 15           # N > 0: up to N ticks in a row that only move instances bake on the device and refit the BVH (0 = rebuild)
+OPT_LIGHT_GRID = 16          # N in 1..64: light candidates from a world-space grid of N cells along its longest axis (0 = every slot)
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
 STAT_WAVELET_TILED_ERRORS = 2
@@ -37,6 +38,7 @@ STAT_LAST_FRAME_FUSED_STRIPS = 6
 STAT_STRIP_FIRST_TIMEOUT = 7
 STAT_NORMAL_MAP_LAUNCHES = 8   # launches of the normal-mapped kernel variants
 STAT_BVH_REFITS = 9            # refit ticks (OPT_BVH_REFIT) since the engine was created
+STAT_LIGHT_GRID_BUILDS = 10    # light grid builds (OPT_LIGHT_GRID) since the engine was created
 
 
 class StrolleError(RuntimeError):

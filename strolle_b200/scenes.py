@@ -364,6 +364,60 @@ def stress_bvh(n=2000, width=1920, height=1080, mode=MODE_IMAGE, denoise=True, t
     return dict(name="stress_bvh", meshes=meshes, materials=materials, instances=instances, lights=lights, sun=(1.0, 0.6), camera=cam)
 
 
+def _hsl_linear(h, s, l):
+    """Bevy's Color::hsl(h, s, l).as_linear_rgba_f32() for the rgb part: HSL -> sRGB, then the sRGB transfer curve."""
+    c = (1.0 - abs(2.0 * l - 1.0)) * s
+    hp = (h % 360.0) / 60.0
+    x = c * (1.0 - abs(hp % 2.0 - 1.0))
+    r, g, b = [(c, x, 0), (x, c, 0), (0, c, x), (0, x, c), (x, 0, c), (c, 0, x)][min(int(hp), 5)]
+    m = l - c / 2.0
+    lin = lambda v: v / 12.92 if v <= 0.04045 else ((v + 0.055) / 1.055) ** 2.4
+    return tuple(lin(v + m) for v in (r, g, b))
+
+
+STRESS_LIGHTS_FIRST = 400   # stress_lights' light handles: 400 .. 499
+
+
+def stress_lights_lights(t):
+    """The 100 point lights of stress_lights at time `t` (stress-lights.rs update_lights): light k, with phase k * 123.456, circles its
+    room's anchor at radius 4 with the angle u = phase * 2 pi + t and takes the hue (u * 90) mod 360; range 20, radius 0.25,
+    intensity 3000 (x 1/4pi, as the reference's extract does)."""
+    out, phase, inten = [], 0.0, 3000.0 / (4.0 * math.pi)
+    k = 0
+    for x in range(-5, 5):
+        for y in range(10):
+            ax, ay = x * 15.0, y * 15.0
+            u = phase * 2.0 * math.pi + t
+            pos = (ax + 4.0 * math.sin(u), 5.0 + ay + 4.0 * math.cos(u), 0.0)
+            col = tuple(v * inten for v in _hsl_linear((u * 90.0) % 360.0, 1.0, 0.5))
+            out.append((STRESS_LIGHTS_FIRST + k, LIGHT_POINT, point_light(pos, 0.25, col, 20.0)))
+            phase += 123.456
+            k += 1
+    return out
+
+
+def stress_lights(width=512, height=512, mode=MODE_IMAGE, denoise=True, ref_depth=1, t=0.0):
+    """bevy-strolle/examples/stress-lights.rs: a 1000 x 1 x 1000 floor box at y = -2 and a 10 x 10 grid of rooms 15 apart (five
+    scaled unit boxes each: two side walls, a back wall, a ceiling and a floor), each with a moving, recolouring point light of
+    range 20 (stress_lights_lights); sun altitude -1, camera (0, 50, 80) -> (0, 50, 0).  `t` is the example's elapsed time."""
+    walls = [((1.0, 10.0, 10.0), (-5.0, 5.0, 0.0)), ((1.0, 10.0, 10.0), (5.0, 5.0, 0.0)), ((10.0, 10.0, 1.0), (0.0, 5.0, -5.0)),
+             ((10.0, 1.0, 10.0), (0.0, 10.0, 0.0)), ((10.0, 1.0, 10.0), (0.0, 0.0, 0.0))]
+    scaled = lambda sc, tr: np.array([sc[0], 0, 0, 0, sc[1], 0, 0, 0, sc[2], tr[0], tr[1], tr[2]], np.float32)
+    instances = [(300, 200, 100, scaled((1000.0, 1.0, 1000.0), (0.0, -2.0, 0.0)))]
+    h = 301
+    for x in range(-5, 5):
+        for y in range(10):
+            for sc, tr in walls:
+                instances.append((h, 200, 100, scaled(sc, (tr[0] + x * 15.0, tr[1] + y * 15.0, tr[2]))))
+                h += 1
+    cam = dict(mode=mode, denoise=denoise, ref_depth=ref_depth, w=width, h=height,
+               transform=look_at_transform((0.0, 50.0, 80.0), (0.0, 50.0, 0.0)),
+               projection=perspective_infinite_reverse_rh(math.pi / 4.0, width / height, 0.1))
+    return dict(name="stress_lights", meshes={200: np.stack(_box((-0.5, -0.5, -0.5), (0.5, 0.5, 0.5)))},
+                materials={100: (material((1.0, 1.0, 1.0, 1.0), perceptual_roughness=0.5), False)}, instances=instances, lights=stress_lights_lights(t),
+                sun=(0.0, -1.0), camera=cam)
+
+
 def _quad(p0, p1, p2, p3, normal, uv_lo=(0.0, 0.0), uv_hi=(1.0, 1.0), tangents=None):
     """Two triangles wound so that the geometric normal agrees with `normal` (Triangle::hit flips the shading normal by
     the sign of the determinant, strolle-gpu/src/triangle.rs:95-101, i.e. it trusts the winding).  `tangents`: one

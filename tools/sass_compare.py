@@ -1,5 +1,6 @@
 """Compare per-kernel SASS of two libstrolle_b200.so builds: every kernel of the old build against the same kernel (for a kernel that
-gained a `bool NMAP` template parameter: its <false> instantiation) of the new one.  Compared: the full instruction text (opcodes,
+gained `bool NMAP` / `bool LGRID` template parameters: its all-<false> instantiation, whose trailing LightGridDev argument is unused)
+of the new one.  Compared: the full instruction text (opcodes,
 registers, immediates, constant-bank operands); normalised: the code-offset comments, branch targets and relocated symbol names."""
 import re, subprocess, sys
 
@@ -22,9 +23,25 @@ def kernels(lib):
             body.append(ins)
     if name: funcs[name] = body
     dem = subprocess.run(["c++filt"], input="\n".join(funcs), capture_output=True, text=True).stdout.split("\n")
-    NM = ("k_prim_gbuffer", "k_gi_sampling_a", "k_gi_sampling_fused", "k_ref_tracing")
-    norm = lambda d: re.sub(r"^void (.*)<false>", r"\1", d) if any("::" + k + "<" in d for k in NM) else d
-    return {norm(d): funcs[m] for d, m in zip(dem, funcs)}, {d for d in dem if "<true>" in d and any("::" + k + "<" in d for k in NM)}
+    NM = ("k_prim_gbuffer", "k_gi_sampling_a", "k_ref_tracing", "k_gi_sampling_fused")                          # bool NMAP
+    LG = {"k_di_sampling": 0, "k_di_sample_temporal": 0, "k_gi_sampling_b": 0, "k_ref_shading": 0, "k_gi_sampling_fused": 1}   # bool LGRID, its position
+    def base(d):
+        m = re.search(r"::(\w+)<", d)
+        return m.group(1) if m and (m.group(1) in NM or m.group(1) in LG) else None
+    def targs(d): return d.split("(")[0].split("<", 1)[1].rstrip(">").split(", ")
+    def norm(d):   # the name the kernel had before it gained LGRID (and NMAP): all-false instantiations lose their template arguments
+        k = base(d)
+        if k is None: return d
+        args = targs(d)
+        if k in LG and len(args) > LG[k]:
+            if args[LG[k]] == "true": return d
+            del args[LG[k]]
+            d = re.sub(r", \w+::LightGridDev\)", ")", d)
+        head = d.split("(")[0]
+        name = head.split("<")[0]
+        if all(a == "false" for a in args): return re.sub(r"^void ", "", name) + d[len(head):]
+        return name + "<" + ", ".join(args) + ">" + d[len(head):]
+    return {norm(d): funcs[m] for d, m in zip(dem, funcs)}, {d for d in dem if base(d) and "true" in targs(d)}
 
 old, _ = kernels(sys.argv[1])
 new, nmap = kernels(sys.argv[2])
@@ -37,5 +54,5 @@ for k, body in sorted(old.items()):
         if "-v" in sys.argv:
             import difflib
             print("\n".join(list(difflib.unified_diff(body, new[k], lineterm="", n=1))[:60]))
-print(f"{same} kernels identical, {diff} differ; {len(old)} kernels in the old build, {len(new)} (+{len(nmap)} NMAP instantiations) in the new")
-for k in sorted(nmap): print("  NMAP:", k)
+print(f"{same} kernels identical, {diff} differ; {len(old)} kernels in the old build, {len(new)} (+{len(nmap)} NMAP / LGRID instantiations) in the new")
+for k in sorted(nmap): print("  NMAP / LGRID:", k)
