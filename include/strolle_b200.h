@@ -148,7 +148,12 @@ int st_read_buffer(st_engine* e, st_camera_handle camera, const char* name, floa
  * "scattering_lut", "sky_lut"; and, while ST_OPT_LIGHT_GRID is on and a tick has built it, "light_grid" as 32-bit words: a 21-word
  * header {dims x, y, z, K = 64, light_count, cells, lo[3], cell[3], inv_cell[3], band[3], margin[3]} (the last 15 are f32 bits), the
  * count of every cell then of the outside list (0xffffffff = overflow: every slot), then K slots per cell and K for the outside list
- * (0xffffffff past the count).  Cell (x, y, z) is index (z dims.y + y) dims.x + x. */
+ * (0xffffffff past the count).  Cell (x, y, z) is index (z dims.y + y) dims.x + x.  While ST_OPT_TEXTURE_FILTER is on and a tick has
+ * built them, "texture_mips" as 32-bit words: {T = pool texels, M = materials}, then per material 3 pairs {pool texel offset of level
+ * 1, level count} for its base colour, emissive and metallic-roughness textures ({0, 0}: none; a count of 1: a 1x1 image, level 0
+ * only), then the T
+ * RGBA8 texels of the pool (byte 0 = red).  The pool holds levels 1.. of every live image in insertion order, level after level,
+ * each row-major; level k + 1 is max(1, w_k >> 1) x max(1, h_k >> 1). */
 int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap_floats, size_t* count);
 int st_bvh_depth(st_engine* e, int* depth);
 uint32_t st_frame(st_engine* e);
@@ -161,7 +166,8 @@ int st_set_frame(st_engine* e, uint32_t frame);
  * used_memory).  any: out = n u32 flags.  `device_ms` (optional) receives kernel time. */
 int st_trace_closest(st_engine* e, const float* rays, size_t n, float* out, float* device_ms);
 int st_trace_any(st_engine* e, const float* rays, size_t n, uint32_t* out, float* device_ms);
-/* elementary functions as evaluated on the device (op: 0 sin, 1 cos, 2 acos, 3 atan2, 4 exp, 5 pow, 6 glam's acos_approx) */
+/* elementary functions as evaluated on the device (op: 0 sin, 1 cos, 2 acos, 3 atan2, 4 exp, 5 pow, 6 glam's acos_approx, 7 the
+ * flag-independent log2 of ST_OPT_TEXTURE_FILTER's level of detail, for finite a > 0) */
 int st_device_math(st_engine* e, int op, const float* a, const float* b, float* out, size_t n);
 /* Per-pass device time (ms, CUDA events) accumulated since the last reset; `ms`/`launches`
  * have ST_PASS_COUNT entries indexed by st_pass_name(). */
@@ -176,7 +182,18 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17 };
+/* ST_OPT_TEXTURE_FILTER (default 0; 1 = on, anything else is ST_ERR_INVALID): material textures are filtered through per-image mip
+ * chains with a ray-cone level of detail, instead of the nearest texel of level 0 (the reference's sampler, so 0 keeps parity).
+ * Level 0 is the image's atlas rect; levels 1.. (each texel the 2x2 box of the level above, averaged in linear light through the
+ * sRGB table and re-encoded to the nearest byte; alpha averaged on the bytes) live in a device pool allocated only while the option
+ * is on, rebuilt at st_tick when images or materials changed or the option turned on (ST_STAT_TEXTURE_MIP_BUILDS).  The level of
+ * detail is lambda = 0.5 log2(A_uv W H w^2 |c| / (c.d)^2) for a hit on a triangle with edge cross product c and uv area A_uv, of
+ * a W x H image, seen along d with cone width w: the spread of the pixel's camera ray to its right and lower neighbours at the
+ * hit (primary hits), or a fresh cone from the segment's origin (the GI bounce, Reference mode at depth >= 1).  The sample is
+ * trilinear: bilinear on levels floor(lambda) and floor(lambda) + 1 with repeat-wrapped taps inside the image.  It applies to base
+ * colour, emissive and metallic-roughness at the G-buffer, to base colour and emissive at the GI bounce and in Reference mode; the
+ * alpha test and normal maps keep the nearest level-0 texel.  Takes effect at the next st_tick (DESIGN.md §2). */
 /* ST_OPT_LIGHT_GRID (default 0 = off; 1..64, anything else is ST_ERR_INVALID): the light candidates of ReSTIR DI sampling, of the GI
  * bounce's next-event estimate and of Reference mode are drawn uniformly from a per-cell list of the light slots that can reach the
  * point's cell, instead of from every slot.  N is the cell count along the longest axis of the grid box, the AABB of the range spheres of
@@ -266,7 +283,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_STRIP_FIRST_TIMEOUT = 7 /* 0, or 0x80000000 | slot << 16 | awaited rank << 8 | sequence & 0xff of the first strip flag wait that gave up */,
        ST_STAT_NORMAL_MAP_LAUNCHES = 8 /* launches of the normal-mapped kernel variants (ST_OPT_NORMAL_MAPS) since creation */,
        ST_STAT_BVH_REFITS = 9 /* refit ticks (ST_OPT_BVH_REFIT) since creation */,
-       ST_STAT_LIGHT_GRID_BUILDS = 10 /* light grid builds (ST_OPT_LIGHT_GRID) since creation */ };
+       ST_STAT_LIGHT_GRID_BUILDS = 10 /* light grid builds (ST_OPT_LIGHT_GRID) since creation */,
+       ST_STAT_TEXTURE_MIP_BUILDS = 11 /* mip-chain builds (ST_OPT_TEXTURE_FILTER) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,

@@ -47,11 +47,13 @@ pub struct StrolleSun {
 /// (0, the default, rebuilds every time, as the reference does).
 /// `light_grid`: sample light candidates from a grid of the point lights that can reach each cell, this many cells along its
 /// longest axis (1..=64; 0, the default, samples every light, as the reference does) - for scenes with many short-range lights.
+/// `texture_filter`: filter material textures through mip chains (false, the default, takes the nearest texel, as the reference does).
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
     pub bvh_refit_ticks: u32,
     pub light_grid: u32,
+    pub texture_filter: bool,
 }
 
 #[derive(Clone, Debug)]
@@ -95,6 +97,7 @@ impl Plugin for StrollePlugin {
         engine.set_normal_maps(settings.normal_maps).expect("strolle_b200: ST_OPT_NORMAL_MAPS");
         engine.set_bvh_refit(settings.bvh_refit_ticks).expect("strolle_b200: ST_OPT_BVH_REFIT");
         engine.set_light_grid(settings.light_grid).expect("strolle_b200: ST_OPT_LIGHT_GRID");
+        engine.set_texture_filter(settings.texture_filter).expect("strolle_b200: ST_OPT_TEXTURE_FILTER");
         render_app.insert_resource(EngineResource(engine));
     }
 }

@@ -440,6 +440,12 @@ impl<P: Params> Engine<P> {
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_LIGHT_GRID, cells.min(c_int::MAX as u32) as c_int) })
     }
 
+    /// Filters material textures through per-image mip chains with a ray-cone level of detail (`ST_OPT_TEXTURE_FILTER`; off, the
+    /// default, takes the nearest texel, as the reference does).  Takes effect with the next frame's scene update.
+    pub fn set_texture_filter(&mut self, on: bool) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_TEXTURE_FILTER, on as c_int) })
+    }
+
     /// Creates or updates a mesh (`lib.rs:161-164`).
     pub fn insert_mesh(&mut self, handle: P::MeshHandle, item: Mesh) {
         let id = self.meshes.id(handle);

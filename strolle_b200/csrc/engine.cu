@@ -482,6 +482,12 @@ struct st_engine {
     // on the device was built for (0 = none, or stale), `lgrid` = its header with the pointers into d_lgrid, `lgrid_frame` = the
     // frame's candidate-sampling kernels run their LGRID instantiation (taken at st_tick)
     int light_grid = 0, lgrid_built = 0; bool lgrid_frame = false; LightGridDev lgrid{}; DevMem d_lgrid; uint64_t light_grid_builds = 0;
+    // ST_OPT_TEXTURE_FILTER: `texture_filter` = the option, `texf_built` = the pool and table on the device follow the current images
+    // and materials, `any_color_texture` = some material has a base colour, emissive or metallic-roughness rect (set when materials are
+    // uploaded), `texf_frame` = the frame's hit-shading kernels run their TEXF instantiation (taken at st_tick)
+    bool texture_filter = false, texf_built = false, any_color_texture = false, texf_frame = false; TexFilterDev texf{};
+    DevMem d_texf_pool, d_texf_table, d_texf_jobs; std::vector<uint2> h_texf_table; std::vector<MipJob> h_texf_jobs; size_t texf_pool_texels = 0;
+    uint64_t texture_mip_builds = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -583,6 +589,73 @@ static int build_light_grid(st_engine* e) {
     g.counts = (const uint32_t*)e->d_lgrid.p; g.lists = g.counts + count_words;
     launch_light_grid_build(g, (const GpuLight*)e->d_lights.p, e->stream);
     e->lgrid = g; e->lgrid_built = e->light_grid; e->light_grid_builds++;
+    return ST_OK;
+}
+
+// ---- ST_OPT_TEXTURE_FILTER (DESIGN.md §2 "Texture filtering") -----------------------------------------------------------------
+// The pool holds levels 1.. of every live image, in the order of e->images, level after level.  Each material gets, for its base
+// colour, emissive and metallic-roughness rects, {pool offset of the image's level 1, level count}: {0, 0} without a texture.  A rect
+// that matches no live image gets {0, 1} (bilinear on level 0); st_tick re-serialises the materials whenever an image is removed, so
+// the table is built from live rects only and this is a guard.  One k_texture_mips launch per level builds level k + 1 of every
+// image that has it from level k; nothing here waits for the device.
+static int upload(st_engine* e, DevMem& d, const void* src, size_t bytes);
+static int build_texture_mips(st_engine* e) {
+    struct Chain { uint32_t x, y, w, h, off1, levels; };
+    std::vector<Chain> chains;
+    size_t total = 0;
+    uint32_t max_levels = 1;
+    for (const auto& r : e->images) {
+        Chain c = {r.x, r.y, r.w, r.h, (uint32_t)total, 1u};
+        for (uint32_t w = r.w, h = r.h; w > 1u || h > 1u; c.levels++) { w = std::max(1u, w >> 1); h = std::max(1u, h >> 1); total += (size_t)w * h; }
+        max_levels = std::max(max_levels, c.levels);
+        chains.push_back(c);
+    }
+    if (total >= (size_t)1 << 31) return fail(ST_ERR_LIMIT, "ST_OPT_TEXTURE_FILTER: mip pool too large");
+    e->h_texf_table.assign(3 * e->h_materials.size(), make_uint2(0u, 0u));
+    for (size_t i = 0; i < e->h_materials.size(); i++) {
+        const GpuMaterial& g = e->h_materials[i];
+        const float4 rects[3] = {g.base_color_texture, g.emissive_texture, g.metallic_roughness_texture};
+        for (int k = 0; k < 3; k++) {
+            const float4 r = rects[k];
+            if (r.x == 0.0f && r.y == 0.0f && r.z == 0.0f && r.w == 0.0f) continue;
+            uint2 entry = make_uint2(0u, 1u);
+            for (const Chain& c : chains)
+                if (r.x == (float)c.x / (float)kAtlasSize && r.y == (float)c.y / (float)kAtlasSize && r.z == (float)c.w / (float)kAtlasSize && r.w == (float)c.h / (float)kAtlasSize) {
+                    entry = make_uint2(c.off1, c.levels); break;
+                }
+            e->h_texf_table[3 * i + k] = entry;
+        }
+    }
+    // jobs of level k + 1 (k = 0 .. max_levels - 2), grouped by level
+    e->h_texf_jobs.clear();
+    std::vector<uint32_t> first, blocks;
+    for (uint32_t k = 0; k + 1 < max_levels; k++) {
+        first.push_back((uint32_t)e->h_texf_jobs.size());
+        uint32_t widest = 0;
+        for (const Chain& c : chains) {
+            if (c.levels <= k + 1) continue;
+            uint32_t w = c.w, h = c.h, off = c.off1, prev_off = 0;
+            for (uint32_t j = 1; j <= k + 1; j++) { if (j > 1) { prev_off = off; off += w * h; } w = std::max(1u, w >> 1); h = std::max(1u, h >> 1); }
+            const uint32_t sw = std::max(1u, k == 0 ? c.w : (c.w >> k)), sh = std::max(1u, k == 0 ? c.h : (c.h >> k));
+            MipJob jb;
+            if (k == 0) { jb.src = c.y * kAtlasSize + c.x; jb.src_stride = kAtlasSize; jb.from_atlas = 1u; }
+            else { jb.src = prev_off; jb.src_stride = sw; jb.from_atlas = 0u; }
+            jb.src_w = sw; jb.src_h = sh; jb.dst = off; jb.dst_w = w; jb.dst_h = h;
+            e->h_texf_jobs.push_back(jb);
+            widest = std::max(widest, (w * h + 255u) / 256u);
+        }
+        blocks.push_back(widest);
+    }
+    first.push_back((uint32_t)e->h_texf_jobs.size());
+    int rc;
+    if ((rc = e->d_texf_pool.ensure(std::max<size_t>(total, 1) * 4))) return rc;   // grow-only
+    if ((rc = upload(e, e->d_texf_table, e->h_texf_table.data(), e->h_texf_table.size() * sizeof(uint2)))) return rc;
+    if ((rc = upload(e, e->d_texf_jobs, e->h_texf_jobs.data(), e->h_texf_jobs.size() * sizeof(MipJob)))) return rc;
+    if (!e->h_texf_jobs.empty() && e->d_atlas.p)
+        CK(launch_texture_mips((const MipJob*)e->d_texf_jobs.p, first.data(), blocks.data(), (int)blocks.size(), (const uchar4*)e->d_atlas.p,
+                               (uchar4*)e->d_texf_pool.p, (const float*)e->d_srgb.p, e->stream));
+    e->texf.pool = (const uchar4*)e->d_texf_pool.p; e->texf.table = (const uint2*)e->d_texf_table.p;
+    e->texf_pool_texels = total; e->texf_built = true; e->texture_mip_builds++;
     return ST_OK;
 }
 
@@ -868,6 +941,8 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     const bool nm = e->nmap_frame;     // normal-mapped shading normals (ST_OPT_NORMAL_MAPS)
     const bool lgon = e->lgrid_frame;  // light-grid candidate lists (ST_OPT_LIGHT_GRID)
     const LightGridDev lgd = e->lgrid;
+    const bool tfon = e->texf_frame;   // filtered material textures (ST_OPT_TEXTURE_FILTER)
+    const TexFilterDev tfd = e->texf;
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
     auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
@@ -881,9 +956,9 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         for (uint32_t depth = 0; depth <= (uint32_t)d.ref_depth; depth++) {
             uint32_t sd = seed(P_REF_SHADING_SEED + depth);
             add(P_REF_TRACING, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_ref_tracing(cam, sc, depth, nm, s); });
-            add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, sd, depth, lgon ? &lgd : nullptr, s); });
+            add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, sd, depth, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, s); });
         }
-        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, s); });
+        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, nullptr, s); });
         add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, 6u, di_final, gi_final, s); });
         return;
     }
@@ -892,7 +967,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     // K4 inside the G-buffer launch: only where nothing has to happen between the two (a strip pulls last frame's rows in between,
     // unless nothing moved: then every reprojected read is the pixel itself)
     const int k4_in_k0 = (e->fused_passes && (ext == nullptr || ext->still) && !e->instances.empty()) ? 1 : 0;
-    add(P_PRIM_GBUFFER, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_prim_gbuffer(camG, sc, cur, k4_in_k0, nm, s); });
+    add(P_PRIM_GBUFFER, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_prim_gbuffer(camG, sc, cur, k4_in_k0, nm, tfon ? &tfd : nullptr, s); });
     // ST_OPT_FUSED_PASSES: passes whose hand-over is private to a pixel (or to a checkerboard pair) run as one launch; the step keeps
     // the pass id of the member that gathers from other pixels, which is what the strip plans key on.
     const bool fp = e->fused_passes;
@@ -919,8 +994,8 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
             const int inline_rp = (fp && tracing) ? 1 : 0;   // K11 inside K14; validation frames keep K11 (K12 / K13 read its output)
             if (!inline_rp) add(P_GI_REPROJECTION, [=](cudaStream_t s) { (fs ? stf::launch_gi_reprojection : st::launch_gi_reprojection)(cam, sc, cur, s); });
             auto sampling = [&]() {
-                if (fp) { add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, nm, lgon ? &lgd : nullptr, s); }); return; }
-                add(P_GI_SAMPLING_A, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, nm, s); });
+                if (fp) { add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, nm, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, s); }); return; }
+                add(P_GI_SAMPLING_A, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, nm, tfon ? &tfd : nullptr, s); });
                 add(P_GI_SAMPLING_B, [=](cudaStream_t s) { (fs ? stf::launch_gi_sampling_b : st::launch_gi_sampling_b)(cam, sc, cur, sb, f, lgon ? &lgd : nullptr, s); });
             };
             if (tracing) {
@@ -1361,7 +1436,7 @@ void st_engine_destroy(st_engine* e) {
     if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
     for (CameraSlot* c : e->cameras) { for (int k = 0; k < 2; k++) { if (c->side[k]) { cudaStreamSynchronize(c->side[k]); cudaStreamDestroy(c->side[k]); } if (c->ev_pushed[k]) cudaEventDestroy(c->ev_pushed[k]); } if (c->ev_produced) cudaEventDestroy(c->ev_produced);
         c->arena.release(); c->svgf_pairs.release(); c->rgba8.release(); for (int k = 0; k < 2; k++) { if (c->ev_ready[k]) cudaEventDestroy(c->ev_ready[k]); if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]); } delete c; }
-    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake, &e->d_lgrid};
+    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake, &e->d_lgrid, &e->d_texf_pool, &e->d_texf_table, &e->d_texf_jobs};
     for (DevMem* d : all) d->release();
     for (auto& m : e->d_meshes) m.second.release();
     for (int k = 0; k < 2; k++) { if (e->staging[k]) cudaFreeHost(e->staging[k]); if (e->staging_ev[k]) cudaEventDestroy(e->staging_ev[k]); }
@@ -1566,6 +1641,7 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
     if (!e) return fail(ST_ERR_INVALID, "null engine");
     CK(cudaSetDevice(e->device));
     int rc; bool too_deep = false;
+    const bool textures_changed = e->materials_dirty || e->images_dirty;
     if (e->materials_dirty || e->images_dirty) {   // Materials::refresh + Material::serialize (materials.rs:79-85, material.rs:29-50)
         e->materials_dirty = false; e->images_dirty = false;
         auto rect = [&](const st_engine::MatTex& mt, int k) {   // Images::lookup (images.rs:114-127)
@@ -1590,6 +1666,10 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
             const float4 r = g.normal_map_texture;
             if (r.x != 0.0f || r.y != 0.0f || r.z != 0.0f || r.w != 0.0f) e->any_normal_map = true;
         }
+        e->any_color_texture = false;
+        for (const GpuMaterial& g : e->h_materials)
+            for (const float4 r : {g.base_color_texture, g.emissive_texture, g.metallic_roughness_texture})
+                if (r.x != 0.0f || r.y != 0.0f || r.z != 0.0f || r.w != 0.0f) e->any_color_texture = true;
         if ((rc = upload(e, e->d_materials, e->h_materials.data(), e->h_materials.size() * sizeof(GpuMaterial)))) return rc;
         if ((rc = e->d_matpacked.ensure(e->h_materials.size() * 4))) return rc;
         launch_material_derive((const GpuMaterial*)e->d_materials.p, (uint32_t)e->h_materials.size(), (uint32_t*)e->d_matpacked.p, e->stream);
@@ -1672,6 +1752,12 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
     e->lgrid_frame = e->light_grid > 0;
     for (CameraSlot* c : e->cameras) if (c->alive) c->frame = e->frame;   // CameraController::flush (camera_controller.rs:81-85)
     e->nmap_frame = e->normal_maps && e->any_normal_map;
+    // ST_OPT_TEXTURE_FILTER: the chains follow the images and materials just uploaded; the pool exists only while the option is on
+    if (!e->texture_filter) {
+        if (e->texf_built || e->d_texf_pool.p) { e->d_texf_pool.release(); e->d_texf_table.release(); e->d_texf_jobs.release(); e->texf = TexFilterDev{}; }
+        e->texf_built = false;
+    } else if (textures_changed || !e->texf_built) { if ((rc = build_texture_mips(e))) return rc; }
+    e->texf_frame = e->texture_filter && e->any_color_texture;
     e->frame += 1;
     if (too_deep) return fail(ST_ERR_LIMIT, "BVH deeper than the 24-entry traversal stack (strolle-gpu/src/lib.rs:72-76): the scene is not drawn until it changes");
     return ST_OK;
@@ -1785,6 +1871,18 @@ int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap, size_t
         if (dst) std::memcpy(dst, w.data(), 4 * std::min(cap, w.size()));
         return ST_OK;
     }
+    if (s == "texture_mips") {   // {pool texels, materials}, the table, the pool (include/strolle_b200.h)
+        if (!e->texf_built) return fail(ST_ERR_NOT_FOUND, "no mip chains: ST_OPT_TEXTURE_FILTER is off or no st_tick has built them");
+        std::vector<uint32_t> w = {(uint32_t)e->texf_pool_texels, (uint32_t)e->h_materials.size()};
+        for (const uint2& t : e->h_texf_table) { w.push_back(t.x); w.push_back(t.y); }
+        const size_t head = w.size();
+        w.resize(head + e->texf_pool_texels);
+        CK(cudaStreamSynchronize(e->stream));
+        if (e->texf_pool_texels) CK(cudaMemcpy(w.data() + head, e->d_texf_pool.p, e->texf_pool_texels * 4, cudaMemcpyDeviceToHost));
+        *count = w.size();
+        if (dst) std::memcpy(dst, w.data(), 4 * std::min(cap, w.size()));
+        return ST_OK;
+    }
     if (s == "triangles") { dev = e->d_triangles.p; n = e->h_triangles.size() * 4; }
     else if (s == "bvh") { dev = e->d_bvh.p; n = e->bvh_out.buf.size() * 4; }
     else if (s == "materials") { dev = e->d_materials.p; n = e->h_materials.size() * 28; }
@@ -1834,7 +1932,7 @@ int st_device_math(st_engine* e, int op, const float* a, const float* b, float* 
     if ((rc = da.ensure(n * 4)) || (rc = db.ensure(n * 4)) || (rc = dc.ensure(n * 4))) return rc;
     CK(cudaMemcpyAsync(da.p, a, n * 4, cudaMemcpyHostToDevice, e->stream));
     if (b) CK(cudaMemcpyAsync(db.p, b, n * 4, cudaMemcpyHostToDevice, e->stream));
-    // op 0-6: the strict elementary functions; op 16-21: the fast-shading build's sin, cos, exp, pow, sqrt and division
+    // op 0-6: the strict elementary functions, op 7: the texture filter's log2; op 16-21: the fast-shading build's sin, cos, exp, pow, sqrt and division
     if (op >= 16) stf::launch_math_shading(op - 16, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
     else launch_math(op, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
     CK(cudaMemcpyAsync(out, dc.p, n * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -1862,6 +1960,10 @@ int st_set_option(st_engine* e, int option, int value) {
     if (option == ST_OPT_LIGHT_GRID) {   // takes effect at the next st_tick
         if (value < 0 || value > 64) return fail(ST_ERR_INVALID, "ST_OPT_LIGHT_GRID: 0 (off) or 1..64 cells along the longest axis");
         e->light_grid = value; return ST_OK;
+    }
+    if (option == ST_OPT_TEXTURE_FILTER) {   // takes effect at the next st_tick
+        if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_TEXTURE_FILTER: 0 (nearest level-0 texel) or 1 (filtered)");
+        e->texture_filter = value == 1; return ST_OK;
     }
     if (option == ST_OPT_BVH_REFIT) { if (value < 0) return fail(ST_ERR_INVALID, "ST_OPT_BVH_REFIT: 0 or a positive budget"); e->bvh_refit = value; return ST_OK; }
     return fail(ST_ERR_INVALID, "unknown option");
@@ -1907,6 +2009,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_NORMAL_MAP_LAUNCHES) { *value = e->normal_map_launches; return ST_OK; }
     if (stat == ST_STAT_BVH_REFITS) { *value = e->bvh_refits; return ST_OK; }
     if (stat == ST_STAT_LIGHT_GRID_BUILDS) { *value = e->light_grid_builds; return ST_OK; }
+    if (stat == ST_STAT_TEXTURE_MIP_BUILDS) { *value = e->texture_mip_builds; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
         CK(cudaSetDevice(e->device)); CK(cudaStreamSynchronize(e->stream));
         uint64_t total = 0;

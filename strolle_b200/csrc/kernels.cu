@@ -153,8 +153,9 @@ template <int ALL, int ONE> struct LbMin { static constexpr int value = ALL > 0 
 ST_DEV float4 frame_reprojection_px(const CameraDev& cam, int cur, Px p, float4 surface_texel, float4 vel);
 // `with_reprojection` (ST_OPT_FUSED_PASSES; single GPU, or a strip on a frame where nothing moved): K4 runs in this launch too — its inputs for the pixel are still in registers
 // NMAP (ST_OPT_NORMAL_MAPS, only while some material has a normal map): the shading normal is the mapped one (nmap_normal)
-template <bool NMAP>
-__global__ void ST_LB_PRIM_GBUFFER k_prim_gbuffer(KPARAMS, int cur, int with_reprojection) {
+// TEXF (ST_OPT_TEXTURE_FILTER, only while some material has a colour texture): the material's textures are filtered (texf_sample)
+template <bool NMAP, bool TEXF>
+__global__ void ST_LB_PRIM_GBUFFER k_prim_gbuffer(KPARAMS, int cur, int with_reprojection, const __grid_constant__ TexFilterDev tf) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
@@ -166,8 +167,18 @@ __global__ void ST_LB_PRIM_GBUFFER k_prim_gbuffer(KPARAMS, int cur, int with_rep
         const GpuMaterial m = sc.materials[th.material_id];
         if (NMAP) th.normal = nmap_normal(sc, th, m.normal_map_texture);
         GBuf g;
-        float2 mr = mat_metallic_roughness(sc, m, th.uv);
-        g.base_color = mat_base_color(sc, m, th.uv); g.normal = th.normal; g.metallic = mr.x; g.emissive = mat_emissive(sc, m, th.uv);
+        float2 mr;
+        if (TEXF) {
+            TexFoot ft; ft.tri = th.triangle_id; ft.dir = ray.d; ft.w = texf_cone_width(cam.curr, p.x, p.y, th.t, true);
+            const float4 t = texf_sample(sc, tf, th.material_id, 2u, m.metallic_roughness_texture, f4(1.0f, m.roughness, m.metallic, 1.0f), th.uv, ft);
+            mr = f2(t.z, t.y);
+            g.base_color = texf_sample(sc, tf, th.material_id, 0u, m.base_color_texture, m.base_color, th.uv, ft);
+            g.emissive = xyz(texf_sample(sc, tf, th.material_id, 1u, m.emissive_texture, m.emissive, th.uv, ft));
+        } else {
+            mr = mat_metallic_roughness(sc, m, th.uv);
+            g.base_color = mat_base_color(sc, m, th.uv); g.emissive = mat_emissive(sc, m, th.uv);
+        }
+        g.normal = th.normal; g.metallic = mr.x;
         g.roughness = mr.y; g.reflectance = m.reflectance; g.depth = dist(ray.o, th.point);
         // untextured base colour: its gamma-encoded bytes come from the per-material table
         gbuf_pack_pre(g, all_zero(m.base_color_texture) ? __ldg(sc.material_packed + th.material_id) : gbuf_pack_color(g.base_color), &g0, &g1);
@@ -499,8 +510,10 @@ __global__ void __launch_bounds__(ST_BLOCK) k_gi_reprojection(KPARAMS, int cur) 
 // K12 gi_sampling_a::main (gi_sampling_a.rs:4-122)
 // returns false where the kernel leaves without writing its three scratch texels (gi_d0: ray direction + pdf, gi_d1/gi_d2: the packed
 // G-buffer entry of what the ray hit)
-template <bool NMAP>
-ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4* t0, float4* t1, float4* t2) {
+// TEXF: the bounce hit's textures are filtered, with a fresh cone from the segment's origin
+template <bool NMAP, bool TEXF>
+ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4* t0, float4* t1, float4* t2,
+                               const TexFilterDev& tf) {
     bool tracing = gi_tracing_frame(frame);
     uint2 sp = tracing ? checker(g.x, g.y, frame / 2u) : checker(g.x, g.y, frame);
     if (!cam_contains_u(cam.curr, sp.x, sp.y)) return false;
@@ -525,7 +538,14 @@ ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const T
     if (trihit_some(gh)) {
         GpuMaterial m = sc.materials[gh.material_id];
         m.roughness = rmax(m.roughness, 0.75f * 0.75f);   // Material::regularize (material.rs:25-27)
-        gg.base_color = mat_base_color(sc, m, gh.uv); gg.normal = NMAP ? nmap_normal(sc, gh, m.normal_map_texture) : gh.normal; gg.metallic = m.metallic; gg.emissive = mat_emissive(sc, m, gh.uv);
+        if (TEXF) {
+            TexFoot ft; ft.tri = gh.triangle_id; ft.dir = gi_r.d; ft.w = texf_cone_width(cam.curr, sp.x, sp.y, gh.t, false);
+            gg.base_color = texf_sample(sc, tf, gh.material_id, 0u, m.base_color_texture, m.base_color, gh.uv, ft);
+            gg.emissive = xyz(texf_sample(sc, tf, gh.material_id, 1u, m.emissive_texture, m.emissive, gh.uv, ft));
+            gg.normal = NMAP ? nmap_normal(sc, gh, m.normal_map_texture) : gh.normal; gg.metallic = m.metallic;
+        } else {
+            gg.base_color = mat_base_color(sc, m, gh.uv); gg.normal = NMAP ? nmap_normal(sc, gh, m.normal_map_texture) : gh.normal; gg.metallic = m.metallic; gg.emissive = mat_emissive(sc, m, gh.uv);
+        }
         gi_color_bits = all_zero(m.base_color_texture) ? __ldg(sc.material_packed + gh.material_id) : gbuf_pack_color(gg.base_color);
         gg.roughness = m.roughness; gg.reflectance = m.reflectance; gg.depth = dist(gi_r.o, gh.point);
     }
@@ -533,13 +553,13 @@ ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const T
     *t0 = f4(gi_r.d, gi_pdf_);
     return true;
 }
-template <bool NMAP>
-__global__ void ST_LB_GI_SAMPLING_A k_gi_sampling_a(KPARAMS, int cur, u32 seed, u32 frame) {
+template <bool NMAP, bool TEXF>
+__global__ void ST_LB_GI_SAMPLING_A k_gi_sampling_a(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ TexFilterDev tf) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
-    if (!gi_sampling_a_pair<NMAP>(cam, sc, stk, cur, seed, frame, g, &t0, &t1, &t2)) return;
+    if (!gi_sampling_a_pair<NMAP, TEXF>(cam, sc, stk, cur, seed, frame, g, &t0, &t1, &t2, tf)) return;
     size_t gi = pix(cam, g.x, g.y);
     cam.gi_d0[gi] = t0; cam.gi_d1[gi] = t1; cam.gi_d2[gi] = t2;
 }
@@ -614,13 +634,14 @@ __global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, 
 }
 // K12 + K13 in one launch (ST_OPT_FUSED_PASSES): the bounce ray is traced and shaded by the same thread; the hit still goes through
 // GBufferEntry's pack / unpack (its 8-bit quantisation is part of the result), just not through memory.
-template <bool NMAP, bool LGRID>
-__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_fused(KPARAMS, int cur, u32 seed_a, u32 seed_b, u32 frame, const __grid_constant__ LightGridDev lg) {
+template <bool NMAP, bool LGRID, bool TEXF>
+__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_fused(KPARAMS, int cur, u32 seed_a, u32 seed_b, u32 frame, const __grid_constant__ LightGridDev lg,
+                                                        const __grid_constant__ TexFilterDev tf) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
-    if (!gi_sampling_a_pair<NMAP>(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2)) return;
+    if (!gi_sampling_a_pair<NMAP, TEXF>(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2, tf)) return;
     gi_sampling_b_pair<LGRID>(cam, sc, stk, cur, seed_b, frame, g, t0, t1, t2, lg);
 }
 
@@ -1278,8 +1299,11 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
 }
 
 // K2 ref_shading::main (ref_shading.rs:4-177); LGRID: the one light is drawn from the light grid's list for the nudged hit point
-template <bool LGRID>
-__global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32 depth, const __grid_constant__ LightGridDev lg) {
+// TEXF: the hit's textures are filtered; the packed hit carries no triangle, so the segment's ray is traced again (same ray, same
+// BVH: the same triangle and distance)
+template <bool LGRID, bool TEXF>
+__global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32 depth, const __grid_constant__ LightGridDev lg,
+                                                          const __grid_constant__ TexFilterDev tf) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
@@ -1309,7 +1333,14 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32
     if (depth > 0u) m.roughness = rmax(m.roughness, 0.75f * 0.75f);
     Hit hit;
     hit.point = th.point + th.normal * 0.01f; hit.origin = ray.o; hit.dir = ray.d;
-    hit.g.base_color = mat_base_color(sc, m, th.uv); hit.g.normal = th.normal; hit.g.metallic = m.metallic; hit.g.emissive = mat_emissive(sc, m, th.uv);
+    if (TEXF) {
+        const TriHit again = trace_closest(ray, sc, stk);
+        uncount_ray(sc);
+        TexFoot ft; ft.tri = again.triangle_id; ft.dir = ray.d; ft.w = texf_cone_width(cam.curr, p.x, p.y, again.t, depth == 0u);
+        hit.g.base_color = texf_sample(sc, tf, th.material_id, 0u, m.base_color_texture, m.base_color, th.uv, ft);
+        hit.g.emissive = xyz(texf_sample(sc, tf, th.material_id, 1u, m.emissive_texture, m.emissive, th.uv, ft));
+    } else { hit.g.base_color = mat_base_color(sc, m, th.uv); hit.g.emissive = mat_emissive(sc, m, th.uv); }
+    hit.g.normal = th.normal; hit.g.metallic = m.metallic;
     hit.g.roughness = m.roughness; hit.g.reflectance = m.reflectance; hit.g.depth = 0.0f;
     color = color + thr * hit.g.emissive;
     const LgList list = LGRID ? lgrid_list(lg, hit.point) : LgList{nullptr, sc.world.light_count};
@@ -1383,6 +1414,43 @@ __global__ void k_math(int op, const float* __restrict__ a, const float* __restr
         case 6: r = acos_approx_glam(a[i]); break;
     }
     out[i] = r;
+}
+// st_device_math op 7: the level of detail's log2 (ST_OPT_TEXTURE_FILTER)
+__global__ void k_math_log2(const float* __restrict__ a, float* __restrict__ out, long n) {
+    long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = log2_x(a[i]);
+}
+
+// ST_OPT_TEXTURE_FILTER: level k+1 of the images of `jobs` (blockIdx.y) from their level k, one thread per output texel.  Texel (x, y)
+// averages level-k texels (min(2x + i, w - 1), min(2y + j, h - 1)), i, j in {0, 1}: r, g, b decoded through the sRGB table, summed
+// ((c00 + c10) + c01) + c11, times 0.25, re-encoded to the byte whose table value is nearest (ties to the lower byte: the count of the
+// 255 midpoints below the value); alpha (a00 + a10 + a01 + a11 + 2) >> 2.
+__global__ void __launch_bounds__(256) k_texture_mips(const MipJob* __restrict__ jobs, const uchar4* __restrict__ atlas, uchar4* __restrict__ pool,
+                                                      const float* __restrict__ srgb) {
+    __shared__ float lut[256], mid[255];
+    lut[threadIdx.x] = srgb[threadIdx.x];
+    __syncthreads();
+    if (threadIdx.x < 255u) mid[threadIdx.x] = xmul(xadd(lut[threadIdx.x], lut[threadIdx.x + 1u]), 0.5f);
+    __syncthreads();
+    const MipJob j = jobs[blockIdx.y];
+    const u32 i = blockIdx.x * 256u + threadIdx.x;
+    if (i >= j.dst_w * j.dst_h) return;
+    const u32 x = i % j.dst_w, y = i / j.dst_w;
+    const u32 xa = min(2u * x, j.src_w - 1u), xb = min(2u * x + 1u, j.src_w - 1u), ya = min(2u * y, j.src_h - 1u), yb = min(2u * y + 1u, j.src_h - 1u);
+    const uchar4* src = (j.from_atlas ? atlas : pool) + j.src;
+    const size_t st = j.src_stride;
+    const uchar4 c00 = src[ya * st + xa], c10 = src[ya * st + xb], c01 = src[yb * st + xa], c11 = src[yb * st + xb];
+    const u32 b0[3] = {c00.x, c00.y, c00.z}, b1[3] = {c10.x, c10.y, c10.z}, b2[3] = {c01.x, c01.y, c01.z}, b3[3] = {c11.x, c11.y, c11.z};
+    u32 out[3];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const float s = xmul(xadd(xadd(xadd(lut[b0[c]], lut[b1[c]]), lut[b2[c]]), lut[b3[c]]), 0.25f);
+        u32 b = 0u;
+        for (u32 step = 128u; step > 0u; step >>= 1) if (b + step <= 255u && mid[b + step - 1u] < s) b += step;
+        out[c] = b;
+    }
+    const u32 a = ((u32)c00.w + (u32)c10.w + (u32)c01.w + (u32)c11.w + 2u) >> 2;
+    pool[j.dst + i] = make_uchar4((unsigned char)out[0], (unsigned char)out[1], (unsigned char)out[2], (unsigned char)a);
 }
 
 // ST_OPT_LIGHT_GRID: the candidate lists (DESIGN.md §2 "Light grid").  One warp per cell, the outside list last (cell == ncell: no
@@ -1624,8 +1692,13 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_sample, c, st, c, s, seed, frame); }
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_di_resolving<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_gi_reprojection<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, cudaStream_t st) {
-    if (nmap) HALF_LAUNCH(k_gi_sampling_a<true>, c, st, c, s, cur, seed, frame); else HALF_LAUNCH(k_gi_sampling_a<false>, c, st, c, s, cur, seed, frame);
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st) {
+    if (tf) {
+        if (nmap) HALF_LAUNCH((k_gi_sampling_a<true, true>), c, st, c, s, cur, seed, frame, *tf); else HALF_LAUNCH((k_gi_sampling_a<false, true>), c, st, c, s, cur, seed, frame, *tf);
+    } else {
+        const TexFilterDev none{};
+        if (nmap) HALF_LAUNCH((k_gi_sampling_a<true, false>), c, st, c, s, cur, seed, frame, none); else HALF_LAUNCH((k_gi_sampling_a<false, false>), c, st, c, s, cur, seed, frame, none);
+    }
 }
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st) {
     if (lg) HALF_LAUNCH(k_gi_sampling_b<true>, c, st, c, s, cur, seed, frame, *lg); else HALF_LAUNCH(k_gi_sampling_b<false>, c, st, c, s, cur, seed, frame, LightGridDev{});
@@ -1640,20 +1713,33 @@ void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u
     else k_di_sample_temporal<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed_sampling, seed_temporal, frame, LightGridDev{});
 }
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, cudaStream_t st) {
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf,
+                              cudaStream_t st) {
     const LightGridDev none{};
-    if (lg) {
-        if (nmap) HALF_LAUNCH((k_gi_sampling_fused<true, true>), c, st, c, s, cur, seed_a, seed_b, frame, *lg); else HALF_LAUNCH((k_gi_sampling_fused<false, true>), c, st, c, s, cur, seed_a, seed_b, frame, *lg);
+    const LightGridDev& g = lg ? *lg : none;
+    const TexFilterDev tnone{};
+    const TexFilterDev& t = tf ? *tf : tnone;
+#define ST_GSF(N_, L_, T_) HALF_LAUNCH((k_gi_sampling_fused<N_, L_, T_>), c, st, c, s, cur, seed_a, seed_b, frame, g, t)
+    if (tf) {
+        if (lg) { if (nmap) ST_GSF(true, true, true); else ST_GSF(false, true, true); }
+        else { if (nmap) ST_GSF(true, false, true); else ST_GSF(false, false, true); }
     } else {
-        if (nmap) HALF_LAUNCH((k_gi_sampling_fused<true, false>), c, st, c, s, cur, seed_a, seed_b, frame, none); else HALF_LAUNCH((k_gi_sampling_fused<false, false>), c, st, c, s, cur, seed_a, seed_b, frame, none);
+        if (lg) { if (nmap) ST_GSF(true, true, false); else ST_GSF(false, true, false); }
+        else { if (nmap) ST_GSF(true, false, false); else ST_GSF(false, false, false); }
     }
+#undef ST_GSF
 }
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st) { k_gi_preview_resolve<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, in, source); }
 void launch_math_shading(int op, const float* a, const float* b, float* out, long n, cudaStream_t st) { k_math_shading<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n); }
 #if ST_EXACT_ONLY
-void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, cudaStream_t st) {
-    if (nmap) k_prim_gbuffer<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, with_reprojection); else k_prim_gbuffer<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, with_reprojection);
+void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, const TexFilterDev* tf, cudaStream_t st) {
+    const TexFilterDev none{};
+    const TexFilterDev& t = tf ? *tf : none;
+#define ST_PG(N_, T_) k_prim_gbuffer<N_, T_><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, with_reprojection, t)
+    if (tf) { if (nmap) ST_PG(true, true); else ST_PG(false, true); }
+    else { if (nmap) ST_PG(true, false); else ST_PG(false, false); }
+#undef ST_PG
 }
 void launch_frame_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_frame_reprojection<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
 void launch_denoise_reproject(const CameraDev& c, const SceneDev& s, int cur, const float4* pc, const float4* pm, const float4* smp, float4* col, float4* mom, cudaStream_t st) { k_denoise_reproject<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, pc, pm, smp, col, mom); }
@@ -1858,13 +1944,37 @@ void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cud
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {
     if (nmap) k_ref_tracing<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); else k_ref_tracing<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth);
 }
-void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, cudaStream_t st) {
-    if (lg) k_ref_shading<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, *lg); else k_ref_shading<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, LightGridDev{});
+void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st) {
+    const LightGridDev none{};
+    const LightGridDev& g = lg ? *lg : none;
+    const TexFilterDev tnone{};
+    const TexFilterDev& t = tf ? *tf : tnone;
+#define ST_RS(L_, T_) k_ref_shading<L_, T_><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, g, t)
+    if (tf) { if (lg) ST_RS(true, true); else ST_RS(false, true); }
+    else { if (lg) ST_RS(true, false); else ST_RS(false, false); }
+#undef ST_RS
+}
+// ST_OPT_TEXTURE_FILTER: one launch per level (split into launches of at most 65535 images, the grid's y limit), `first[k]` ..
+// `first[k + 1]` the jobs of level k + 1, `blocks[k]` their widest grid; returns the first launch error
+cudaError_t launch_texture_mips(const MipJob* jobs, const u32* first, const u32* blocks, int levels, const uchar4* atlas, uchar4* pool, const float* srgb,
+                                cudaStream_t st) {
+    for (int k = 0; k < levels; k++) {
+        if (!blocks[k]) continue;
+        for (u32 j = first[k]; j < first[k + 1]; j += 65535u) {
+            const u32 n = min(first[k + 1] - j, 65535u);
+            k_texture_mips<<<dim3(blocks[k], n), 256, 0, st>>>(jobs + j, atlas, pool, srgb);
+            const cudaError_t err = cudaGetLastError();
+            if (err != cudaSuccess) return err;
+        }
+    }
+    return cudaSuccess;
 }
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st) { k_bvh_heatmap<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s); }
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st) { k_trace_stream_closest<<<(unsigned)((n + ST_BLOCK - 1) / ST_BLOCK), ST_BLOCK, 0, st>>>(s, rays, n, out); }
 void launch_trace_stream_any(const SceneDev& s, const float4* rays, long n, u32* out, cudaStream_t st) { k_trace_stream_any<<<(unsigned)((n + ST_BLOCK - 1) / ST_BLOCK), ST_BLOCK, 0, st>>>(s, rays, n, out); }
-void launch_math(int op, const float* a, const float* b, float* out, long n, cudaStream_t st) { k_math<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n); }
+void launch_math(int op, const float* a, const float* b, float* out, long n, cudaStream_t st) {
+    if (op == 7) k_math_log2<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, out, n); else k_math<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n);
+}
 void launch_light_grid_build(const LightGridDev& lg, const GpuLight* lights, cudaStream_t st) {
     const u32 ncell = lg.dims[0] * lg.dims[1] * lg.dims[2];
     k_light_grid_build<<<(ncell + 1u + 3u) / 4u, 128, 0, st>>>(lg, lights, ncell, const_cast<u32*>(lg.counts), const_cast<u32*>(lg.lists));

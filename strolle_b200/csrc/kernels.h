@@ -6,8 +6,9 @@
 namespace st {
 typedef uint32_t u32;
 
-// nmap: the NMAP instantiation (normal-mapped shading normal, ST_OPT_NORMAL_MAPS) of the kernels that shade a closest hit
-void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, cudaStream_t st);
+// nmap: the NMAP instantiation (normal-mapped shading normal, ST_OPT_NORMAL_MAPS) of the kernels that shade a closest hit;
+// tf (non-null): their TEXF instantiation (filtered material textures, ST_OPT_TEXTURE_FILTER)
+void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, const TexFilterDev* tf, cudaStream_t st);
 void launch_frame_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_di_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, cudaStream_t st);
@@ -16,7 +17,7 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, cudaStream_t st);
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st);
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
@@ -25,7 +26,7 @@ void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed,
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st);
 void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, cudaStream_t st);
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st);
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st);
 void launch_denoise_reproject(const CameraDev& c, const SceneDev& s, int cur, const float4* pc, const float4* pm, const float4* smp, float4* col, float4* mom, cudaStream_t st);
@@ -37,13 +38,16 @@ bool launch_denoise_variance_tiled(const CameraDev& c, const SceneDev& s, int cu
 void launch_composition(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, cudaStream_t st);
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st);
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st);
-void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, cudaStream_t st);
+void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st);
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st);
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st);
 void launch_trace_stream_any(const SceneDev& s, const float4* rays, long n, u32* out, cudaStream_t st);
 void launch_math(int op, const float* a, const float* b, float* out, long n, cudaStream_t st);
 // ST_OPT_LIGHT_GRID: fills lg.counts / lg.lists (dims.x * dims.y * dims.z cells, then the outside list) from the device lights
 void launch_light_grid_build(const LightGridDev& lg, const GpuLight* lights, cudaStream_t st);
+// ST_OPT_TEXTURE_FILTER: k_texture_mips for level k + 1 over jobs [first[k], first[k + 1]) with blocks[k] x 256 threads, k < levels,
+// in launches of at most 65535 jobs; returns the first launch error
+cudaError_t launch_texture_mips(const MipJob* jobs, const u32* first, const u32* blocks, int levels, const uchar4* atlas, uchar4* pool, const float* srgb, cudaStream_t st);
 void launch_material_derive(const GpuMaterial* mats, u32 n, u32* packed, cudaStream_t st);
 void launch_srgb_lut(float* lut, cudaStream_t st);
 void launch_unpack_lut(float* lut, cudaStream_t st);
@@ -100,7 +104,7 @@ void launch_refit(const uint4* runs, u32 nruns, const uint2* nodes, const u32* l
 // The ReSTIR kernels K5-K19 built a second time with FMA contraction and SFU approximations (kernels.cu compiled with
 // -DST_FAST=1, see st_math.cuh): same launch interface, selected by ST_OPT_SHADING_FAST_MATH.
 namespace stf {
-using st::CameraDev; using st::SceneDev; using st::LightGridDev; using st::u32;
+using st::CameraDev; using st::SceneDev; using st::LightGridDev; using st::TexFilterDev; using st::u32;
 int preload_kernels();   // the fast-shading build's kernels
 void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_di_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, cudaStream_t st);
@@ -109,7 +113,7 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, cudaStream_t st);
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st);
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
@@ -118,7 +122,7 @@ void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed,
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st);
 void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, cudaStream_t st);
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st);
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st);
 void launch_math_shading(int op, const float* a, const float* b, float* out, long n, cudaStream_t st);   // test hook: this build's sin/cos/exp/pow/sqrt/div

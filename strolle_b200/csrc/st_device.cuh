@@ -403,6 +403,115 @@ ST_DEV bool cam_is_eq(const GpuCamera& a, const GpuCamera& b) {   // camera.rs:1
     return ok;
 }
 
+// ---- Texture filtering (ST_OPT_TEXTURE_FILTER; DESIGN.md §2 "Texture filtering") ------------------------------------------------
+// The level of detail, the texel addresses and the weights use the x*() primitives only, so the filtered value is the same in the
+// strict and the fast-shading builds.
+// log2 of a finite x > 0: the exponent bits plus the Cephes logf polynomial of the mantissa, times log2(e) (st_device_math op 7)
+ST_DEV float log2_x(float x) {
+    u32 bits = fbits(x);
+    int e;
+    if ((bits & 0x7f800000u) == 0u) { x = xmul(x, 8388608.0f); bits = fbits(x); e = (int)((bits >> 23) & 0xffu) - 126 - 23; }
+    else e = (int)((bits >> 23) & 0xffu) - 126;
+    float m = bitsf((bits & 0x007fffffu) | 0x3f000000u);   // [0.5, 1)
+    if (m < 0.707106781186547524f) { e -= 1; m = xsub(xadd(m, m), 1.0f); } else m = xsub(m, 1.0f);
+    const float z = xmul(m, m);
+    float y = 7.0376836292e-2f;
+    y = xadd(xmul(y, m), -1.1514610310e-1f); y = xadd(xmul(y, m), 1.1676998740e-1f); y = xadd(xmul(y, m), -1.2420140846e-1f);
+    y = xadd(xmul(y, m), 1.4249322787e-1f); y = xadd(xmul(y, m), -1.6668057665e-1f); y = xadd(xmul(y, m), 2.0000714765e-1f);
+    y = xadd(xmul(y, m), -2.4999993993e-1f); y = xadd(xmul(y, m), 3.3333331174e-1f);
+    y = xmul(xmul(y, m), z);
+    y = xadd(y, xmul(-0.5f, z));
+    const float ln_m = xadd(m, y);   // ln(1 + m), m in [sqrt(1/2) - 1, sqrt(2) - 1)
+    return xadd(xmul(ln_m, 1.44269504088896341f), (float)e);
+}
+ST_DEV float xlen(float3 a) { return xsqrt(xdot(a, a)); }
+ST_DEV float4 xscale4(float4 a, float s) { return f4(xmul(a.x, s), xmul(a.y, s), xmul(a.z, s), xmul(a.w, s)); }
+ST_DEV float4 xadd4(float4 a, float4 b) { return f4(xadd(a.x, b.x), xadd(a.y, b.y), xadd(a.z, b.z), xadd(a.w, b.w)); }
+// cam_ray through the x*() primitives (the same bits as cam_ray in the strict build)
+ST_DEV void cam_ray_x(const GpuCamera& c, u32 px, u32 py, float3* o, float3* d) {
+    const Mat4& m = cam_n2w(c);
+    const float nx = xsub(xdiv(xmul(xadd((float)px, 0.5f), 2.0f), c.screen.x), 1.0f);
+    const float ny = -xsub(xdiv(xmul(xadd((float)py, 0.5f), 2.0f), c.screen.y), 1.0f);
+    float3 pl[2];
+    const float zs[2] = {kF32Eps, 1.0f};
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+        float4 r = xscale4(m.c[0], nx);
+        r = xadd4(r, xscale4(m.c[1], ny)); r = xadd4(r, xscale4(m.c[2], zs[k])); r = xadd4(r, m.c[3]);
+        const float rw = xdiv(1.0f, r.w);
+        pl[k] = f3(xmul(r.x, rw), xmul(r.y, rw), xmul(r.z, rw));
+    }
+    *o = pl[1]; *d = xnorm(xsub3(pl[0], pl[1]));
+}
+// Ray-cone width at a hit `t` along the ray.  (o0, d0), (o1, d1), (o2, d2): the camera rays of pixel (px, py), (px + 1, py) and
+// (px, py + 1).  Primary hits: max(|(o1 - o0) + t (d1 - d0)|, |(o2 - o0) + t (d2 - d0)|) (perspective and orthographic alike).
+// Secondary hits start a fresh cone at the segment's origin: t max(|d1 - d0|, |d2 - d0|).
+ST_DEV float texf_cone_width(const GpuCamera& c, u32 px, u32 py, float t, bool primary) {
+    float3 o0, d0, o1, d1, o2, d2;
+    cam_ray_x(c, px, py, &o0, &d0); cam_ray_x(c, px + 1u, py, &o1, &d1); cam_ray_x(c, px, py + 1u, &o2, &d2);
+    if (primary) return rmax(xlen(xadd3(xsub3(o1, o0), xscale(xsub3(d1, d0), t))), xlen(xadd3(xsub3(o2, o0), xscale(xsub3(d2, d0), t))));
+    return xmul(t, rmax(xlen(xsub3(d1, d0)), xlen(xsub3(d2, d0))));
+}
+// What the filtered fetch needs of a hit: its triangle, the ray direction and the cone width there
+struct TexFoot { u32 tri; float3 dir; float w; };
+// lambda = 0.5 log2(q), q = A_uv W H w^2 |c| / (c.d)^2, c = (p1 - p0) x (p2 - p0), A_uv = |(uv1 - uv0) x (uv2 - uv0)|, clamped to
+// [0, levels - 1]; q <= 0 or NaN -> 0, q = +inf -> the last level
+ST_DEV float texf_lambda(const SceneDev& sc, const TexFoot& f, u32 W, u32 H, u32 levels) {
+    const float4* tri = sc.triangles + 9u * (size_t)f.tri;
+    const float4 a0 = ldg4(tri), a1 = ldg4(tri + 1), a3 = ldg4(tri + 3), a4 = ldg4(tri + 4), a6 = ldg4(tri + 6), a7 = ldg4(tri + 7);
+    const float3 p0 = xyz(a0);
+    const float3 c = xcross(xsub3(xyz(a3), p0), xsub3(xyz(a6), p0));
+    const float auv = fabs_(xsub(xmul(xsub(a3.w, a0.w), xsub(a7.w, a1.w)), xmul(xsub(a6.w, a0.w), xsub(a4.w, a1.w))));
+    const float cd = xdot(c, f.dir);
+    const float q = xdiv(xmul(xmul(xmul(xmul(auv, (float)W), (float)H), xmul(f.w, f.w)), xlen(c)), xmul(cd, cd));
+    const float top = (float)(levels - 1u);
+    if (!(q > 0.0f)) return 0.0f;
+    if (q == finf()) return top;
+    return rclamp(xmul(0.5f, log2_x(q)), 0.0f, top);
+}
+// Bilinear on level k of an image (level 0: its atlas rect at (ax, ay), W x H; level 1 at pool texel `off1`): s = u w_k - 0.5,
+// taps floor(s) and floor(s) + 1 modulo w_k (the same for v), rgb decoded through the sRGB table, alpha / 255
+ST_DEV float4 texf_texel(const SceneDev& sc, const uchar4* src, size_t i) {
+    const uchar4 t = __ldg(src + i);
+    return f4(__ldg(sc.srgb_lut + t.x), __ldg(sc.srgb_lut + t.y), __ldg(sc.srgb_lut + t.z), xdiv((float)t.w, 255.0f));
+}
+ST_DEV float4 xlerp4(float4 a, float4 b, float wa, float wb) {
+    return f4(xadd(xmul(a.x, wa), xmul(b.x, wb)), xadd(xmul(a.y, wa), xmul(b.y, wb)), xadd(xmul(a.z, wa), xmul(b.z, wb)), xadd(xmul(a.w, wa), xmul(b.w, wb)));
+}
+ST_DEV float4 texf_bilinear(const SceneDev& sc, const TexFilterDev& tf, u32 ax, u32 ay, u32 W, u32 H, u32 off1, u32 k, float u, float v) {
+    u32 w = W, h = H, off = off1;
+    for (u32 j = 1u; j <= k; j++) { if (j > 1u) off += w * h; w = max(1u, w >> 1); h = max(1u, h >> 1); }
+    const float s = xsub(xmul(u, (float)w), 0.5f), t = xsub(xmul(v, (float)h), 0.5f);
+    const float sx = floorf(s), sy = floorf(t);
+    const float fx = xsub(s, sx), fy = xsub(t, sy);
+    const int ix = max(-1, min(to_i32_sat(sx), (int)w - 1)), iy = max(-1, min(to_i32_sat(sy), (int)h - 1));
+    const u32 xa = ix < 0 ? w - 1u : (u32)ix, xb = (u32)(ix + 1) >= w ? 0u : (u32)(ix + 1);
+    const u32 ya = iy < 0 ? h - 1u : (u32)iy, yb = (u32)(iy + 1) >= h ? 0u : (u32)(iy + 1);
+    const uchar4* src; size_t stride;
+    if (k == 0u) { src = sc.atlas + (size_t)ay * kAtlasSize + ax; stride = kAtlasSize; } else { src = tf.pool + off; stride = w; }
+    const float4 c00 = texf_texel(sc, src, ya * stride + xa), c10 = texf_texel(sc, src, ya * stride + xb);
+    const float4 c01 = texf_texel(sc, src, yb * stride + xa), c11 = texf_texel(sc, src, yb * stride + xb);
+    const float gx = xsub(1.0f, fx), gy = xsub(1.0f, fy);
+    return xlerp4(xlerp4(c00, c10, gx, fx), xlerp4(c01, c11, gx, fx), gy, fy);
+}
+// Material::sample_atlas with the filter: trilinear between levels floor(lambda) and floor(lambda) + 1, times the factor.  `slot`:
+// 0 base colour, 1 emissive, 2 metallic-roughness.
+ST_DEV float4 texf_sample(const SceneDev& sc, const TexFilterDev& tf, u32 material_id, u32 slot, float4 rect, float4 multiplier, float2 hit_uv, const TexFoot& f) {
+    if (all_zero(rect) || !sc.atlas) return sample_atlas(sc, hit_uv, multiplier, rect);
+    const uint2 e = __ldg(tf.table + 3u * (size_t)material_id + slot);
+    const u32 levels = max(e.y, 1u);
+    const u32 ax = to_u32_sat(xmul(rect.x, (float)kAtlasSize)), ay = to_u32_sat(xmul(rect.y, (float)kAtlasSize));
+    const u32 W = to_u32_sat(xmul(rect.z, (float)kAtlasSize)), H = to_u32_sat(xmul(rect.w, (float)kAtlasSize));
+    const float u = wrap_uv(hit_uv.x), v = wrap_uv(hit_uv.y);
+    const float lambda = levels > 1u ? texf_lambda(sc, f, W, H, levels) : 0.0f;
+    const float lf = floorf(lambda);
+    const u32 k0 = (u32)lf;
+    const float fl = xsub(lambda, lf);
+    float4 t = texf_bilinear(sc, tf, ax, ay, W, H, e.x, k0, u, v);
+    if (fl > 0.0f && k0 + 1u < levels) t = xlerp4(t, texf_bilinear(sc, tf, ax, ay, W, H, e.x, k0 + 1u, u, v), xsub(1.0f, fl), fl);
+    return f4(xmul(multiplier.x, t.x), xmul(multiplier.y, t.y), xmul(multiplier.z, t.z), xmul(multiplier.w, t.w));
+}
+
 // ---- Hit / Surface (hit.rs:8-73, surface.rs) -----------------------------------------
 struct Hit { float3 origin, dir, point; GBuf g; };
 ST_DEV Hit hit_zero() { Hit h; h.origin = f3s(0.f); h.dir = f3s(0.f); h.point = f3s(0.f); h.g = gbuf_zero(); return h; }

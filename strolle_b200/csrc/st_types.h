@@ -64,6 +64,18 @@ struct LightGridDev {
     const uint32_t* lists;           // kLightGridK slots per cell, the outside list last
 };
 
+// ST_OPT_TEXTURE_FILTER (DESIGN.md §2 "Texture filtering"): levels 1.. of every live image's mip chain, and per material and colour
+// slot (base colour, emissive, metallic-roughness) {texel offset of the image's level 1 in `pool`, level count}: 0 = no texture, 1 =
+// level 0 only (a 1x1 image, or a stale rect).  Built on the device at st_tick (k_texture_mips); passed by value to the TEXF
+// instantiations of the hit-shading kernels only.
+struct TexFilterDev {
+    const uchar4* pool;     // RGBA8 texels: per image, level after level, each row-major
+    const uint2* table;     // 3 entries per material
+};
+// One image of one k_texture_mips launch: level k+1 (dst_w x dst_h at `dst` in the pool) from level k (src_w x src_h, rows `src_stride`
+// texels apart from `src`, in the atlas for k = 0, else in the pool)
+struct MipJob { uint32_t src, src_stride, src_w, src_h, dst, dst_w, dst_h, from_atlas; };
+
 // Per-camera device buffers: the logical buffers of
 // strolle/src/camera_controller/buffers.rs:53-339 as linear row-major float4
 // arrays indexed by full-frame coordinates (each GPU of a strip-partitioned run

@@ -28,6 +28,7 @@ OPT_SHADING_FAST_MATH = 9  # ReSTIR kernels K5-K19 from the fast-shading build (
 OPT_NORMAL_MAPS = 14         # shade with the materials' normal maps (off by default: the reference ignores them); from the next tick
 OPT_BVH_REFIT = 15           # N > 0: up to N ticks in a row that only move instances bake on the device and refit the BVH (0 = rebuild)
 OPT_LIGHT_GRID = 16          # N in 1..64: light candidates from a world-space grid of N cells along its longest axis (0 = every slot)
+OPT_TEXTURE_FILTER = 17      # 1: material textures filtered through per-image mip chains with a ray-cone level of detail (0 = nearest texel)
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
 STAT_WAVELET_TILED_ERRORS = 2
@@ -39,6 +40,7 @@ STAT_STRIP_FIRST_TIMEOUT = 7
 STAT_NORMAL_MAP_LAUNCHES = 8   # launches of the normal-mapped kernel variants
 STAT_BVH_REFITS = 9            # refit ticks (OPT_BVH_REFIT) since the engine was created
 STAT_LIGHT_GRID_BUILDS = 10    # light grid builds (OPT_LIGHT_GRID) since the engine was created
+STAT_TEXTURE_MIP_BUILDS = 11   # mip-chain builds (OPT_TEXTURE_FILTER) since the engine was created
 
 
 class StrolleError(RuntimeError):
@@ -270,6 +272,9 @@ class Engine:
         a = np.ascontiguousarray(rgba8, dtype=np.uint8)
         self._check(self.lib.st_insert_image(self._h, handle, a.ctypes.data, a.shape[1], a.shape[0]))
 
+    def remove_image(self, handle):
+        self._check(self.lib.st_remove_image(self._h, handle))
+
     def set_material_textures(self, handle, base_color=None, emissive=None, metallic_roughness=None, normal_map=None):
         t = [base_color, emissive, metallic_roughness, normal_map]
         mask = sum((1 << i) for i, v in enumerate(t) if v is not None)
@@ -388,7 +393,7 @@ class Engine:
         return (out, ms.value) if return_ms else out
 
     def device_math(self, op, a, b=None):
-        ops = {"sin": 0, "cos": 1, "acos": 2, "atan2": 3, "exp": 4, "pow": 5, "acos_approx": 6,
+        ops = {"sin": 0, "cos": 1, "acos": 2, "atan2": 3, "exp": 4, "pow": 5, "acos_approx": 6, "log2_lod": 7,
                # the fast-shading build's forms (ST_OPT_SHADING_FAST_MATH): SFU sin / cos / exp / pow, sqrt.approx, div.full
                "sin_fast": 16, "cos_fast": 17, "exp_fast": 18, "pow_fast": 19, "sqrt_fast": 20, "div_fast": 21}
         a = _f(a)

@@ -473,6 +473,47 @@ def textured_room(width=320, height=180, mode=MODE_IMAGE, denoise=True):
                 images=images, material_textures=material_textures)
 
 
+def tiled_ground(width=320, height=180, mode=MODE_IMAGE, denoise=True, ref_depth=1):
+    """Exercises texture filtering (ST_OPT_TEXTURE_FILTER): a large ground plane carrying a 256x256 texture tiled 60 times each way,
+    seen at grazing angles (minification up to the last mip levels); a 45x27 (non-power-of-two) textured wall close to the camera
+    (magnification); an emissive-textured panel; a metallic-roughness-textured box; and an alpha-cut-out fence."""
+    rng = np.random.RandomState(5)
+    yy, xx = np.mgrid[0:256, 0:256]
+    ground = np.zeros((256, 256, 4), np.uint8)
+    m = ((xx // 16) + (yy // 16)) % 2 == 0
+    ground[m] = (230, 220, 200, 255); ground[~m] = (40, 60, 90, 255)
+    ground[(xx % 64) < 2] = (200, 30, 30, 255)                                       # thin lines: the aliasing a minified fetch shows
+    wall = rng.randint(0, 256, size=(27, 45, 4)).astype(np.uint8); wall[..., 3] = 255
+    panel = np.zeros((32, 32, 4), np.uint8); panel[..., 3] = 255
+    panel[..., 0] = (np.mgrid[0:32, 0:32][1] * 8).astype(np.uint8); panel[..., 1] = 120; panel[..., 2] = (255 - np.mgrid[0:32, 0:32][0] * 8).astype(np.uint8)
+    mr = rng.randint(0, 256, size=(8, 8, 4)).astype(np.uint8); mr[..., 3] = 255
+    fence = np.zeros((32, 32, 4), np.uint8); fence[...] = (255, 255, 255, 255)
+    fence[(np.mgrid[0:32, 0:32][1] % 8) >= 4] = (0, 0, 0, 0)
+    images = {720: ground, 721: wall, 722: panel, 723: mr, 724: fence}
+    materials = {
+        110: (material((1.0, 1.0, 1.0, 1.0)), False), 111: (material((0.9, 0.9, 0.9, 1.0)), False),
+        112: (material((0.2, 0.2, 0.2, 1.0), emissive=(2.0, 2.0, 2.0, 1.0)), False),
+        113: (material((0.9, 0.8, 0.6, 1.0), perceptual_roughness=0.8, metallic=1.0), False),
+        114: (material((0.8, 0.8, 0.8, 1.0)), True),
+    }
+    material_textures = {110: dict(base_color=720), 111: dict(base_color=721), 112: dict(emissive=722), 113: dict(metallic_roughness=723),
+                         114: dict(base_color=724)}
+    meshes = {
+        210: np.stack(_quad((-60, 0, -60), (60, 0, -60), (60, 0, 60), (-60, 0, 60), (0, 1, 0), (0.0, 0.0), (60.0, 60.0))),   # ground
+        211: np.stack(_quad((0.6, 0.2, 2.2), (0.6, 1.4, 2.2), (1.4, 1.4, 3.0), (1.4, 0.2, 3.0), (-1, 0, 1))),                   # wall near the camera
+        212: np.stack(_quad((-3, 0.5, -4), (-3, 2.5, -4), (-1, 2.5, -4), (-1, 0.5, -4), (0, 0, 1), (0, 0), (2, 2))),             # emissive panel
+        213: np.stack(_box((0.8, 0.0, -1.6), (1.8, 1.0, -0.6))),                                                                 # metal box
+        214: np.stack(_quad((-2.5, 0, -1), (-0.5, 0, -1), (-0.5, 1.2, -1), (-2.5, 1.2, -1), (0, 0, 1), (0, 0), (4, 2))),         # fence
+    }
+    instances = [(310, 210, 110, IDENTITY_AFFINE), (311, 211, 111, IDENTITY_AFFINE), (312, 212, 112, IDENTITY_AFFINE),
+                 (313, 213, 113, IDENTITY_AFFINE), (314, 214, 114, IDENTITY_AFFINE)]
+    lights = [(410, LIGHT_POINT, point_light((0.0, 3.0, 1.0), 0.1, (8.0, 8.0, 8.0), 30.0))]
+    cam = dict(mode=mode, denoise=denoise, ref_depth=ref_depth, w=width, h=height, transform=look_at_transform((0.0, 0.9, 4.0), (0.0, 0.6, -10.0)),
+               projection=perspective_infinite_reverse_rh(math.pi / 4.0, width / height, 0.1))
+    return dict(name="tiled_ground", meshes=meshes, materials=materials, instances=instances, lights=lights, sun=(1.0, 0.35), camera=cam,
+                images=images, material_textures=material_textures)
+
+
 def brick_normal_map(n=64, rows=4, cols=2, mortar=0.06, bevel=0.05, seed=11):
     """A brick-wall tangent-space normal map (RGBA8, n x n, linear bytes 255 (t + 1) / 2): bevelled bricks in running bond,
     flat mortar joints, a little per-brick tilt and grain, and one 6 x 6 patch whose texels point below the surface

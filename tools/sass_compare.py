@@ -1,6 +1,6 @@
 """Compare per-kernel SASS of two libstrolle_b200.so builds: every kernel of the old build against the same kernel (for a kernel that
-gained `bool NMAP` / `bool LGRID` template parameters: its all-<false> instantiation, whose trailing LightGridDev argument is unused)
-of the new one.  Compared: the full instruction text (opcodes,
+gained `bool NMAP` / `bool LGRID` / `bool TEXF` template parameters: its all-<false> instantiation, whose trailing LightGridDev and
+TexFilterDev arguments are unused) of the new one.  Compared: the full instruction text (opcodes,
 registers, immediates, constant-bank operands); normalised: the code-offset comments, branch targets and relocated symbol names."""
 import re, subprocess, sys
 
@@ -29,10 +29,15 @@ def kernels(lib):
         m = re.search(r"::(\w+)<", d)
         return m.group(1) if m and (m.group(1) in NM or m.group(1) in LG) else None
     def targs(d): return d.split("(")[0].split("<", 1)[1].rstrip(">").split(", ")
-    def norm(d):   # the name the kernel had before it gained LGRID (and NMAP): all-false instantiations lose their template arguments
+    def norm(d):   # the name the kernel had before it gained TEXF, LGRID (and NMAP): all-false instantiations lose their template arguments
         k = base(d)
         if k is None: return d
         args = targs(d)
+        if "TexFilterDev)" in d:   # bool TEXF, the last template argument
+            if args[-1] == "true": return d
+            del args[-1]
+            head = d.split("(")[0]
+            d = head.split("<")[0] + "<" + ", ".join(args) + ">" + re.sub(r", \w+::TexFilterDev\)", ")", d[len(head):])
         if k in LG and len(args) > LG[k]:
             if args[LG[k]] == "true": return d
             del args[LG[k]]
@@ -54,5 +59,5 @@ for k, body in sorted(old.items()):
         if "-v" in sys.argv:
             import difflib
             print("\n".join(list(difflib.unified_diff(body, new[k], lineterm="", n=1))[:60]))
-print(f"{same} kernels identical, {diff} differ; {len(old)} kernels in the old build, {len(new)} (+{len(nmap)} NMAP / LGRID instantiations) in the new")
-for k in sorted(nmap): print("  NMAP / LGRID:", k)
+print(f"{same} kernels identical, {diff} differ; {len(old)} kernels in the old build, {len(new)} (+{len(nmap)} NMAP / LGRID / TEXF instantiations) in the new")
+for k in sorted(nmap): print("  NMAP / LGRID / TEXF:", k)
