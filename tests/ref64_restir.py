@@ -496,14 +496,14 @@ def _decide(r, W, weight):
         return margin > 0, (~(np.abs(margin) <= bound) | ((margin == 0) & (W.e == 0) & (weight.e == 0))) & np.isfinite(margin)
 
 
-def _mis_eval(lm, rm, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, rpdf):
-    """Mis::eval (mis.rs:96-145) with rhs_jacobian = 1: (m, lhs_mis, rhs_mis)."""
+def _mis_eval(lm, rm, lpdf, lhs_rhs_pdf, rhs_lhs_pdf, rpdf, rhs_jacobian=1.0):
+    """Mis::eval (mis.rs:96-145): (m, lhs_mis, rhs_mis).  DI passes rhs_jacobian = 1; the GI spatial merge the texel's jacobian."""
     mm_a, mm_b = _mis_m(rpdf, rhs_lhs_pdf), _mis_m(lhs_rhs_pdf, lpdf)
     mmin = where(mm_a.v <= mm_b.v, mm_a, mm_b)
     mmin = Num(mmin.v, np.maximum(mm_a.e, mm_b.e), lm.fast)
     t = _ratio(lm, rm)
     lhs_mis = t + (1.0 - t) * _ratio(lm * lpdf, rm * lhs_rhs_pdf)
-    rhs_mis = (1.0 - t) * _ratio((rm * rpdf) * 1.0, lm * rhs_lhs_pdf)
+    rhs_mis = (1.0 - t) * _ratio((rm * rpdf) * rhs_jacobian, lm * rhs_lhs_pdf)
     return rm * mmin, lhs_mis, rhs_mis
 
 
