@@ -182,7 +182,7 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18 };
 /* ST_OPT_TEXTURE_FILTER (default 0; 1 = on, anything else is ST_ERR_INVALID): material textures are filtered through per-image mip
  * chains with a ray-cone level of detail, instead of the nearest texel of level 0 (the reference's sampler, so 0 keeps parity).
  * Level 0 is the image's atlas rect; levels 1.. (each texel the 2x2 box of the level above, averaged in linear light through the
@@ -194,6 +194,20 @@ enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3,
  * trilinear: bilinear on levels floor(lambda) and floor(lambda) + 1 with repeat-wrapped taps inside the image.  It applies to base
  * colour, emissive and metallic-roughness at the G-buffer, to base colour and emissive at the GI bounce and in Reference mode; the
  * alpha test and normal maps keep the nearest level-0 texel.  Takes effect at the next st_tick (DESIGN.md §2). */
+/* ST_OPT_TEMPORAL_AA (default 0; 1 = on, anything else is ST_ERR_INVALID): sub-pixel camera jitter and a temporal resolve.  Frame f
+ * renders through J(f) = (h2(k) - 0.5, h3(k) - 0.5) pixels, k = ((f - 1) mod 16) + 1, h2 / h3 the base-2 / base-3 radical inverses
+ * (in double, rounded to f32; screen y points down): pixel p's ray passes through the unjittered screen point p + 0.5 + J(f).  The
+ * jitter is applied to the projection on the host (dx = -2 Jx / W, dy = 2 Jy / H; m[4c] += dx m[4c + 3], m[4c + 1] += dy m[4c + 3]
+ * for every column c) before projection_view and ndc_to_world are derived, so every pass sees one consistent jittered camera; last
+ * frame's camera is jittered with J(f - 1), J(0) = J(16).  Consequences: on a still camera the velocity map holds
+ * -(J(f) - J(f - 1)), and st_read_buffer("curr_camera" / "prev_camera") returns the jittered cameras.  The composition step
+ * (timed as P_COMPOSITION) then resolves instead of composing: per pixel the composed colour is tonemapped (c / (1 + max c)), the
+ * history (Catmull-Rom at the surface's unjittered position last frame) is clipped into the 3x3 neighbourhood's YCoCg box and blended
+ * with alpha = max(1 / (n + 1), 0.1), n the history's frame count (<= 16); `output` holds the resolved colour.  History lives in
+ * "taa_history_a" / "taa_history_b" (st_read_buffer: tonemapped rgb, count), allocated while the option is on and reset by turning it
+ * on and by camera reallocation.  Reference mode and CameraMode::BvhHeatmap are neither jittered nor resolved.  With the option on,
+ * st_render_strips and st_multi_render_camera over more than one member return ST_ERR_INVALID.  ST_STAT_TAA_RESOLVES counts the
+ * resolve launches.  Takes effect at the next st_tick (DESIGN.md §2). */
 /* ST_OPT_LIGHT_GRID (default 0 = off; 1..64, anything else is ST_ERR_INVALID): the light candidates of ReSTIR DI sampling, of the GI
  * bounce's next-event estimate and of Reference mode are drawn uniformly from a per-cell list of the light slots that can reach the
  * point's cell, instead of from every slot.  N is the cell count along the longest axis of the grid box, the AABB of the range spheres of
@@ -284,7 +298,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_NORMAL_MAP_LAUNCHES = 8 /* launches of the normal-mapped kernel variants (ST_OPT_NORMAL_MAPS) since creation */,
        ST_STAT_BVH_REFITS = 9 /* refit ticks (ST_OPT_BVH_REFIT) since creation */,
        ST_STAT_LIGHT_GRID_BUILDS = 10 /* light grid builds (ST_OPT_LIGHT_GRID) since creation */,
-       ST_STAT_TEXTURE_MIP_BUILDS = 11 /* mip-chain builds (ST_OPT_TEXTURE_FILTER) since creation */ };
+       ST_STAT_TEXTURE_MIP_BUILDS = 11 /* mip-chain builds (ST_OPT_TEXTURE_FILTER) since creation */,
+       ST_STAT_TAA_RESOLVES = 12 /* temporal resolve launches (ST_OPT_TEMPORAL_AA) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,

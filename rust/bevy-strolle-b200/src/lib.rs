@@ -48,12 +48,15 @@ pub struct StrolleSun {
 /// `light_grid`: sample light candidates from a grid of the point lights that can reach each cell, this many cells along its
 /// longest axis (1..=64; 0, the default, samples every light, as the reference does) - for scenes with many short-range lights.
 /// `texture_filter`: filter material textures through mip chains (false, the default, takes the nearest texel, as the reference does).
+/// `temporal_aa`: anti-alias with sub-pixel camera jitter and a temporal resolve (false, the default, renders one ray through each
+/// pixel centre, as the reference does); needs one GPU.
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
     pub bvh_refit_ticks: u32,
     pub light_grid: u32,
     pub texture_filter: bool,
+    pub temporal_aa: bool,
 }
 
 #[derive(Clone, Debug)]
@@ -98,6 +101,7 @@ impl Plugin for StrollePlugin {
         engine.set_bvh_refit(settings.bvh_refit_ticks).expect("strolle_b200: ST_OPT_BVH_REFIT");
         engine.set_light_grid(settings.light_grid).expect("strolle_b200: ST_OPT_LIGHT_GRID");
         engine.set_texture_filter(settings.texture_filter).expect("strolle_b200: ST_OPT_TEXTURE_FILTER");
+        engine.set_temporal_aa(settings.temporal_aa).expect("strolle_b200: ST_OPT_TEMPORAL_AA");
         render_app.insert_resource(EngineResource(engine));
     }
 }

@@ -446,6 +446,13 @@ impl<P: Params> Engine<P> {
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_TEXTURE_FILTER, on as c_int) })
     }
 
+    /// Anti-aliases frames with sub-pixel camera jitter and a temporal resolve in place of the frame composition
+    /// (`ST_OPT_TEMPORAL_AA`; off, the default, renders one ray through each pixel centre, as the reference does).  Needs an engine
+    /// over one device: row strips over several refuse to render while it is on.  Takes effect with the next frame's scene update.
+    pub fn set_temporal_aa(&mut self, on: bool) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_TEMPORAL_AA, on as c_int) })
+    }
+
     /// Creates or updates a mesh (`lib.rs:161-164`).
     pub fn insert_mesh(&mut self, handle: P::MeshHandle, item: Mesh) {
         let id = self.meshes.id(handle);

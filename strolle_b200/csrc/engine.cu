@@ -388,6 +388,7 @@ static uint32_t dispatch_seed(uint32_t base, uint32_t frame, uint32_t k) {
 struct CameraSlot {
     bool alive = false;
     st_camera desc;
+    st_camera prev_desc;   // the camera `dev.prev` was serialised from (ST_OPT_TEMPORAL_AA jitters both)
     uint32_t frame = 0;
     CameraDev dev;
     std::vector<std::pair<std::string, float4**>> named;   // buffer name -> pointer slot in `dev`
@@ -395,6 +396,7 @@ struct CameraSlot {
     DevMem arena;
     DevMem svgf_pairs; float4* pair[2] = {nullptr, nullptr};   // interleaved {DI, GI} records of the wide-stride à-trous iterations (ST_OPT_WAVELET_PAIRED); private scratch, never exchanged
     DevMem rgba8; int rgba8_slot = 0;
+    DevMem taa; float4* taa_hist[2] = {nullptr, nullptr};   // ST_OPT_TEMPORAL_AA history {tonemapped rgb, count}, a / b by frame parity; zero-filled
     // asynchronous RGBA8 read-back: slot k of the staging buffer is converted on the engine stream (ev_ready[k]) and copied to
     // the host on the copy stream (ev_copied[k]); the engine stream only waits for ev_copied[k] before reusing slot k
     cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
@@ -488,6 +490,8 @@ struct st_engine {
     bool texture_filter = false, texf_built = false, any_color_texture = false, texf_frame = false; TexFilterDev texf{};
     DevMem d_texf_pool, d_texf_table, d_texf_jobs; std::vector<uint2> h_texf_table; std::vector<MipJob> h_texf_jobs; size_t texf_pool_texels = 0;
     uint64_t texture_mip_builds = 0;
+    // ST_OPT_TEMPORAL_AA: `temporal_aa` = the option, `taa_frame` = the option as st_tick took it for the frame's cameras and resolve
+    bool temporal_aa = false, taa_frame = false; uint64_t taa_resolves = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -883,6 +887,38 @@ static GpuCamera serialize_camera(const st_camera& c) {   // Camera::serialize (
     return g;
 }
 
+// ---- ST_OPT_TEMPORAL_AA (DESIGN.md §2 "Temporal anti-aliasing") ------------------------------------------------------------------
+// J(f) = (h2(k) - 0.5, h3(k) - 0.5) pixels, k = ((f - 1) mod 16) + 1 (u32 arithmetic: J(0) = J(16)); radical inverses in double
+static double radical_inverse(uint32_t k, uint32_t base) {
+    const double inv = 1.0 / (double)base;
+    double r = 0.0, f = inv;
+    for (; k > 0u; k /= base) { r += f * (double)(k % base); f *= inv; }
+    return r;
+}
+static float2 taa_jitter(uint32_t frame) {
+    const uint32_t k = ((frame - 1u) % 16u) + 1u;
+    return make_float2((float)radical_inverse(k, 2u) - 0.5f, (float)radical_inverse(k, 3u) - 0.5f);
+}
+// the camera rendered through the jitter: the projection's x and y rows gain dx / dy times its w row, so that every screen point moves by
+// -j (pixel p's ray passes through the unjittered point p + 0.5 + j)
+static GpuCamera serialize_jittered(const st_camera& c, float2 j) {
+    st_camera t = c;
+    const float dx = (-2.0f * j.x) / (float)c.width, dy = (2.0f * j.y) / (float)c.height;
+    for (int col = 0; col < 4; col++) {
+        t.projection[4 * col] = t.projection[4 * col] + dx * t.projection[4 * col + 3];
+        t.projection[4 * col + 1] = t.projection[4 * col + 1] + dy * t.projection[4 * col + 3];
+    }
+    return serialize_camera(t);
+}
+// Whether this frame of the camera is jittered and resolved; if so, its jittered cameras and (J(f), J(f - 1))
+static bool taa_cameras(const st_engine* e, const CameraSlot* cs, GpuCamera* curr, GpuCamera* prev, float4* jit) {
+    if (!e->taa_frame || cs->desc.mode == ST_MODE_REFERENCE || cs->desc.mode == ST_MODE_BVH_HEATMAP) return false;
+    const float2 j = taa_jitter(cs->frame), pj = taa_jitter(cs->frame - 1u);
+    *curr = serialize_jittered(cs->desc, j); *prev = serialize_jittered(cs->prev_desc, pj);
+    *jit = make_float4(j.x, j.y, pj.x, pj.y);
+    return true;
+}
+
 // CameraBuffers::new (strolle/src/camera_controller/buffers.rs:53-339): one zero-filled arena
 static int allocate_camera(st_engine* e, CameraSlot* cs) {
     CameraDev& d = cs->dev;
@@ -919,6 +955,7 @@ static int allocate_camera(st_engine* e, CameraSlot* cs) {
     for (size_t i = 0; i < cs->named.size(); i++) { *cs->named[i].second = (float4*)((char*)cs->arena.p + off); off += (cs->sizes[i].second * 16 + 255) / 256 * 256; }
     d.w = (int)cs->desc.width; d.h = (int)cs->desc.height; d.y0 = 0; d.y1 = d.h;
     d.own_y0 = 0; d.own_y1 = d.h; d.mirror_up = 0; d.mirror_dn = 0; d.need_rows = nullptr; d.gi_mirror_reach = 128; d.di_mirror_reach = 128;
+    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr;   // ST_OPT_TEMPORAL_AA: history restarts (allocated zeroed at the next resolve)
     return ST_OK;
 }
 
@@ -929,7 +966,9 @@ static int allocate_camera(st_engine* e, CameraSlot* cs) {
 struct StripExt { int gbuffer = 0, variance = 0, wavelet[5] = {0, 0, 0, 0, 0}; int preview_mirror[2] = {0, 0}; bool still = false; /* nothing moved: no rows of last frame are pulled */ };
 static CameraDev grown(const CameraDev& c, int rows) { CameraDev g = c; g.y0 = std::max(0, c.y0 - rows); g.y1 = std::min(c.h, c.y1 + rows); return g; }
 static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* steps, const StripExt* ext = nullptr) {
-    const CameraDev cam = cs->dev;   // snapshot (pointers + cameras)
+    GpuCamera jc, jp; float4 jit;
+    const bool taa = taa_cameras(e, cs, &jc, &jp, &jit);   // ST_OPT_TEMPORAL_AA: every pass sees the jittered cameras
+    const CameraDev cam = [&] { CameraDev c = cs->dev; if (taa) { c.curr = jc; c.prev = jp; } return c; }();   // snapshot (pointers + cameras)
     const StripExt no_ext; const StripExt& x = ext ? *ext : no_ext;
     const CameraDev camG = grown(cam, x.gbuffer), camV = grown(cam, x.variance);
     const int pm0 = x.preview_mirror[0], pm1 = x.preview_mirror[1];
@@ -1059,6 +1098,11 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         }
     }
     uint32_t mode = (uint32_t)d.mode;
+    if (taa) {   // the resolve composes the frame itself; history a / b alternate with the frame parity like the G-buffer
+        const float4* hin = cs->taa_hist[cur ^ 1]; float4* hout = cs->taa_hist[cur];
+        add(P_COMPOSITION, [=](cudaStream_t s) { e->taa_resolves++; launch_taa_resolve(cam, sc, cur, mode, di_final, gi_final, hin, hout, jit, s); });
+        return;
+    }
     add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, mode, di_final, gi_final, s); });
 }
 
@@ -1603,7 +1647,7 @@ int st_create_camera(st_engine* e, const st_camera* c, st_camera_handle* out) { 
     CameraSlot* cs = new CameraSlot();
     cs->alive = true; cs->desc = *c;
     int rc = allocate_camera(e, cs); if (rc) { delete cs; return rc; }
-    cs->dev.curr = serialize_camera(*c); cs->dev.prev = cs->dev.curr;
+    cs->dev.curr = serialize_camera(*c); cs->dev.prev = cs->dev.curr; cs->prev_desc = *c;
     e->cameras.push_back(cs);
     *out = (st_camera_handle)e->cameras.size() - 1;
     return ST_OK;
@@ -1613,7 +1657,7 @@ int st_update_camera(st_engine* e, st_camera_handle h, const st_camera* c) {   /
     if (!cs || !c) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     CK(cudaSetDevice(e->device));
     bool invalidated = cs->desc.mode != c->mode || cs->desc.denoise != c->denoise || cs->desc.ref_depth != c->ref_depth || cs->desc.width != c->width || cs->desc.height != c->height;
-    cs->desc = *c;
+    cs->prev_desc = cs->desc; cs->desc = *c;
     cs->dev.prev = cs->dev.curr;
     cs->dev.curr = serialize_camera(*c);
     if (invalidated) { GpuCamera a = cs->dev.curr, b = cs->dev.prev; CK(cudaStreamSynchronize(e->stream)); int rc = allocate_camera(e, cs); if (rc) return rc; cs->dev.curr = a; cs->dev.prev = b; }
@@ -1627,6 +1671,7 @@ int st_delete_camera(st_engine* e, st_camera_handle h) {
     if (e->copy_stream) CK(cudaStreamSynchronize(e->copy_stream));
     for (int k = 0; k < 2; k++) if (cs->side[k]) CK(cudaStreamSynchronize(cs->side[k]));
     cs->alive = false; cs->arena.release(); cs->svgf_pairs.release(); cs->pair[0] = cs->pair[1] = nullptr; cs->rgba8.release();
+    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr;
     return ST_OK;
 }
 int st_camera_set_strip(st_engine* e, st_camera_handle h, int y0, int y1) {
@@ -1758,6 +1803,9 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
         e->texf_built = false;
     } else if (textures_changed || !e->texf_built) { if ((rc = build_texture_mips(e))) return rc; }
     e->texf_frame = e->texture_filter && e->any_color_texture;
+    // ST_OPT_TEMPORAL_AA: the history exists only while the option is on, and starts over when it turns on
+    if (e->temporal_aa != e->taa_frame) for (CameraSlot* c : e->cameras) { c->taa.release(); c->taa_hist[0] = c->taa_hist[1] = nullptr; }
+    e->taa_frame = e->temporal_aa;
     e->frame += 1;
     if (too_deep) return fail(ST_ERR_LIMIT, "BVH deeper than the 24-entry traversal stack (strolle-gpu/src/lib.rs:72-76): the scene is not drawn until it changes");
     return ST_OK;
@@ -1771,12 +1819,22 @@ int st_frame_schedule(st_engine* e, st_camera_handle h, int* pass_ids, int cap, 
     for (int i = 0; i < cap && i < *count; i++) pass_ids[i] = steps[i].pass;
     return ST_OK;
 }
+// ST_OPT_TEMPORAL_AA: both history buffers of a camera that resolves, in one zero-filled allocation of their own
+static int ensure_taa_history(st_engine* e, CameraSlot* cs) {
+    GpuCamera a, b; float4 j;
+    if (cs->taa.p || !taa_cameras(e, cs, &a, &b, &j)) return ST_OK;
+    const size_t bytes = ((size_t)cs->desc.width * cs->desc.height * 16 + 255) / 256 * 256;
+    int rc = cs->taa.ensure(2 * bytes); if (rc) return rc;
+    cs->taa_hist[0] = (float4*)cs->taa.p; cs->taa_hist[1] = (float4*)((char*)cs->taa.p + bytes);
+    return ST_OK;
+}
 int st_render_range(st_engine* e, st_camera_handle h, int first, int last) {
     CameraSlot* cs = e ? get_camera(e, h) : nullptr;
     if (!cs) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     if (cs->frame == 0) return fail(ST_ERR_INVALID, "st_tick must precede st_render_camera");
     CK(cudaSetDevice(e->device));
     int rc = ensure_luts(e); if (rc) return rc;
+    if ((rc = ensure_taa_history(e, cs))) return rc;
     std::vector<Step> steps; build_schedule(e, cs, &steps);
     if (last < 0 || last >= (int)steps.size()) last = (int)steps.size() - 1;
     for (int i = std::max(first, 0); i <= last; i++) e->run_timed(steps[i].pass, steps[i].run, steps[i].sub);
@@ -1834,8 +1892,17 @@ int st_read_buffer(st_engine* e, st_camera_handle h, const char* name, float* ds
     if (!cs || !name || !count) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     CK(cudaSetDevice(e->device));
     if (!std::strcmp(name, "curr_camera") || !std::strcmp(name, "prev_camera")) {
-        const GpuCamera& c = !std::strcmp(name, "curr_camera") ? cs->dev.curr : cs->dev.prev;
+        GpuCamera jc, jp; float4 jit;
+        const bool taa = taa_cameras(e, cs, &jc, &jp, &jit);   // ST_OPT_TEMPORAL_AA: the cameras the frame renders through
+        const GpuCamera& c = !std::strcmp(name, "curr_camera") ? (taa ? jc : cs->dev.curr) : (taa ? jp : cs->dev.prev);
         *count = 40; if (dst) std::memcpy(dst, &c, 4 * std::min<size_t>(cap, 40)); return ST_OK;
+    }
+    if (!std::strcmp(name, "taa_history_a") || !std::strcmp(name, "taa_history_b")) {
+        const float4* p = cs->taa_hist[name[12] == 'a' ? 0 : 1];
+        if (!p) return fail(ST_ERR_NOT_FOUND, "no temporal history: ST_OPT_TEMPORAL_AA is off or the camera has not resolved a frame since");
+        *count = (size_t)cs->desc.width * cs->desc.height * 4;
+        if (dst) { CK(cudaStreamSynchronize(e->stream)); CK(cudaMemcpy(dst, p, 4 * std::min(cap, *count), cudaMemcpyDeviceToHost)); }
+        return ST_OK;
     }
     for (size_t i = 0; i < cs->named.size(); i++) if (cs->named[i].first == name) {
         *count = cs->sizes[i].second * 4;
@@ -1848,6 +1915,9 @@ int st_buffer_device_ptr(st_engine* e, st_camera_handle h, const char* name, voi
     CameraSlot* cs = e ? get_camera(e, h) : nullptr;
     if (!cs || !name || !ptr || !bytes) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     for (size_t i = 0; i < cs->named.size(); i++) if (cs->named[i].first == name) { *ptr = *cs->named[i].second; *bytes = cs->sizes[i].second * 16; return ST_OK; }
+    if ((!std::strcmp(name, "taa_history_a") || !std::strcmp(name, "taa_history_b")) && cs->taa_hist[0]) {
+        *ptr = cs->taa_hist[name[12] == 'a' ? 0 : 1]; *bytes = (size_t)cs->desc.width * cs->desc.height * 16; return ST_OK;
+    }
     return fail(ST_ERR_NOT_FOUND, std::string("unknown buffer ") + name);
 }
 int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap, size_t* count) {
@@ -1965,6 +2035,10 @@ int st_set_option(st_engine* e, int option, int value) {
         if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_TEXTURE_FILTER: 0 (nearest level-0 texel) or 1 (filtered)");
         e->texture_filter = value == 1; return ST_OK;
     }
+    if (option == ST_OPT_TEMPORAL_AA) {   // takes effect at the next st_tick
+        if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_TEMPORAL_AA: 0 (off) or 1 (jitter + temporal resolve)");
+        e->temporal_aa = value == 1; return ST_OK;
+    }
     if (option == ST_OPT_BVH_REFIT) { if (value < 0) return fail(ST_ERR_INVALID, "ST_OPT_BVH_REFIT: 0 or a positive budget"); e->bvh_refit = value; return ST_OK; }
     return fail(ST_ERR_INVALID, "unknown option");
 }
@@ -2010,6 +2084,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_BVH_REFITS) { *value = e->bvh_refits; return ST_OK; }
     if (stat == ST_STAT_LIGHT_GRID_BUILDS) { *value = e->light_grid_builds; return ST_OK; }
     if (stat == ST_STAT_TEXTURE_MIP_BUILDS) { *value = e->texture_mip_builds; return ST_OK; }
+    if (stat == ST_STAT_TAA_RESOLVES) { *value = e->taa_resolves; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
         CK(cudaSetDevice(e->device)); CK(cudaStreamSynchronize(e->stream));
         uint64_t total = 0;
@@ -2233,9 +2308,12 @@ int st_plan_strip_order(const int* schedule, int n, int dma, char* out, size_t c
     std::memcpy(out, text.c_str(), text.size() + 1);
     return ST_OK;
 }
+// The resolve would need the neighbours' rows of last frame's history and a composed halo row: not supported (yet) for strips
+static const char* const kTaaStripsError = "ST_OPT_TEMPORAL_AA: row strips are not supported; render the camera on one engine (st_render_camera)";
 int st_render_strips(st_engine* e, st_camera_handle h, void* host_out, int format, int temporal_reach, int gather) {
     CameraSlot* cs = e ? get_camera(e, h) : nullptr;
     if (!cs) return fail(ST_ERR_NOT_FOUND, "unknown camera");
+    if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
     CK(cudaSetDevice(e->device));
     int rc = enqueue_strip_frame(e, cs, temporal_reach); if (rc) return rc;
     if (!gather) return ST_OK;
@@ -2429,6 +2507,7 @@ int st_multi_render_camera(st_multi* m, st_camera_handle h, void* host_out, int 
     if (!m || h < 0 || (size_t)h >= m->cams.size()) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     const size_t n = m->e.size();
     if (n == 1) return st_render_camera(m->e[0], m->cams[h][0], host_out, format);
+    for (st_engine* e : m->e) if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
     std::vector<CameraSlot*> cs(n);
     for (size_t i = 0; i < n; i++) {   // first-use allocations and LUT generation synchronise their device: do them before anything can wait on a peer
         cs[i] = get_camera(m->e[i], m->cams[h][i]);

@@ -1238,11 +1238,9 @@ __global__ void __launch_bounds__(TW * TH, (TW * TH <= 256 && S <= 8) ? ST_WAVEL
     ctr.store(di_out, gi_out, pair_out, i);
 }
 
-// R2 frame_composition::fs (frame_composition.rs:19-82), linear HDR out
-__global__ void __launch_bounds__(ST_BLOCK) k_composition(KPARAMS, int cur, u32 mode, const float4* __restrict__ di_diff, const float4* __restrict__ gi_diff) {
-    Px p = pixel_full(cam);
-    if (!p.in) return;
-    size_t i = pix(cam, p.x, p.y);
+// R2 frame_composition::fs (frame_composition.rs:19-82) for pixel i: the linear HDR colour that k_composition stores and that
+// k_taa_resolve composes into shared memory
+ST_DEV float3 compose_px(const CameraDev& cam, const SceneDev& sc, int cur, u32 mode, const float4* __restrict__ di_diff, const float4* __restrict__ gi_diff, size_t i) {
     float3 color;
     if (mode == 0u) {
         GBuf g = gbuf_unpack(sc, cam.prim_gbuffer_d0[cur][i], cam.prim_gbuffer_d1[cur][i]);
@@ -1256,7 +1254,105 @@ __global__ void __launch_bounds__(ST_BLOCK) k_composition(KPARAMS, int cur, u32 
     else if (mode == 5u) color = xyz(cam.ref_colors[i]);
     else if (mode == 6u) { float4 c = cam.ref_colors[i]; color = xyz(c) / c.w; }
     else color = f3s(0.f);
-    cam.output[i] = f4(color, 1.0f);
+    return color;
+}
+// R2 frame_composition::fs (frame_composition.rs:19-82), linear HDR out
+__global__ void __launch_bounds__(ST_BLOCK) k_composition(KPARAMS, int cur, u32 mode, const float4* __restrict__ di_diff, const float4* __restrict__ gi_diff) {
+    Px p = pixel_full(cam);
+    if (!p.in) return;
+    size_t i = pix(cam, p.x, p.y);
+    cam.output[i] = f4(compose_px(cam, sc, cur, mode, di_diff, gi_diff, i), 1.0f);
+}
+
+// ---- ST_OPT_TEMPORAL_AA (DESIGN.md §2 "Temporal anti-aliasing"): the resolve, in place of k_composition --------------------------
+// Every step below is one IEEE operation in the order written (strict build only); oracle_taa/taa.cpp restates it operation for
+// operation.  Colours are tonemapped, t(c) = c / (1 + max(c)), before they are boxed, filtered and blended.
+#define TAA_TW 32
+#define TAA_TH 8
+static const float kTaaClipEps = 1e-8f;   // added to the box's half extent (Playdead's clip_aabb)
+ST_DEV float taa_max(float a, float b) { return a > b ? a : b; }
+ST_DEV float taa_min(float a, float b) { return a < b ? a : b; }
+ST_DEV float3 taa_tonemap(float3 c) { const float d = 1.0f + taa_max(taa_max(c.x, c.y), c.z); return f3(c.x / d, c.y / d, c.z / d); }
+ST_DEV float3 taa_untonemap(float3 t) { const float d = 1.0f - taa_max(taa_max(t.x, t.y), t.z); return f3(t.x / d, t.y / d, t.z / d); }
+ST_DEV float3 taa_ycocg(float3 c) { return f3((0.25f * c.x + 0.5f * c.y) + 0.25f * c.z, 0.5f * c.x - 0.5f * c.z, (-0.25f * c.x + 0.5f * c.y) - 0.25f * c.z); }
+ST_DEV float3 taa_rgb(float3 v) { const float t = v.x - v.z; return f3(t + v.y, v.x + v.z, t - v.y); }
+// Catmull-Rom weights of the four taps around a sample at fraction f past the second one
+ST_DEV void taa_cr_weights(float f, float w[4]) {
+    w[0] = f * (-0.5f + f * (1.0f - 0.5f * f));
+    w[1] = 1.0f + (f * f) * (-2.5f + 1.5f * f);
+    w[2] = f * (0.5f + f * (2.0f - 1.5f * f));
+    w[3] = (f * f) * (-0.5f + 0.5f * f);
+}
+// `jit` = (J(f), J(f - 1)) in pixels; cam.curr / cam.prev are the jittered cameras of this frame and the last
+__global__ void __launch_bounds__(TAA_TW * TAA_TH) k_taa_resolve(KPARAMS, int cur, u32 mode, const float4* __restrict__ di_diff, const float4* __restrict__ gi_diff,
+                                                                 const float4* __restrict__ hist_in, float4* __restrict__ hist_out, float4 jit) {
+    const int HW = TAA_TW + 2, HH = TAA_TH + 2;
+    __shared__ float4 s_t[HW * HH];   // tonemapped composed colours of the tile and a 1-pixel halo, taps clamped to the screen
+    const int bx = (int)blockIdx.x * TAA_TW - 1, by = (int)blockIdx.y * TAA_TH - 1;
+    for (int k = threadIdx.x; k < HW * HH; k += TAA_TW * TAA_TH) {
+        const int x = min(max(bx + k % HW, 0), cam.w - 1), y = min(max(by + k / HW, 0), cam.h - 1);
+        s_t[k] = f4(taa_tonemap(compose_px(cam, sc, cur, mode, di_diff, gi_diff, pix(cam, (u32)x, (u32)y))), 0.0f);
+    }
+    __syncthreads();
+    const int tx = threadIdx.x % TAA_TW, ty = threadIdx.x / TAA_TW;
+    const u32 px = blockIdx.x * TAA_TW + tx, py = blockIdx.y * TAA_TH + ty;
+    if (px >= (u32)cam.w || py >= (u32)cam.h) return;
+    const size_t i = pix(cam, px, py);
+    // 1-2. the current value and the 3x3 box in YCoCg (row by row)
+    const float3 t = xyz(s_t[(ty + 1) * HW + tx + 1]);
+    float3 lo = taa_ycocg(xyz(s_t[ty * HW + tx])), hi = lo;
+#pragma unroll
+    for (int k = 1; k < 9; k++) {
+        const float3 v = taa_ycocg(xyz(s_t[(ty + k / 3) * HW + tx + k % 3]));
+        lo = f3(taa_min(lo.x, v.x), taa_min(lo.y, v.y), taa_min(lo.z, v.z)); hi = f3(taa_max(hi.x, v.x), taa_max(hi.y, v.y), taa_max(hi.z, v.z));
+    }
+    // 3. where the surface seen through the unjittered pixel centre was in last frame's unjittered screen
+    const float W = cam.curr.screen.x, H = cam.curr.screen.y;
+    float2 q; bool ok = true;
+    if (cam.prim_gbuffer_d0[cur][i].x != 0.0f) {
+        const float4 v = cam.velocity_map[i];
+        q = f2((((float)px + 0.5f) - v.x) - (jit.x - jit.z), (((float)py + 0.5f) - v.y) - (jit.y - jit.w));
+    } else {   // sky: the direction through the unjittered centre (jittered screen point p + 0.5 - J(f)), at w = 0 through last frame's camera
+        const float sx = ((float)px + 0.5f) - jit.x, sy = ((float)py + 0.5f) - jit.y;
+        const float nx = sx * 2.0f / W - 1.0f, ny = -(sy * 2.0f / H - 1.0f);
+        const float3 far_plane = project_point(cam_n2w(cam.curr), f3(nx, ny, kF32Eps)), near_plane = project_point(cam_n2w(cam.curr), f3(nx, ny, 1.0f));
+        const float4 clip = mat_mul(cam_pv(cam.prev), f4(norm(far_plane - near_plane), 0.0f));
+        const float2 s = cam_clip_to_screen(cam.prev, clip);
+        q = f2(s.x + jit.z, s.y + jit.w);
+        ok = clip.w > 0.0f;
+    }
+    // 4. validity: on screen, and a non-zero count at the nearest history texel
+    ok = ok && q.x >= 0.0f && q.y >= 0.0f && q.x < W && q.y < H;
+    float n = 0.0f;
+    if (ok) n = hist_in[pix(cam, (u32)floorf(q.x), (u32)floorf(q.y))].w;
+    float3 h = t;
+    if (n > 0.0f) {
+        // 5. separable 4x4 Catmull-Rom over the tonemapped history, texel centres at i + 0.5, taps clamped to the screen
+        const float ux = q.x - 0.5f, uy = q.y - 0.5f, fx0 = floorf(ux), fy0 = floorf(uy);
+        float wx[4], wy[4];
+        taa_cr_weights(ux - fx0, wx); taa_cr_weights(uy - fy0, wy);
+        const int ix = (int)fx0 - 1, iy = (int)fy0 - 1;
+        h = f3s(0.0f);
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const u32 yy = (u32)min(max(iy + j, 0), cam.h - 1);
+            float3 row = f3s(0.0f);
+#pragma unroll
+            for (int k = 0; k < 4; k++) row = row + wx[k] * xyz(hist_in[pix(cam, (u32)min(max(ix + k, 0), cam.w - 1), yy)]);
+            h = h + wy[j] * row;
+        }
+        // 6. clip toward the box centre, into the box (YCoCg)
+        const float3 c = 0.5f * (hi + lo), e = 0.5f * (hi - lo) + f3s(kTaaClipEps);
+        const float3 d = taa_ycocg(h) - c;
+        const float m = taa_max(taa_max(fabs_(d.x / e.x), fabs_(d.y / e.y)), fabs_(d.z / e.z));
+        if (m > 1.0f) h = taa_rgb(c + d / m);
+    } else n = 0.0f;
+    // 7-8. blend, count, store
+    const float a = 1.0f / (n + 1.0f), alpha = a > 0.1f ? a : 0.1f;
+    const float3 r = (1.0f - alpha) * h + alpha * t;
+    const float n1 = n + 1.0f;
+    hist_out[i] = f4(r, n1 < 16.0f ? n1 : 16.0f);
+    cam.output[i] = f4(taa_untonemap(r), 1.0f);
 }
 
 
@@ -1940,6 +2036,11 @@ bool launch_denoise_variance_tiled(const CameraDev& c, const SceneDev& s, int cu
     return fast ? variance_tiled_go<true>(c, s, cur, errors, st) : variance_tiled_go<false>(c, s, cur, errors, st);
 }
 void launch_composition(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, cudaStream_t st) { k_composition<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, mode, di_diff, gi_diff); }
+void launch_taa_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, const float4* hist_in, float4* hist_out,
+                        float4 jit, cudaStream_t st) {
+    const dim3 grid((c.w + TAA_TW - 1) / TAA_TW, (c.h + TAA_TH - 1) / TAA_TH);
+    k_taa_resolve<<<grid, TAA_TW * TAA_TH, 0, st>>>(c, s, cur, mode, di_diff, gi_diff, hist_in, hist_out, jit);
+}
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st) { k_output_rgba8<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out); }
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {
     if (nmap) k_ref_tracing<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); else k_ref_tracing<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth);

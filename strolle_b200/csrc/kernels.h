@@ -36,6 +36,10 @@ void launch_denoise_wavelet(const CameraDev& c, const SceneDev& s, int cur, u32 
 bool launch_denoise_wavelet_tiled(const CameraDev& c, const SceneDev& s, u32 frame, u32 stride, float strength, const float4* di_in, float4* di_out, const float4* gi_in, float4* gi_out, float4* pair_out, bool fast, int cfg, u32* errors, cudaStream_t st);
 bool launch_denoise_variance_tiled(const CameraDev& c, const SceneDev& s, int cur, bool fast, u32* errors, cudaStream_t st);
 void launch_composition(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, cudaStream_t st);
+// ST_OPT_TEMPORAL_AA: composes the frame (as launch_composition) into shared memory and resolves it against last frame's history
+// (hist_in) into `output` and hist_out; jit = (J(f), J(f - 1)) in pixels, c.curr / c.prev the jittered cameras (strict build only)
+void launch_taa_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, const float4* hist_in, float4* hist_out,
+                        float4 jit, cudaStream_t st);
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st);
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st);
 void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st);

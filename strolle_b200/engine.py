@@ -29,6 +29,7 @@ OPT_NORMAL_MAPS = 14         # shade with the materials' normal maps (off by def
 OPT_BVH_REFIT = 15           # N > 0: up to N ticks in a row that only move instances bake on the device and refit the BVH (0 = rebuild)
 OPT_LIGHT_GRID = 16          # N in 1..64: light candidates from a world-space grid of N cells along its longest axis (0 = every slot)
 OPT_TEXTURE_FILTER = 17      # 1: material textures filtered through per-image mip chains with a ray-cone level of detail (0 = nearest texel)
+OPT_TEMPORAL_AA = 18         # 1: sub-pixel camera jitter + temporal resolve in place of the composition (0 = one centred ray per pixel)
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
 STAT_WAVELET_TILED_ERRORS = 2
@@ -41,6 +42,7 @@ STAT_NORMAL_MAP_LAUNCHES = 8   # launches of the normal-mapped kernel variants
 STAT_BVH_REFITS = 9            # refit ticks (OPT_BVH_REFIT) since the engine was created
 STAT_LIGHT_GRID_BUILDS = 10    # light grid builds (OPT_LIGHT_GRID) since the engine was created
 STAT_TEXTURE_MIP_BUILDS = 11   # mip-chain builds (OPT_TEXTURE_FILTER) since the engine was created
+STAT_TAA_RESOLVES = 12         # temporal resolve launches (OPT_TEMPORAL_AA) since the engine was created
 
 
 class StrolleError(RuntimeError):

@@ -626,3 +626,28 @@ def apply(engine, scene):
     engine.update_sun(*scene["sun"])
     c = scene["camera"]
     return engine.create_camera(c["mode"], c["denoise"], c["ref_depth"], c["w"], c["h"], c["transform"], c["projection"])
+
+
+def aa_edges(width=96, height=64, mode=MODE_IMAGE, denoise=True, ref_depth=1):
+    """Measures anti-aliasing (ST_OPT_TEMPORAL_AA): a black (albedo 0, metallic 0, reflectance 0) backdrop filling the view, and in front
+    of it, 0.1 units off the backdrop, an emissive quad rotated by 0.3 rad about the view axis and an emissive bar 0.3 pixels wide and
+    tilted by 0.05 rad.  No lights, the sun below the horizon: every composed pixel is exactly an emissive colour or 0, so the frame is
+    free of noise and its edges are the only signal.  The camera at the origin looks down -z; the backdrop is at z = -5."""
+    black = material((0.0, 0.0, 0.0, 1.0), reflectance=0.0)
+    materials = {120: (black, False),
+                 121: (material((0.0, 0.0, 0.0, 1.0), emissive=(1.0, 0.6, 0.3, 1.0), reflectance=0.0), False),
+                 122: (material((0.0, 0.0, 0.0, 1.0), emissive=(0.4, 0.8, 1.0, 1.0), reflectance=0.0), False)}
+    z, zf = -5.0, -4.9
+    px = 2.0 * -zf * math.tan(math.pi / 8.0) / height   # one pixel at the depth of the emissive shapes
+
+    def rotated(cx, cy, hw, hh, a, zz):
+        c, s = math.cos(a), math.sin(a)
+        pts = [(cx + c * x - s * y, cy + s * x + c * y, zz) for x, y in ((-hw, -hh), (hw, -hh), (hw, hh), (-hw, hh))]
+        return np.stack(_quad(*pts, (0, 0, 1)))
+    meshes = {220: np.stack(_quad((-20, -20, z), (20, -20, z), (20, 20, z), (-20, 20, z), (0, 0, 1))),
+              221: rotated(-0.35 * px * width, 0.0, 0.25 * px * width, 0.3 * px * height, 0.3, zf),
+              222: rotated(0.3 * px * width, 0.0, 0.15 * px, 0.4 * px * height, 0.05, zf)}
+    instances = [(320, 220, 120, IDENTITY_AFFINE), (321, 221, 121, IDENTITY_AFFINE), (322, 222, 122, IDENTITY_AFFINE)]
+    cam = dict(mode=mode, denoise=denoise, ref_depth=ref_depth, w=width, h=height, transform=look_at_transform((0.0, 0.0, 0.0), (0.0, 0.0, -1.0)),
+               projection=perspective_infinite_reverse_rh(math.pi / 4.0, width / height, 0.1))
+    return dict(name="aa_edges", meshes=meshes, materials=materials, instances=instances, lights=[], sun=(0.0, -1.0), camera=cam)
