@@ -2002,7 +2002,7 @@ int st_device_math(st_engine* e, int op, const float* a, const float* b, float* 
     if ((rc = da.ensure(n * 4)) || (rc = db.ensure(n * 4)) || (rc = dc.ensure(n * 4))) return rc;
     CK(cudaMemcpyAsync(da.p, a, n * 4, cudaMemcpyHostToDevice, e->stream));
     if (b) CK(cudaMemcpyAsync(db.p, b, n * 4, cudaMemcpyHostToDevice, e->stream));
-    // op 0-6: the strict elementary functions, op 7: the texture filter's log2; op 16-21: the fast-shading build's sin, cos, exp, pow, sqrt and division
+    // op 0-6: the strict elementary functions, op 7: the texture filter's log2; op 16-23: the fast-shading build's sin, cos, exp, pow, sqrt, division, acos and atan2
     if (op >= 16) stf::launch_math_shading(op - 16, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
     else launch_math(op, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
     CK(cudaMemcpyAsync(out, dc.p, n * 4, cudaMemcpyDeviceToHost, e->stream));

@@ -1768,6 +1768,7 @@ __global__ void k_math_shading(int op, const float* __restrict__ a, const float*
     switch (op) {
         case 0: r = sin_det(x); break; case 1: r = cos_det(x); break; case 2: r = exp_det(x); break;
         case 3: r = pow_det(x, y); break; case 4: r = sqrtf(x); break; case 5: r = x / y; break;
+        case 6: r = acos_det(x); break; case 7: r = atan2_det(x, y); break;
     }
     out[i] = r;
 }

@@ -396,8 +396,10 @@ class Engine:
 
     def device_math(self, op, a, b=None):
         ops = {"sin": 0, "cos": 1, "acos": 2, "atan2": 3, "exp": 4, "pow": 5, "acos_approx": 6, "log2_lod": 7,
-               # the fast-shading build's forms (ST_OPT_SHADING_FAST_MATH): SFU sin / cos / exp / pow, sqrt.approx, div.full
-               "sin_fast": 16, "cos_fast": 17, "exp_fast": 18, "pow_fast": 19, "sqrt_fast": 20, "div_fast": 21}
+               # the fast-shading build's forms (ST_OPT_SHADING_FAST_MATH): SFU sin / cos / exp / pow, sqrt.approx, div.full, and the
+               # Cephes acos / atan2 compiled with FMA contraction, sqrt.approx and div.full
+               "sin_fast": 16, "cos_fast": 17, "exp_fast": 18, "pow_fast": 19, "sqrt_fast": 20, "div_fast": 21, "acos_fast": 22,
+               "atan2_fast": 23}
         a = _f(a)
         b = _f(b) if b is not None else np.zeros_like(a)
         out = np.empty_like(a)

@@ -450,10 +450,12 @@ def di_fields(res):
                 occ=(b & 0xFF) > 0, conf=((b >> 8) & 0xFF).astype(np.float64), point=r[:, 4:7].copy(), id=r[:, 7].view(np.uint32).copy())
 
 
-def di_resolving(n2w, w, h, d0, d1, lights, res_in, res_out, fast):
-    """K10 for the pixels with a surface.  `res_in` = the reservoirs it reads (next), `res_out` = what it wrote (prev): the occluded
-    bit there is the visibility the kernel traced.  Returns dict(diff, spec (Num (H, W, 3)), conf (H, W), some, undecided, res)
-    where `res` is the (N, 8) reservoir copy expected (with the device's visibility)."""
+def di_resolving(n2w, w, h, d0, d1, lights, res_in, res_out, fast, atm, mutation=None):
+    """K10.  `res_in` = the reservoirs it reads (next), `res_out` = what it wrote (prev): the occluded bit there is the visibility the
+    kernel traced.  `atm` = atmosphere_inputs(engine): the sky pixels' diffuse output is Atmosphere::sample along the camera ray
+    times (1 - 0) / pi (an empty G-buffer entry has metallic 0) and their specular output 0.  Returns dict(diff, spec (Num (H, W,
+    3)), conf (H, W), some, undecided, res, sky) where `res` is the (N, 8) reservoir copy expected (with the device's visibility)
+    and `sky` the atmosphere restatement of the pixels without a surface (`mutation`: one of SKY_MUTATIONS)."""
     ht = hit(n2w, w, h, d0, d1, fast)
     some = ht["g"]["some"]
     ri, ro = di_fields(res_in), di_fields(res_out)
@@ -471,7 +473,9 @@ def di_resolving(n2w, w, h, d0, d1, lights, res_in, res_out, fast):
     b = want[:, 3].view(np.uint32)
     bits = np.where(some.reshape(-1), (np.where(occ.reshape(-1), 1, 0) | (1 << 8)).astype(np.uint32), b)
     want[:, 3] = bits.view(np.float32)
-    return dict(diff=diff, spec=spec, conf=conf, some=some, undecided=lr["undecided"] & ~occ & some, res=want)
+    sky = atmosphere_sample(atm, ht["dir"][~some], fast, mutation)
+    sky["diff"] = sky["lum"] * ((1.0 - Num(np.zeros(len(sky["domain"])), 0.0, fast)) / PI).x3()
+    return dict(diff=diff, spec=spec, conf=conf, some=some, undecided=lr["undecided"] & ~occ & some, res=want, sky=sky)
 
 
 def _mis_m(q0, q1):
@@ -1504,6 +1508,10 @@ def check_resolving(diff, spec, res_out, r, what, check_within):
     want = np.where(took_zero, 0.0, r["spec"].v)
     bound = np.where(took_zero, 0.0, r["spec"].e)
     ratio = max(ratio, check_within(spec[..., :3][some], want[some], bound[some], f"{what} specular"))
+    sky = r["sky"]
+    ok = sky["domain"]
+    assert (spec[..., :3][~some][ok].view(np.uint32) == 0).all(), f"{what}: sky specular is not +0"
+    ratio = max(ratio, check_within(diff[..., :3][~some][ok], sky["diff"].v[ok], sky["diff"].e[ok], f"{what} sky"))
     return ratio, int(und.sum()), (r["diff"], r["spec"])
 
 
@@ -1516,6 +1524,216 @@ def tight_fraction(nums, some):
         n += int(fin.sum())
         t += int((e[fin] < 1e-3 * np.abs(v[fin])).sum())
     return t / max(n, 1), n
+
+
+# ---- the sky: Atmosphere::sample -------------------------------------------------------------------------------------------------
+# Atmosphere::sample (atmosphere.rs:86-205), World::sun_dir (world.rs:19-25), Ray::intersect_sphere (ray.rs:304-321).  The LUTs are
+# read from the engine as exact inputs; the port fetches them with an explicit f32 bilinear filter, clamp to edge, texel centres at
+# +0.5.  The fetched value is bounded through its sensitivity to the coordinates: the largest difference of neighbouring texels over
+# every cell the coordinates' bounds reach, times those bounds, plus 24 u of the largest texel for the two lerps' roundings.  acos
+# near +-1 and sqrt(|altitude|) near the horizon have unbounded derivatives: acos takes its modulus of continuity acos(1 - d) where
+# that is smaller than the derivative bound, and Num.sqrt already takes sqrt(e) there.  Four decisions: the nadir branch
+# |altitude| > pi / 2 - 1e-4 (altitude is horizon - zenith angle, so the branch is taken looking straight down), the atan2 cut (u
+# jumps between 0 and 1 opposite the sun), the sun disc cos >= min_cos and the ground test ray_sphere >= 0.  Where one is within its
+# bound, both outcomes are computed and the value is accepted anywhere between them (their hull); the pixel is counted.
+ACOS_ABS = 2.0 ** -21           # the strict Cephes acosf on [-1, 1], absolute: 3.0e-7 measured (test_ref64_constants)
+ATAN2_ABS = 2.0 ** -21          # the strict Cephes atan2f, absolute: 2.7e-7 measured (test_ref64_constants)
+# the fast build runs the same Cephes kernels with FMA contraction, sqrt.approx and div.full inside: measured on an H100, acos 3.2e-7
+# and atan2 2.9e-7 (test_fast_elementary_functions_within_assumed_constants).  Inlined into a pass, the compiler may contract them
+# differently, each change moving the result by a few of its ulps (<= 2^-22 on results <= pi), so the constant is four times the
+# strict one
+ACOS_ABS_FAST = ATAN2_ABS_FAST = 2.0 ** -19
+ATM_GROUND, ATM_TOP = _f32c(6.360), _f32c(6.460)
+ATM_VIEW_Y = _f32c(np.float32(6.360) + np.float32(0.0002))
+ATM_ZENITH = _f32c(np.float32(0.5 * np.float32(np.pi)) - np.float32(0.0001))
+ATM_EXPOSURE = 20.0
+# misreadings of atmosphere.rs that the sky check must catch (test_restir_gi_reference.py)
+SKY_MUTATIONS = ("sky_azimuth_no_pi", "sky_altitude_no_sqrt")
+SKY_BRANCHES = ("sun disc", "bloom", "ground", "nadir", "atan2 cut")
+
+
+def atmosphere_inputs(engine):
+    """What Atmosphere::sample reads from an engine (the CUDA engine or the oracle): the sky LUT (256 x 256), the transmittance LUT
+    (256 x 64) and the sun's (azimuth, altitude)."""
+    world = engine.read_scene("world")
+    return dict(sky=engine.read_scene("sky_lut").reshape(256, 256, 4), trans=engine.read_scene("transmittance_lut").reshape(64, 256, 4),
+                sun=(float(world[1]), float(world[2])))
+
+
+def cross3(a, b):
+    """glam Vec3::cross."""
+    ax, ay, az, bx, by, bz = a.col(0), a.col(1), a.col(2), b.col(0), b.col(1), b.col(2)
+    return stack3(ay * bz - az * by, az * bx - ax * bz, ax * by - ay * bx)
+
+
+def _hull(mask, a, b):
+    """Where `mask`, a value that covers both a and b; elsewhere a."""
+    lo, hi = np.minimum(a.v - a.e, b.v - b.e), np.maximum(a.v + a.e, b.v + b.e)
+    with np.errstate(invalid="ignore"):
+        return Num(np.where(mask, (lo + hi) / 2, a.v), np.where(mask, (hi - lo) / 2, a.e), a.fast)
+
+
+def _acos(x):
+    """acos of a Num: 1 / sqrt(1 - (|x| + e)^2) times e, or acos(1 - 2 e) wherever that is smaller (the steepest change of acos over
+    an interval of width 2 e is at +-1), plus the function's error.  Returns (Num, domain): domain is False where the f32 argument may
+    lie outside [-1, 1] (the device returns NaN there)."""
+    k = ACOS_ABS_FAST if x.fast else ACOS_ABS
+    with np.errstate(invalid="ignore", divide="ignore"):
+        reach = np.abs(x.v) + x.e
+        slope = np.where(reach < 1, x.e / np.sqrt(np.maximum(1 - reach * reach, 1e-300)), np.inf)
+        modulus = np.arccos(np.clip(1 - 2 * x.e, -1, 1))
+        v = np.arccos(np.clip(x.v, -1, 1))
+    return Num(v, np.minimum(slope, modulus) + k, x.fast), reach <= 1
+
+
+def _atan2(y, x):
+    """atan2(y, x) + nothing: a move of (x, y) by at most d = ex + ey turns the angle by at most asin(d / r), r = |(x, y)|, away from
+    the cut (d >= r: anything), plus the function's error."""
+    k = ATAN2_ABS_FAST if x.fast else ATAN2_ABS
+    r = np.hypot(x.v, y.v)
+    d = x.e + y.e
+    with np.errstate(invalid="ignore", divide="ignore"):
+        turn = np.where(d < r, np.arcsin(np.minimum(d / np.where(r > 0, r, 1.0), 1.0)), np.pi)
+    return Num(np.arctan2(y.v, x.v), turn + k, x.fast)
+
+
+def _exp(x):
+    """exp of a Num <= 0: exp(x + e) e for the argument's bound, plus the tier's relative error (R.EXP_REL strict; EXP_REL_FAST and
+    __expf's scaled argument in the fast build)."""
+    from tests.ref64_svgf import EXP_REL
+    rel = (EXP_REL_FAST + 2 * U * np.abs(x.v) * np.log2(np.e)) if x.fast else EXP_REL
+    with np.errstate(over="ignore"):
+        v = np.exp(x.v)
+        return Num(v, np.exp(x.v + x.e) * x.e + rel * v + SUB, x.fast)
+
+
+def lut_fetch(lut, fx, fy):
+    """The port's bilinear fetch of an (H, W, 4) LUT at texel coordinates fx = u W - 0.5, fy = v H - 0.5 (Num (N,)): the exact
+    bilinear value at the coordinates' values (clamped to the edge texels' centres), bounded by the coordinates' bounds times the
+    largest neighbouring-texel difference over the cells they reach, plus the lerps' roundings.  Returns Num (N, 3)."""
+    h, w = lut.shape[:2]
+    L = np.asarray(lut, np.float32)[..., :3].astype(np.float64)
+    fin = np.isfinite(fx.v) & np.isfinite(fy.v)
+    x = np.clip(np.where(fin, fx.v, 0.0), 0, w - 1); y = np.clip(np.where(fin, fy.v, 0.0), 0, h - 1)
+    x0 = np.minimum(np.floor(x), w - 2).astype(np.int64); y0 = np.minimum(np.floor(y), h - 2).astype(np.int64)
+    tx, ty = (x - x0)[:, None], (y - y0)[:, None]
+    a, b, c, d = L[y0, x0], L[y0, x0 + 1], L[y0 + 1, x0], L[y0 + 1, x0 + 1]
+    top, bot = a + (b - a) * tx, c + (d - c) * tx
+    val = top + (bot - top) * ty
+    dx, dy = np.abs(np.diff(L, axis=1)), np.abs(np.diff(L, axis=0))      # (H, W-1, 3), (H-1, W, 3)
+    absl = np.abs(L)
+    ex, ey = np.where(fin, fx.e, np.inf), np.where(fin, fy.e, np.inf)
+    with np.errstate(invalid="ignore"):
+        xl = np.clip(np.floor(np.where(fin, fx.v - ex, 0.0)), 0, w - 1).astype(np.int64)
+        yl = np.clip(np.floor(np.where(fin, fy.v - ey, 0.0)), 0, h - 1).astype(np.int64)
+    # coordinate bounds below one texel reach cells xl..xl+2 and yl..yl+2: the x differences of rows yl..yl+3, the y differences of
+    # columns xl..xl+3 (indices clipped to the LUT: a repeated entry only repeats a maximum)
+    def win(arr, r, c):
+        p = np.pad(arr, ((0, r - 1), (0, c - 1), (0, 0)), mode="edge")
+        mx = np.max([p[i:i + arr.shape[0], j:j + arr.shape[1]] for i in range(r) for j in range(c)], axis=0)
+        return mx[np.minimum(yl, arr.shape[0] - 1), np.minimum(xl, arr.shape[1] - 1)]
+    lx, ly, m = win(dx, 4, 3), win(dy, 3, 4), win(absl, 4, 4)
+    err = lx * ex[:, None] + ly * ey[:, None] + 24 * U * m
+    for i in np.flatnonzero(~((ex < 1) & (ey < 1))):
+        if not (np.isfinite(ex[i]) and np.isfinite(ey[i])):
+            err[i] = np.inf
+            continue
+        xh = int(np.clip(np.floor(fx.v[i] + ex[i]), 0, w - 1)); yh = int(np.clip(np.floor(fy.v[i] + ey[i]), 0, h - 1))
+        cx = dx[yl[i]:yh + 2, xl[i]:min(xh + 1, w - 1)].reshape(-1, 3)
+        cy = dy[yl[i]:min(yh + 1, h - 1), xl[i]:xh + 2].reshape(-1, 3)
+        mm = absl[yl[i]:yh + 2, xl[i]:xh + 2].reshape(-1, 3).max(0)
+        err[i] = (cx.max(0) if len(cx) else 0.0) * ex[i] + (cy.max(0) if len(cy) else 0.0) * ey[i] + 24 * U * mm
+    return Num(val, err, fx.fast)
+
+
+def world_sun_dir(azimuth, altitude, fast):
+    """World::sun_dir: (cos alt sin az, sin alt, -cos alt cos az) through `sincos`."""
+    sa, ca = sincos(Num(np.float64(np.float32(altitude)), 0.0, fast))
+    sz, cz = sincos(Num(np.float64(np.float32(azimuth)), 0.0, fast))
+    return stack3(ca * sz, sa, (-ca) * cz)
+
+
+def atmosphere_sample(atm, ray_dir, fast, mutation=None):
+    """Atmosphere::sample(sun_dir, ray_dir) for ray directions ray_dir (Num (N, 3)), exposure included.  Returns dict(lum (Num (N,
+    3)), domain (False where the zenith angle's acos may be NaN: not compared), undecided {decision: mask}, branches {name: count})."""
+    n = ray_dir.v.shape[0]
+    z = lambda a: Num(np.broadcast_to(np.asarray(a, np.float64), (n,)).copy(), 0.0, fast)
+    sun = world_sun_dir(*atm["sun"], fast)
+    sun = Num(np.broadcast_to(sun.v, (n, 3)), np.broadcast_to(sun.e, (n, 3)), fast)
+    vp = stack3(z(0.0), z(ATM_VIEW_Y), z(0.0))
+    height = dot3(vp, vp).sqrt()
+    up = vp / height.x3()
+    t = (height * height - z(ATM_GROUND) * ATM_GROUND).sqrt() / height
+    horizon, _ = _acos(t.clip(-1.0, 1.0))
+    zen, domain = _acos(dot3(ray_dir, up))
+    altitude = horizon - zen
+    und, br = {}, dict.fromkeys(SKY_BRANCHES, 0)
+    # sample_sky_lut: the nadir branch, else the azimuth about the sun
+    a = altitude.abs()
+    nadir = a.v > ATM_ZENITH
+    und["nadir"] = np.abs(a.v - ATM_ZENITH) <= a.e
+    right = cross3(sun, up)
+    forward = cross3(up, right)
+    proj = norm3(ray_dir - up * dot3(ray_dir, up).x3())
+    s, c = dot3(proj, right), dot3(proj, forward)
+    cut = (c.v < 0) & (np.abs(s.v) <= s.e)          # opposite the sun, the sign of sin theta (and so u = 0 or 1) is undecided
+    und["atan2 cut"] = cut & ~nadir
+
+    def fetch(az, nadir):
+        if mutation != "sky_azimuth_no_pi":
+            az = az + PI
+        u = where(nadir, z(0.0), az / _f32c(2 * np.float32(np.pi)))
+        m = (altitude.abs() * 2.0) / PI
+        m = m if mutation == "sky_altitude_no_sqrt" else m.sqrt()
+        sign_known = np.abs(altitude.v) > altitude.e
+        half = where(sign_known, Num(np.copysign(m.v, altitude.v), m.e, fast), Num(np.zeros(n), m.v + m.e, fast))
+        v = 0.5 + 0.5 * half
+        return lut_fetch(atm["sky"], u * 256.0 - 0.5, v * 256.0 - 0.5), u
+
+    ang = _atan2(s, c)
+    lum, u = fetch(ang, nadir)
+    if cut.any():
+        lum = _hull(cut[:, None], lum, fetch(Num(-ang.v, ang.e, fast), nadir)[0])
+    if und["nadir"].any():
+        lum = _hull(und["nadir"][:, None], lum, fetch(ang, ~nadir)[0])
+    br["nadir"] = int((nadir & ~und["nadir"]).sum())
+    br["atan2 cut"] = int((~nadir & (c.v < 0) & ((u.v < 0.5 / 256) | (u.v > 1 - 0.5 / 256))).sum())
+    # evaluate_bloom / interpolate_bloom
+    min_cos = sincos(Num(_f32c(0.53), 0.0, fast) * PI / 180.0)[1]
+    cos_t = dot3(ray_dir, sun)
+    dc = cos_t - min_cos
+    disc = dc.v >= 0
+    und["sun disc"] = np.abs(dc.v) <= dc.e
+    offset = min_cos - cos_t
+    gauss = _exp((-offset) * 50000.0) * 0.5
+    inv = (1.0 / (0.02 + offset * 300.0)) * 0.01
+    bloom = where(disc, z(1.0), gauss + inv)
+    bloom = _hull(und["sun disc"], bloom, where(disc, gauss + inv, z(1.0)))
+
+    def smooth(b):
+        tt = ((b - 0.002) / (1.0 - z(0.002))).sat()
+        return (tt * tt) * (3.0 - 2.0 * tt)
+    sl = smooth(bloom)
+    # sun_lum.length_squared() > 0, then Ray::intersect_sphere(GROUND) >= 0 from the view position
+    lit = sl.v > 0
+    lit_und = (sl.v <= sl.e) & (sl.e > 0)
+    b = dot3(vp, ray_dir)
+    disc_r = b * b - (dot3(vp, vp) - z(ATM_GROUND) * ATM_GROUND)
+    ground = (b.v <= 0) & (disc_r.v >= 0)
+    und["ground"] = lit & ((np.abs(disc_r.v) <= disc_r.e) | ((np.abs(b.v) <= b.e) & (disc_r.v + disc_r.e >= 0)))
+    trans = lut_fetch(atm["trans"], (0.5 + 0.5 * dot3(sun, up)).sat() * 256.0 - 0.5,
+                      ((height - ATM_GROUND) / (z(ATM_TOP) - ATM_GROUND)).sat() * 64.0 - 0.5)
+    sun_lum = sl.x3() * trans
+    zero3 = Num(np.zeros((n, 3)), 0.0, fast)
+    out = where(lit & ~ground, sun_lum, zero3)
+    out = _hull((und["ground"] | lit_und)[:, None], out, where(ground & ~und["ground"], zero3, sun_lum))
+    br["sun disc"] = int((disc & ~und["sun disc"]).sum())
+    br["bloom"] = int((~disc & lit & ~lit_und & ~ground & ~und["ground"]).sum())
+    br["ground"] = int((lit & ground & ~und["ground"]).sum())
+    lum = (lum + out) * ATM_EXPOSURE
+    und = {k: v & domain for k, v in und.items()}
+    und["acos domain"] = ~domain
+    return dict(lum=lum, domain=domain, undecided=und, branches=br)
 
 
 # ---- fast-tier elementary functions -----------------------------------------------------------------------------------------

@@ -292,6 +292,15 @@ def test_ref64_constants(oracle):
     x = np.concatenate([np.linspace(0.0, 2 * np.pi, 400001), np.random.RandomState(1).uniform(0, 2 * np.pi, 10 ** 6)]).astype(np.float32)
     for op, fn in (("sin", np.sin), ("cos", np.cos)):
         assert np.abs(oracle.math(op, x) - fn(x.astype(np.float64))).max() <= Q.SIN_ABS, op
+    # the strict acos and atan2 that Atmosphere::sample's zenith angle, horizon and azimuth take, on all of [-1, 1] (densely toward
+    # +-1) and on points of every angle at radii 1e-3 to 1.26
+    rng = np.random.RandomState(2)
+    x = np.concatenate([np.linspace(-1.0, 1.0, 400001), 1 - np.logspace(-8, 0, 10 ** 5), np.logspace(-8, 0, 10 ** 5) - 1]).astype(np.float32)
+    x = x[np.abs(x) <= 1]
+    assert np.abs(oracle.math("acos", x) - np.arccos(x.astype(np.float64))).max() <= Q.ACOS_ABS
+    a, r = rng.uniform(0, 2 * np.pi, 10 ** 6), 10 ** rng.uniform(-3, 0.1, 10 ** 6)
+    ys, xs = (r * np.sin(a)).astype(np.float32), (r * np.cos(a)).astype(np.float32)
+    assert np.abs(oracle.math("atan2", ys, xs) - np.arctan2(ys.astype(np.float64), xs.astype(np.float64))).max() <= Q.ATAN2_ABS
 
 
 def _svgf_chain_check(oracle, blue_noise, scene, frames=6, moves=(3, 4, 5)):
@@ -486,7 +495,8 @@ def _restir_chain_check(oracle, blue_noise, scene, frames=13, moves=(3, 5, 8, 11
         r2 = rd("di_reservoirs_2")
         e.render_range(cam, k10, k10)
         n2w = Q.ndc_to_world(t, c["projection"])
-        k10r = Q.di_resolving(n2w, w, h, d0, d1, e.read_scene("lights"), r2, rd("di_reservoirs_0"), fast=False)
+        k10r = Q.di_resolving(n2w, w, h, d0, d1, e.read_scene("lights"), r2, rd("di_reservoirs_0"), fast=False,
+                              atm=Q.atmosphere_inputs(e))
         ratio, und, _ = Q.check_resolving(rd("di_diff_samples").reshape(h, w, 4), rd("di_spec_samples").reshape(h, w, 4),
                                           rd("di_reservoirs_0"), k10r, f"f{f} K10", check_within)
         stats["K10"] = [max(stats["K10"][0], ratio), stats["K10"][1] + und]

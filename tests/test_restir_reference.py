@@ -251,7 +251,8 @@ class Chain:
         r2 = e.read_buffer(cam, "di_reservoirs_2")
         fr.run_to(k10)
         res0 = e.read_buffer(cam, "di_reservoirs_0")
-        r = Q.di_resolving(Q.ndc_to_world(self.t, self.scene["camera"]["projection"]), w, h, d0, d1, e.read_scene("lights"), r2, res0, self.fast)
+        r = Q.di_resolving(Q.ndc_to_world(self.t, self.scene["camera"]["projection"]), w, h, d0, d1, e.read_scene("lights"), r2, res0, self.fast,
+                            Q.atmosphere_inputs(e))
         ratio, und, b = Q.check_resolving(fr.read("di_diff_samples"), fr.read("di_spec_samples"), res0, r, f"f{f} K10", check_within)
         s = self.stats["K10"]
         self.stats["K10"] = [max(s[0], ratio), s[1] + und, s[2] + int(r["some"].sum())]
@@ -539,8 +540,9 @@ def test_fast_shading_build_is_not_strict(gpu, blue_noise):
 # ---- the fast build's elementary functions ------------------------------------------------------------------------------------
 
 def test_fast_elementary_functions_within_assumed_constants(gpu, blue_noise):
-    """sin / cos (__sincosf), exp (__expf), pow (__powf), sqrt (sqrt.approx) and division (div.full) of the fast-shading build, measured
-    on the argument ranges the ReSTIR kernels use, within the constants a bound on them assumes (tests/ref64_restir.py)."""
+    """sin / cos (__sincosf), exp (__expf), pow (__powf), sqrt (sqrt.approx), division (div.full), acos and atan2 of the fast-shading
+    build, measured on the argument ranges the ReSTIR kernels and the sky use, within the constants a bound on them assumes
+    (tests/ref64_restir.py)."""
     e = gpu.Engine(blue_noise=blue_noise)
     rng = np.random.RandomState(3)
     x = np.concatenate([np.linspace(0, 2 * np.pi, 200001), rng.uniform(0, 2 * np.pi, 10 ** 6)]).astype(np.float32)
@@ -568,8 +570,17 @@ def test_fast_elementary_functions_within_assumed_constants(gpu, blue_noise):
     want = a.astype(np.float64) / b.astype(np.float64)
     fin = (np.abs(want) > 1e-37) & (np.abs(want) < 1e37)
     rel_d = (np.abs(got - want) / np.abs(want))[fin].max()
-    print(f"\nfast elementary functions: sin {err_s:.3g} cos {err_c:.3g} (abs), exp {rel_e:.3g}, pow {rel_p:.3g}, sqrt {rel_q:.3g}, "
-          f"div {rel_d:.3g} (rel)")
+    # acos on all of [-1, 1] (densely toward +-1: the sky's zenith angle and horizon), atan2 of points of every angle at radii 1e-3 to
+    # 1.26 (the sky's azimuth)
+    xa = np.concatenate([np.linspace(-1.0, 1.0, 400001), 1 - np.logspace(-8, 0, 10 ** 5), np.logspace(-8, 0, 10 ** 5) - 1]).astype(np.float32)
+    xa = xa[np.abs(xa) <= 1]
+    err_a = np.abs(e.device_math("acos_fast", xa) - np.arccos(xa.astype(np.float64))).max()
+    ang, rad = rng.uniform(0, 2 * np.pi, 10 ** 6), 10 ** rng.uniform(-3, 0.1, 10 ** 6)
+    ys, xs2 = (rad * np.sin(ang)).astype(np.float32), (rad * np.cos(ang)).astype(np.float32)
+    err_t = np.abs(e.device_math("atan2_fast", ys, xs2) - np.arctan2(ys.astype(np.float64), xs2.astype(np.float64))).max()
+    print(f"\nfast elementary functions: sin {err_s:.3g} cos {err_c:.3g} acos {err_a:.3g} atan2 {err_t:.3g} (abs), exp {rel_e:.3g}, "
+          f"pow {rel_p:.3g}, sqrt {rel_q:.3g}, div {rel_d:.3g} (rel)")
+    assert err_a <= Q.ACOS_ABS_FAST and err_t <= Q.ATAN2_ABS_FAST
     assert err_s <= Q.SIN_ABS_FAST and err_c <= Q.SIN_ABS_FAST
     assert rel_e <= Q.EXP_REL_FAST and rel_p <= Q.POW_REL_FAST
     assert rel_q <= Q.SQRT_REL_FAST and rel_d <= Q.DIV_REL
