@@ -113,6 +113,18 @@ int st_insert_light(st_engine* e, st_handle light, const st_light* l);
 int st_remove_light(st_engine* e, st_handle light);
 /* Engine::update_sun (lib.rs:242-245) */
 int st_update_sun(st_engine* e, float azimuth, float altitude);
+/* An equirectangular environment map in place of the procedural sky (default: none, the reference's atmosphere).  `rgba32f` holds
+ * width x height texels of linear RGB (4 floats each, alpha ignored), row-major, row 0 the zenith; NULL clears the map (the procedural
+ * sky comes back and the device copy is freed at the next st_tick).  The map's radiance along a direction d is the bilinear blend at
+ * u = (atan2(d.x, -d.z) + rotation) / 2 pi + 0.5, v = acos(d.y) / pi (columns wrapped, rows clamped), times `intensity`: with
+ * rotation 0 the centre column is seen looking down -Z, u = 0.75 looking down +X.  It replaces the sky at every site that evaluates it
+ * (sky pixels, GI bounces that miss, the GI bounce's sky draw, Reference mode's miss) without the procedural sky's x20 exposure; the
+ * GI sky draw keeps its probability of 0.25 whatever the sun's altitude.  The sun light still follows st_update_sun: to light a scene
+ * from the map alone, put the sun below the horizon (altitude < 0: its colour is then 0).  ST_ERR_INVALID, and no change, when a side
+ * is outside 1..16384, an RGB value is negative or not finite, `intensity` is negative or not finite, or `rotation` is not finite.
+ * `rotation` is reduced into [0, 2 pi) in double, then rounded to f32.  Takes effect at the next st_tick, which uploads the texels;
+ * ST_STAT_ENVIRONMENT_MAP_LAUNCHES counts the launches that evaluate it (DESIGN.md §2 "Environment map"). */
+int st_set_environment_map(st_engine* e, const float* rgba32f, uint32_t width, uint32_t height, float intensity, float rotation);
 
 /* Engine::create_camera / update_camera / delete_camera (lib.rs:252-294) */
 int st_create_camera(st_engine* e, const st_camera* camera, st_camera_handle* out);
@@ -153,7 +165,9 @@ int st_read_buffer(st_engine* e, st_camera_handle camera, const char* name, floa
  * 1, level count} for its base colour, emissive and metallic-roughness textures ({0, 0}: none; a count of 1: a 1x1 image, level 0
  * only), then the T
  * RGBA8 texels of the pool (byte 0 = red).  The pool holds levels 1.. of every live image in insertion order, level after level,
- * each row-major; level k + 1 is max(1, w_k >> 1) x max(1, h_k >> 1). */
+ * each row-major; level k + 1 is max(1, w_k >> 1) x max(1, h_k >> 1).  While the frames render with an environment map (set, and
+ * taken by a tick), "environment_map" as 32-bit words: {W, H, intensity bits, rotation bits (reduced)}, then the W x H x 4 floats of
+ * the texels as uploaded. */
 int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap_floats, size_t* count);
 int st_bvh_depth(st_engine* e, int* depth);
 uint32_t st_frame(st_engine* e);
@@ -167,7 +181,8 @@ int st_set_frame(st_engine* e, uint32_t frame);
 int st_trace_closest(st_engine* e, const float* rays, size_t n, float* out, float* device_ms);
 int st_trace_any(st_engine* e, const float* rays, size_t n, uint32_t* out, float* device_ms);
 /* elementary functions as evaluated on the device (op: 0 sin, 1 cos, 2 acos, 3 atan2, 4 exp, 5 pow, 6 glam's acos_approx, 7 the
- * flag-independent log2 of ST_OPT_TEXTURE_FILTER's level of detail, for finite a > 0) */
+ * flag-independent log2 of ST_OPT_TEXTURE_FILTER's level of detail, for finite a > 0, 8 and 9 the flag-independent acos and
+ * atan2(a, b) of the environment map's lookup) */
 int st_device_math(st_engine* e, int op, const float* a, const float* b, float* out, size_t n);
 /* Per-pass device time (ms, CUDA events) accumulated since the last reset; `ms`/`launches`
  * have ST_PASS_COUNT entries indexed by st_pass_name(). */
@@ -299,7 +314,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_BVH_REFITS = 9 /* refit ticks (ST_OPT_BVH_REFIT) since creation */,
        ST_STAT_LIGHT_GRID_BUILDS = 10 /* light grid builds (ST_OPT_LIGHT_GRID) since creation */,
        ST_STAT_TEXTURE_MIP_BUILDS = 11 /* mip-chain builds (ST_OPT_TEXTURE_FILTER) since creation */,
-       ST_STAT_TAA_RESOLVES = 12 /* temporal resolve launches (ST_OPT_TEMPORAL_AA) since creation */ };
+       ST_STAT_TAA_RESOLVES = 12 /* temporal resolve launches (ST_OPT_TEMPORAL_AA) since creation */,
+       ST_STAT_ENVIRONMENT_MAP_LAUNCHES = 13 /* launches of the environment-mapped kernel variants (st_set_environment_map) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,
@@ -391,6 +407,7 @@ int st_multi_remove_instance(st_multi* m, st_handle instance);
 int st_multi_insert_light(st_multi* m, st_handle light, const st_light* l);
 int st_multi_remove_light(st_multi* m, st_handle light);
 int st_multi_update_sun(st_multi* m, float azimuth, float altitude);
+int st_multi_set_environment_map(st_multi* m, const float* rgba32f, uint32_t width, uint32_t height, float intensity, float rotation);
 int st_multi_create_camera(st_multi* m, const st_camera* camera, st_camera_handle* out);
 int st_multi_update_camera(st_multi* m, st_camera_handle camera, const st_camera* desc);
 int st_multi_delete_camera(st_multi* m, st_camera_handle camera);

@@ -50,6 +50,8 @@ pub struct StrolleSun {
 /// `texture_filter`: filter material textures through mip chains (false, the default, takes the nearest texel, as the reference does).
 /// `temporal_aa`: anti-alias with sub-pixel camera jitter and a temporal resolve (false, the default, renders one ray through each
 /// pixel centre, as the reference does); needs one GPU.
+/// `environment_map`: light the scene from an equirectangular HDR map in place of the procedural sky (None, the default, keeps the
+/// reference's sky); put the sun (`StrolleSun`) below the horizon to light from the map alone.
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
@@ -57,6 +59,7 @@ pub struct StrolleSettings {
     pub light_grid: u32,
     pub texture_filter: bool,
     pub temporal_aa: bool,
+    pub environment_map: Option<st::EnvironmentMap>,
 }
 
 #[derive(Clone, Debug)]
@@ -102,6 +105,7 @@ impl Plugin for StrollePlugin {
         engine.set_light_grid(settings.light_grid).expect("strolle_b200: ST_OPT_LIGHT_GRID");
         engine.set_texture_filter(settings.texture_filter).expect("strolle_b200: ST_OPT_TEXTURE_FILTER");
         engine.set_temporal_aa(settings.temporal_aa).expect("strolle_b200: ST_OPT_TEMPORAL_AA");
+        sync::set_environment_map(&mut engine, settings.environment_map.as_ref());
         render_app.insert_resource(EngineResource(engine));
     }
 }

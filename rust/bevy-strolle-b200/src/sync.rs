@@ -48,6 +48,13 @@ struct Pending {
     cameras: Vec<PendingCamera>,
 }
 
+/// `StrolleSettings::environment_map`, handed to the engine once it exists; the map is uploaded by the first frame's `tick`.
+pub(crate) fn set_environment_map(engine: &mut st::Engine<EngineParams>, map: Option<&st::EnvironmentMap>) {
+    if let Err(err) = engine.set_environment_map(map) {
+        error!("strolle: {err}");
+    }
+}
+
 pub(crate) fn setup(render_app: &mut App) {
     render_app.insert_resource(Pending::default());
     render_app.add_systems(ExtractSchedule, (extract_assets, extract_instances, extract_lights, extract_cameras));

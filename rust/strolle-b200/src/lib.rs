@@ -226,6 +226,18 @@ impl Image {
     }
 }
 
+/// An equirectangular environment map of linear RGB that lights the scene in place of the procedural sky: `width` x `height`
+/// texels, row-major, row 0 the zenith (alpha ignored); with `rotation` 0 the centre column is seen looking down -Z.  The radiance is
+/// the bilinear blend times `intensity`.  See `st_set_environment_map` in include/strolle_b200.h.
+#[derive(Clone, Debug, PartialEq)]
+pub struct EnvironmentMap {
+    pub width: u32,
+    pub height: u32,
+    pub texels: Vec<[f32; 4]>,
+    pub intensity: f32,
+    pub rotation: f32,
+}
+
 /// `strolle::Sun` (`sun.rs:1-14`)
 #[derive(Clone, Copy, Debug, PartialEq)]
 pub struct Sun {
@@ -451,6 +463,23 @@ impl<P: Params> Engine<P> {
     /// over one device: row strips over several refuse to render while it is on.  Takes effect with the next frame's scene update.
     pub fn set_temporal_aa(&mut self, on: bool) -> Result<(), Error> {
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_TEMPORAL_AA, on as c_int) })
+    }
+
+    /// Lights the scene from an equirectangular environment map in place of the procedural sky (`st_set_environment_map`; `None`,
+    /// the default, keeps the reference's procedural sky).  The sun light still follows `update_sun`: to light from the map alone,
+    /// put the sun below the horizon.  Takes effect with the next frame's scene update.
+    pub fn set_environment_map(&mut self, map: Option<&EnvironmentMap>) -> Result<(), Error> {
+        match map {
+            None => check(unsafe { sys::st_multi_set_environment_map(self.raw, std::ptr::null(), 0, 0, 0.0, 0.0) }),
+            Some(m) => {
+                if m.texels.len() as u64 != m.width as u64 * m.height as u64 {
+                    return Err(Error { code: sys::ST_ERR_INVALID, message: "environment map: texels.len() != width * height".into() });
+                }
+                check(unsafe {
+                    sys::st_multi_set_environment_map(self.raw, m.texels.as_ptr() as *const f32, m.width, m.height, m.intensity, m.rotation)
+                })
+            }
+        }
     }
 
     /// Creates or updates a mesh (`lib.rs:161-164`).

@@ -492,6 +492,11 @@ struct st_engine {
     uint64_t texture_mip_builds = 0;
     // ST_OPT_TEMPORAL_AA: `temporal_aa` = the option, `taa_frame` = the option as st_tick took it for the frame's cameras and resolve
     bool temporal_aa = false, taa_frame = false; uint64_t taa_resolves = 0;
+    // st_set_environment_map: the map as last set (`envm_set`, the caller's texels in `h_envm`; `envm_dirty` = not yet taken by a
+    // tick), and as st_tick took it: `envm` points into d_envm, `envm_frame` = the frame's sky-evaluating kernels run their ENVM
+    // instantiation
+    std::vector<float4> h_envm; uint32_t envm_w = 0, envm_h = 0; float envm_intensity = 0.0f, envm_rotation = 0.0f;
+    bool envm_set = false, envm_dirty = false, envm_frame = false; EnvMapDev envm{}; DevMem d_envm; uint64_t envm_launches = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -982,6 +987,8 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     const LightGridDev lgd = e->lgrid;
     const bool tfon = e->texf_frame;   // filtered material textures (ST_OPT_TEXTURE_FILTER)
     const TexFilterDev tfd = e->texf;
+    const bool emon = e->envm_frame;   // the environment map in place of the procedural sky (st_set_environment_map)
+    const EnvMapDev emd = e->envm;
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
     auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
@@ -995,9 +1002,9 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         for (uint32_t depth = 0; depth <= (uint32_t)d.ref_depth; depth++) {
             uint32_t sd = seed(P_REF_SHADING_SEED + depth);
             add(P_REF_TRACING, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_ref_tracing(cam, sc, depth, nm, s); });
-            add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, sd, depth, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, s); });
+            add(P_REF_SHADING, [=](cudaStream_t s) { if (emon) e->envm_launches++; launch_ref_shading(cam, sc, sd, depth, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, emon ? &emd : nullptr, s); });
         }
-        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, nullptr, s); });
+        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, nullptr, nullptr, s); });
         add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, 6u, di_final, gi_final, s); });
         return;
     }
@@ -1024,7 +1031,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
                 add(P_DI_SPATIAL_TRACE, [=](cudaStream_t s) { (fs ? stf::launch_spatial_trace : st::launch_spatial_trace)(cam, sc, cam.di_diff_samples, cam.di_diff_curr_colors, cam.di_diff_stash, s); });
                 add(P_DI_SPATIAL_SAMPLE, [=](cudaStream_t s) { (fs ? stf::launch_di_spatial_sample : st::launch_di_spatial_sample)(cam, sc, s5, f, s); });
             }
-            add(P_DI_RESOLVING, [=](cudaStream_t s) { (fs ? stf::launch_di_resolving : st::launch_di_resolving)(cam, sc, cur, s); });
+            add(P_DI_RESOLVING, [=](cudaStream_t s) { if (emon) e->envm_launches++; (fs ? stf::launch_di_resolving : st::launch_di_resolving)(cam, sc, cur, emon ? &emd : nullptr, s); });
         }
         if (needs_gi) {
             uint32_t sa = seed(P_GI_SAMPLING_A), sb = seed(P_GI_SAMPLING_B), st_ = seed(P_GI_TEMPORAL), sp = seed(P_GI_SPATIAL_PICK), ss = seed(P_GI_SPATIAL_SAMPLE), sv = seed(P_GI_PREVIEW);
@@ -1033,9 +1040,16 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
             const int inline_rp = (fp && tracing) ? 1 : 0;   // K11 inside K14; validation frames keep K11 (K12 / K13 read its output)
             if (!inline_rp) add(P_GI_REPROJECTION, [=](cudaStream_t s) { (fs ? stf::launch_gi_reprojection : st::launch_gi_reprojection)(cam, sc, cur, s); });
             auto sampling = [&]() {
-                if (fp) { add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, nm, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, s); }); return; }
+                if (fp) {
+                    add(P_GI_SAMPLING_B, [=](cudaStream_t s) {
+                        if (nm) e->normal_map_launches++;
+                        if (emon) e->envm_launches++;
+                        (fs ? stf::launch_gi_sampling_fused : st::launch_gi_sampling_fused)(cam, sc, cur, sa, sb, f, nm, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, emon ? &emd : nullptr, s);
+                    });
+                    return;
+                }
                 add(P_GI_SAMPLING_A, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, nm, tfon ? &tfd : nullptr, s); });
-                add(P_GI_SAMPLING_B, [=](cudaStream_t s) { (fs ? stf::launch_gi_sampling_b : st::launch_gi_sampling_b)(cam, sc, cur, sb, f, lgon ? &lgd : nullptr, s); });
+                add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (emon) e->envm_launches++; (fs ? stf::launch_gi_sampling_b : st::launch_gi_sampling_b)(cam, sc, cur, sb, f, lgon ? &lgd : nullptr, emon ? &emd : nullptr, s); });
             };
             if (tracing) {
                 if (f % 2u == 0u) sampling();
@@ -1480,7 +1494,7 @@ void st_engine_destroy(st_engine* e) {
     if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
     for (CameraSlot* c : e->cameras) { for (int k = 0; k < 2; k++) { if (c->side[k]) { cudaStreamSynchronize(c->side[k]); cudaStreamDestroy(c->side[k]); } if (c->ev_pushed[k]) cudaEventDestroy(c->ev_pushed[k]); } if (c->ev_produced) cudaEventDestroy(c->ev_produced);
         c->arena.release(); c->svgf_pairs.release(); c->rgba8.release(); for (int k = 0; k < 2; k++) { if (c->ev_ready[k]) cudaEventDestroy(c->ev_ready[k]); if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]); } delete c; }
-    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake, &e->d_lgrid, &e->d_texf_pool, &e->d_texf_table, &e->d_texf_jobs};
+    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake, &e->d_lgrid, &e->d_texf_pool, &e->d_texf_table, &e->d_texf_jobs, &e->d_envm};
     for (DevMem* d : all) d->release();
     for (auto& m : e->d_meshes) m.second.release();
     for (int k = 0; k < 2; k++) { if (e->staging[k]) cudaFreeHost(e->staging[k]); if (e->staging_ev[k]) cudaEventDestroy(e->staging_ev[k]); }
@@ -1803,6 +1817,17 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
         e->texf_built = false;
     } else if (textures_changed || !e->texf_built) { if ((rc = build_texture_mips(e))) return rc; }
     e->texf_frame = e->texture_filter && e->any_color_texture;
+    // st_set_environment_map: the map set since the last tick goes up now; a cleared map's device copy is freed
+    if (e->envm_dirty) {
+        e->envm_dirty = false;
+        if (e->envm_set) {
+            const size_t bytes = e->h_envm.size() * sizeof(float4);
+            if ((rc = upload(e, e->d_envm, e->h_envm.data(), bytes))) return rc;
+            e->envm.texels = (const float4*)e->d_envm.p; e->envm.w = e->envm_w; e->envm.h = e->envm_h;
+            e->envm.intensity = e->envm_intensity; e->envm.rotation = e->envm_rotation;
+        } else { e->d_envm.release(); e->envm = EnvMapDev{}; }
+    }
+    e->envm_frame = e->envm_set;
     // ST_OPT_TEMPORAL_AA: the history exists only while the option is on, and starts over when it turns on
     if (e->temporal_aa != e->taa_frame) for (CameraSlot* c : e->cameras) { c->taa.release(); c->taa_hist[0] = c->taa_hist[1] = nullptr; }
     e->taa_frame = e->temporal_aa;
@@ -1941,6 +1966,21 @@ int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap, size_t
         if (dst) std::memcpy(dst, w.data(), 4 * std::min(cap, w.size()));
         return ST_OK;
     }
+    if (s == "environment_map") {   // {W, H, intensity bits, rotation bits}, then the texels (include/strolle_b200.h)
+        if (!e->envm_frame) return fail(ST_ERR_NOT_FOUND, "no environment map: none is set or no st_tick has taken it");
+        const size_t texels = (size_t)e->envm.w * e->envm.h;
+        *count = 4 + 4 * texels;
+        if (dst) {
+            uint32_t head[4] = {e->envm.w, e->envm.h, 0u, 0u};
+            std::memcpy(head + 2, &e->envm.intensity, 4); std::memcpy(head + 3, &e->envm.rotation, 4);
+            std::memcpy(dst, head, 4 * std::min<size_t>(cap, 4));
+            if (cap > 4) {
+                CK(cudaStreamSynchronize(e->stream));
+                CK(cudaMemcpy(dst + 4, e->envm.texels, 4 * std::min(cap - 4, 4 * texels), cudaMemcpyDeviceToHost));
+            }
+        }
+        return ST_OK;
+    }
     if (s == "texture_mips") {   // {pool texels, materials}, the table, the pool (include/strolle_b200.h)
         if (!e->texf_built) return fail(ST_ERR_NOT_FOUND, "no mip chains: ST_OPT_TEXTURE_FILTER is off or no st_tick has built them");
         std::vector<uint32_t> w = {(uint32_t)e->texf_pool_texels, (uint32_t)e->h_materials.size()};
@@ -1994,6 +2034,33 @@ static int trace_stream(st_engine* e, const float* rays, size_t n, void* out, bo
 int st_trace_closest(st_engine* e, const float* rays, size_t n, float* out, float* ms) { return trace_stream(e, rays, n, out, true, ms); }
 int st_trace_any(st_engine* e, const float* rays, size_t n, uint32_t* out, float* ms) { return trace_stream(e, rays, n, out, false, ms); }
 
+// The map is validated whole before anything changes; rotation is reduced into [0, 2 pi) in double, then rounded to f32.
+int st_set_environment_map(st_engine* e, const float* rgba32f, uint32_t width, uint32_t height, float intensity, float rotation) {
+    if (!e) return fail(ST_ERR_INVALID, "null engine");
+    if (!rgba32f) {
+        if (e->envm_set) { e->envm_set = false; e->envm_dirty = true; std::vector<float4>().swap(e->h_envm); }
+        return ST_OK;
+    }
+    if (width < 1u || width > 16384u || height < 1u || height > 16384u) return fail(ST_ERR_INVALID, "environment map: each side must be 1..16384");
+    if (!std::isfinite(intensity) || intensity < 0.0f) return fail(ST_ERR_INVALID, "environment map: the intensity must be finite and >= 0");
+    if (!std::isfinite(rotation)) return fail(ST_ERR_INVALID, "environment map: the rotation must be finite");
+    const size_t n = (size_t)width * height;
+    for (size_t i = 0; i < n; i++)
+        for (int c = 0; c < 3; c++) {
+            const float v = rgba32f[4 * i + c];
+            if (!std::isfinite(v) || v < 0.0f) return fail(ST_ERR_INVALID, "environment map: every RGB value must be finite and >= 0");
+        }
+    const double two_pi = 6.283185307179586476925286766559;
+    double r = std::fmod((double)rotation, two_pi);
+    if (r < 0.0) r += two_pi;
+    if (r >= two_pi) r = 0.0;
+    e->h_envm.resize(n);
+    std::memcpy(e->h_envm.data(), rgba32f, n * sizeof(float4));
+    e->envm_w = width; e->envm_h = height; e->envm_intensity = intensity; e->envm_rotation = (float)r;
+    e->envm_set = true; e->envm_dirty = true;
+    return ST_OK;
+}
+
 int st_device_math(st_engine* e, int op, const float* a, const float* b, float* out, size_t n) {
     if (!e || !a || !out) return fail(ST_ERR_INVALID, "null argument");
     if (n == 0) return ST_OK;   // nothing to evaluate (a zero-block grid would be a launch error)
@@ -2002,7 +2069,7 @@ int st_device_math(st_engine* e, int op, const float* a, const float* b, float* 
     if ((rc = da.ensure(n * 4)) || (rc = db.ensure(n * 4)) || (rc = dc.ensure(n * 4))) return rc;
     CK(cudaMemcpyAsync(da.p, a, n * 4, cudaMemcpyHostToDevice, e->stream));
     if (b) CK(cudaMemcpyAsync(db.p, b, n * 4, cudaMemcpyHostToDevice, e->stream));
-    // op 0-6: the strict elementary functions, op 7: the texture filter's log2; op 16-23: the fast-shading build's sin, cos, exp, pow, sqrt, division, acos and atan2
+    // op 0-6: the strict elementary functions, op 7: the texture filter's log2, ops 8 and 9: the environment map's acos and atan2; op 16-23: the fast-shading build's sin, cos, exp, pow, sqrt, division, acos and atan2
     if (op >= 16) stf::launch_math_shading(op - 16, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
     else launch_math(op, (const float*)da.p, (const float*)db.p, (float*)dc.p, (long)n, e->stream);
     CK(cudaMemcpyAsync(out, dc.p, n * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -2085,6 +2152,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_LIGHT_GRID_BUILDS) { *value = e->light_grid_builds; return ST_OK; }
     if (stat == ST_STAT_TEXTURE_MIP_BUILDS) { *value = e->texture_mip_builds; return ST_OK; }
     if (stat == ST_STAT_TAA_RESOLVES) { *value = e->taa_resolves; return ST_OK; }
+    if (stat == ST_STAT_ENVIRONMENT_MAP_LAUNCHES) { *value = e->envm_launches; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
         CK(cudaSetDevice(e->device)); CK(cudaStreamSynchronize(e->stream));
         uint64_t total = 0;
@@ -2467,6 +2535,9 @@ int st_multi_remove_instance(st_multi* m, st_handle h) { ST_MULTI_ALL(st_remove_
 int st_multi_insert_light(st_multi* m, st_handle h, const st_light* l) { ST_MULTI_ALL(st_insert_light(e, h, l)); }
 int st_multi_remove_light(st_multi* m, st_handle h) { ST_MULTI_ALL(st_remove_light(e, h)); }
 int st_multi_update_sun(st_multi* m, float az, float alt) { ST_MULTI_ALL(st_update_sun(e, az, alt)); }
+int st_multi_set_environment_map(st_multi* m, const float* rgba32f, uint32_t width, uint32_t height, float intensity, float rotation) {
+    ST_MULTI_ALL(st_set_environment_map(e, rgba32f, width, height, intensity, rotation));
+}
 int st_multi_set_option(st_multi* m, int option, int value) { ST_MULTI_ALL(st_set_option(e, option, value)); }
 int st_multi_set_seed_base(st_multi* m, uint32_t base) { ST_MULTI_ALL(st_set_seed_base(e, base)); }
 int st_multi_set_blue_noise(st_multi* m, const uint8_t* rgba) { ST_MULTI_ALL(st_set_blue_noise(e, rgba)); }

@@ -454,8 +454,9 @@ __global__ void ST_LB_DI_SPATIAL_PICK k_di_spatial_fused(KPARAMS, int cur, u32 s
     di_spatial_sample_pair(cam, seed_sample, frame, g, d2a, d2b);
 }
 
-// K10 di_resolving::main (di_resolving.rs:4-119)
-__global__ void ST_LB_DI_RESOLVING k_di_resolving(KPARAMS, int cur) {
+// K10 di_resolving::main (di_resolving.rs:4-119); ENVM (st_set_environment_map, only while a map is set): sky pixels see the map
+template <bool ENVM>
+__global__ void ST_LB_DI_RESOLVING k_di_resolving(KPARAMS, int cur, const __grid_constant__ EnvMapDev em) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
@@ -473,7 +474,7 @@ __global__ void ST_LB_DI_RESOLVING k_di_resolving(KPARAMS, int cur) {
         else { rad = light_radiance(light_load(sc, res.light_id), hit); rad.radiance = rad.radiance * res.w; }
     } else {
         confidence = 1.0f;
-        rad.radiance = atmosphere_sample(sc, world_sun_dir(sc.world), hit.dir);
+        rad.radiance = sky_radiance<ENVM>(sc, em, world_sun_dir(sc.world), hit.dir);
         rad.diff = f3s(1.0f); rad.spec = f3s(0.0f);
     }
     float diff_brdf = (1.0f - hit.g.metallic) / kPi;
@@ -565,9 +566,11 @@ __global__ void ST_LB_GI_SAMPLING_A k_gi_sampling_a(KPARAMS, int cur, u32 seed, 
 }
 
 // K13 gi_sampling_b::main (gi_sampling_b.rs:4-235); LGRID: the light candidates come from the light grid's list for the bounce hit
-// (the sky-or-light draw still tests the global light count, so the RNG sequence keeps its shape)
-template <bool LGRID>
-ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4 d0, float4 d1, float4 d2, const LightGridDev& lg) {
+// (the sky-or-light draw still tests the global light count, so the RNG sequence keeps its shape); ENVM: the missed bounce and the sky
+// draw see the map, and the sky draw's probability is 0.25 whatever the sun's altitude (the map does not darken with the sun)
+template <bool LGRID, bool ENVM>
+ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4 d0, float4 d1, float4 d2, const LightGridDev& lg,
+                               const EnvMapDev& em) {
     bool tracing = gi_tracing_frame(frame);
     uint2 sp = tracing ? checker(g.x, g.y, frame / 2u) : checker(g.x, g.y, frame);
     if (!cam_contains_u(cam.curr, sp.x, sp.y)) return;
@@ -590,13 +593,13 @@ ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const T
     const u32 SKY = 0xffffffffu;
     float3 sun_dir = world_sun_dir(sc.world);
     u32 light_id; float light_pdf; float3 light_rad; float3 light_dir = f3s(0.f);
-    if (!hit_some(gh)) { light_id = SKY; light_pdf = 1.0f; light_rad = atmosphere_sample(sc, sun_dir, gh.dir); }
+    if (!hit_some(gh)) { light_id = SKY; light_pdf = 1.0f; light_rad = sky_radiance<ENVM>(sc, em, sun_dir, gh.dir); }
     else {
-        float atm_pdf = (sc.world.sun_altitude <= -1.0f) ? 0.0f : 0.25f;
+        float atm_pdf = (!ENVM && sc.world.sun_altitude <= -1.0f) ? 0.0f : 0.25f;
         if (sc.world.light_count == 0u || rng_f(rng) < atm_pdf) {
             light_id = SKY; light_pdf = atm_pdf;
             light_dir = rng_hemisphere(rng, gh.g.normal);
-            light_rad = atmosphere_sample(sc, sun_dir, light_dir) * dot(gh.g.normal, light_dir);
+            light_rad = sky_radiance<ENVM>(sc, em, sun_dir, light_dir) * dot(gh.g.normal, light_dir);
         } else {
             EphRes er = LGRID ? ephemeral_build_list(rng, sc, gh, lgrid_list(lg, gh.point)) : ephemeral_build(rng, sc, gh);
             if (er.w > 0.0f) { light_id = er.light_id; light_pdf = (1.0f / er.w) * (1.0f - atm_pdf); light_rad = er.rad.radiance * (f3s(1.0f) + er.rad.spec); }
@@ -624,25 +627,25 @@ ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const T
     }
     gi_store(res, cam.gi_reservoirs[1], idx);
 }
-template <bool LGRID>
-__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ LightGridDev lg) {
+template <bool LGRID, bool ENVM>
+__global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ LightGridDev lg, const __grid_constant__ EnvMapDev em) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     size_t gi = pix(cam, g.x, g.y);
-    gi_sampling_b_pair<LGRID>(cam, sc, stk, cur, seed, frame, g, cam.gi_d0[gi], cam.gi_d1[gi], cam.gi_d2[gi], lg);
+    gi_sampling_b_pair<LGRID, ENVM>(cam, sc, stk, cur, seed, frame, g, cam.gi_d0[gi], cam.gi_d1[gi], cam.gi_d2[gi], lg, em);
 }
 // K12 + K13 in one launch (ST_OPT_FUSED_PASSES): the bounce ray is traced and shaded by the same thread; the hit still goes through
 // GBufferEntry's pack / unpack (its 8-bit quantisation is part of the result), just not through memory.
-template <bool NMAP, bool LGRID, bool TEXF>
+template <bool NMAP, bool LGRID, bool TEXF, bool ENVM>
 __global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_fused(KPARAMS, int cur, u32 seed_a, u32 seed_b, u32 frame, const __grid_constant__ LightGridDev lg,
-                                                        const __grid_constant__ TexFilterDev tf) {
+                                                        const __grid_constant__ TexFilterDev tf, const __grid_constant__ EnvMapDev em) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
     if (!gi_sampling_a_pair<NMAP, TEXF>(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2, tf)) return;
-    gi_sampling_b_pair<LGRID>(cam, sc, stk, cur, seed_b, frame, g, t0, t1, t2, lg);
+    gi_sampling_b_pair<LGRID, ENVM>(cam, sc, stk, cur, seed_b, frame, g, t0, t1, t2, lg, em);
 }
 
 // K14 gi_temporal_resampling::main (gi_temporal_resampling.rs:4-156)
@@ -1396,10 +1399,10 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
 
 // K2 ref_shading::main (ref_shading.rs:4-177); LGRID: the one light is drawn from the light grid's list for the nudged hit point
 // TEXF: the hit's textures are filtered; the packed hit carries no triangle, so the segment's ray is traced again (same ray, same
-// BVH: the same triangle and distance)
-template <bool LGRID, bool TEXF>
+// BVH: the same triangle and distance); ENVM: a path that leaves the scene sees the map
+template <bool LGRID, bool TEXF, bool ENVM>
 __global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32 depth, const __grid_constant__ LightGridDev lg,
-                                                          const __grid_constant__ TexFilterDev tf) {
+                                                          const __grid_constant__ TexFilterDev tf, const __grid_constant__ EnvMapDev em) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
@@ -1421,7 +1424,7 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32
     }
     TriHit th = trihit_unpack(cam.ref_hits[2 * idx], cam.ref_hits[2 * idx + 1]);
     if (!trihit_some(th)) {
-        color = color + thr * atmosphere_sample(sc, world_sun_dir(sc.world), ray.d);
+        color = color + thr * sky_radiance<ENVM>(sc, em, world_sun_dir(sc.world), ray.d);
         rays[3 * idx] = f4zero(); rays[3 * idx + 1] = f4zero(); rays[3 * idx + 2] = f4(color, 0.0f);
         return;
     }
@@ -1515,6 +1518,11 @@ __global__ void k_math(int op, const float* __restrict__ a, const float* __restr
 __global__ void k_math_log2(const float* __restrict__ a, float* __restrict__ out, long n) {
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = log2_x(a[i]);
+}
+// st_device_math ops 8 and 9: the environment map's acos and atan2(a, b)
+__global__ void k_math_envm(int op, const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out, long n) {
+    long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = op == 8 ? acos_x(a[i]) : atan2_x(a[i], b[i]);
 }
 
 // ST_OPT_TEXTURE_FILTER: level k+1 of the images of `jobs` (blockIdx.y) from their level k, one thread per output texel.  Texel (x, y)
@@ -1787,7 +1795,9 @@ void launch_di_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed
 void launch_di_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_pick, c, st, c, s, cur, seed, frame); }
 void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d0, const float4* d1, float4* d2, cudaStream_t st) { k_spatial_trace<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, d0, d1, d2); }
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_sample, c, st, c, s, seed, frame); }
-void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_di_resolving<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
+void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, const EnvMapDev* em, cudaStream_t st) {
+    if (em) k_di_resolving<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, *em); else k_di_resolving<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, EnvMapDev{});
+}
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_gi_reprojection<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
 void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st) {
     if (tf) {
@@ -1797,8 +1807,15 @@ void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 se
         if (nmap) HALF_LAUNCH((k_gi_sampling_a<true, false>), c, st, c, s, cur, seed, frame, none); else HALF_LAUNCH((k_gi_sampling_a<false, false>), c, st, c, s, cur, seed, frame, none);
     }
 }
-void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st) {
-    if (lg) HALF_LAUNCH(k_gi_sampling_b<true>, c, st, c, s, cur, seed, frame, *lg); else HALF_LAUNCH(k_gi_sampling_b<false>, c, st, c, s, cur, seed, frame, LightGridDev{});
+void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, const EnvMapDev* em, cudaStream_t st) {
+    const LightGridDev none{};
+    const LightGridDev& g = lg ? *lg : none;
+    const EnvMapDev enone{};
+    const EnvMapDev& m = em ? *em : enone;
+#define ST_GSB(L_, E_) HALF_LAUNCH((k_gi_sampling_b<L_, E_>), c, st, c, s, cur, seed, frame, g, m)
+    if (em) { if (lg) ST_GSB(true, true); else ST_GSB(false, true); }
+    else { if (lg) ST_GSB(true, false); else ST_GSB(false, false); }
+#undef ST_GSB
 }
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st) { k_gi_temporal<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, frame, inline_reprojection); }
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_pick, c, st, c, s, cur, seed, frame); }
@@ -1811,19 +1828,23 @@ void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u
 }
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_di_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
 void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf,
-                              cudaStream_t st) {
+                              const EnvMapDev* em, cudaStream_t st) {
     const LightGridDev none{};
     const LightGridDev& g = lg ? *lg : none;
     const TexFilterDev tnone{};
     const TexFilterDev& t = tf ? *tf : tnone;
-#define ST_GSF(N_, L_, T_) HALF_LAUNCH((k_gi_sampling_fused<N_, L_, T_>), c, st, c, s, cur, seed_a, seed_b, frame, g, t)
+    const EnvMapDev enone{};
+    const EnvMapDev& m = em ? *em : enone;
+#define ST_GSF(N_, L_, T_, E_) HALF_LAUNCH((k_gi_sampling_fused<N_, L_, T_, E_>), c, st, c, s, cur, seed_a, seed_b, frame, g, t, m)
+#define ST_GSF_E(N_, L_, T_) do { if (em) ST_GSF(N_, L_, T_, true); else ST_GSF(N_, L_, T_, false); } while (0)
     if (tf) {
-        if (lg) { if (nmap) ST_GSF(true, true, true); else ST_GSF(false, true, true); }
-        else { if (nmap) ST_GSF(true, false, true); else ST_GSF(false, false, true); }
+        if (lg) { if (nmap) ST_GSF_E(true, true, true); else ST_GSF_E(false, true, true); }
+        else { if (nmap) ST_GSF_E(true, false, true); else ST_GSF_E(false, false, true); }
     } else {
-        if (lg) { if (nmap) ST_GSF(true, true, false); else ST_GSF(false, true, false); }
-        else { if (nmap) ST_GSF(true, false, false); else ST_GSF(false, false, false); }
+        if (lg) { if (nmap) ST_GSF_E(true, true, false); else ST_GSF_E(false, true, false); }
+        else { if (nmap) ST_GSF_E(true, false, false); else ST_GSF_E(false, false, false); }
     }
+#undef ST_GSF_E
 #undef ST_GSF
 }
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st) { HALF_LAUNCH(k_gi_spatial_fused, c, st, c, s, cur, seed_pick, seed_sample, frame); }
@@ -2046,14 +2067,22 @@ void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cud
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {
     if (nmap) k_ref_tracing<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); else k_ref_tracing<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth);
 }
-void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st) {
+void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, const EnvMapDev* em,
+                        cudaStream_t st) {
     const LightGridDev none{};
     const LightGridDev& g = lg ? *lg : none;
     const TexFilterDev tnone{};
     const TexFilterDev& t = tf ? *tf : tnone;
-#define ST_RS(L_, T_) k_ref_shading<L_, T_><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, g, t)
-    if (tf) { if (lg) ST_RS(true, true); else ST_RS(false, true); }
-    else { if (lg) ST_RS(true, false); else ST_RS(false, false); }
+    const EnvMapDev enone{};
+    const EnvMapDev& m = em ? *em : enone;
+#define ST_RS(L_, T_, E_) k_ref_shading<L_, T_, E_><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, g, t, m)
+    if (em) {
+        if (tf) { if (lg) ST_RS(true, true, true); else ST_RS(false, true, true); }
+        else { if (lg) ST_RS(true, false, true); else ST_RS(false, false, true); }
+    } else {
+        if (tf) { if (lg) ST_RS(true, true, false); else ST_RS(false, true, false); }
+        else { if (lg) ST_RS(true, false, false); else ST_RS(false, false, false); }
+    }
 #undef ST_RS
 }
 // ST_OPT_TEXTURE_FILTER: one launch per level (split into launches of at most 65535 images, the grid's y limit), `first[k]` ..
@@ -2075,7 +2104,9 @@ void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st) 
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st) { k_trace_stream_closest<<<(unsigned)((n + ST_BLOCK - 1) / ST_BLOCK), ST_BLOCK, 0, st>>>(s, rays, n, out); }
 void launch_trace_stream_any(const SceneDev& s, const float4* rays, long n, u32* out, cudaStream_t st) { k_trace_stream_any<<<(unsigned)((n + ST_BLOCK - 1) / ST_BLOCK), ST_BLOCK, 0, st>>>(s, rays, n, out); }
 void launch_math(int op, const float* a, const float* b, float* out, long n, cudaStream_t st) {
-    if (op == 7) k_math_log2<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, out, n); else k_math<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n);
+    if (op == 7) k_math_log2<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, out, n);
+    else if (op == 8 || op == 9) k_math_envm<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n);
+    else k_math<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n);
 }
 void launch_light_grid_build(const LightGridDev& lg, const GpuLight* lights, cudaStream_t st) {
     const u32 ncell = lg.dims[0] * lg.dims[1] * lg.dims[2];

@@ -7,7 +7,8 @@ namespace st {
 typedef uint32_t u32;
 
 // nmap: the NMAP instantiation (normal-mapped shading normal, ST_OPT_NORMAL_MAPS) of the kernels that shade a closest hit;
-// tf (non-null): their TEXF instantiation (filtered material textures, ST_OPT_TEXTURE_FILTER)
+// tf (non-null): their TEXF instantiation (filtered material textures, ST_OPT_TEXTURE_FILTER); em (non-null): the ENVM instantiation
+// of the kernels that evaluate the sky (K10, K13 and the fused K12 + K13, K2: the environment map of st_set_environment_map)
 void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, const TexFilterDev* tf, cudaStream_t st);
 void launch_frame_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
@@ -15,10 +16,10 @@ void launch_di_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed
 void launch_di_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
 void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d0, const float4* d1, float4* d2, cudaStream_t st);
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
-void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
+void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st);
-void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
+void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
 void launch_gi_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
@@ -26,7 +27,8 @@ void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed,
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st);
 void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st);
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf,
+                              const EnvMapDev* em, cudaStream_t st);
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st);
 void launch_denoise_reproject(const CameraDev& c, const SceneDev& s, int cur, const float4* pc, const float4* pm, const float4* smp, float4* col, float4* mom, cudaStream_t st);
@@ -42,7 +44,7 @@ void launch_taa_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 mode
                         float4 jit, cudaStream_t st);
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st);
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st);
-void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st);
+void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, const EnvMapDev* em, cudaStream_t st);
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st);
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st);
 void launch_trace_stream_any(const SceneDev& s, const float4* rays, long n, u32* out, cudaStream_t st);
@@ -108,17 +110,17 @@ void launch_refit(const uint4* runs, u32 nruns, const uint2* nodes, const u32* l
 // The ReSTIR kernels K5-K19 built a second time with FMA contraction and SFU approximations (kernels.cu compiled with
 // -DST_FAST=1, see st_math.cuh): same launch interface, selected by ST_OPT_SHADING_FAST_MATH.
 namespace stf {
-using st::CameraDev; using st::SceneDev; using st::LightGridDev; using st::TexFilterDev; using st::u32;
+using st::CameraDev; using st::SceneDev; using st::LightGridDev; using st::TexFilterDev; using st::EnvMapDev; using st::u32;
 int preload_kernels();   // the fast-shading build's kernels
 void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_di_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, cudaStream_t st);
 void launch_di_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
 void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d0, const float4* d1, float4* d2, cudaStream_t st);
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
-void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
+void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st);
-void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
+void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
 void launch_gi_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
@@ -126,7 +128,8 @@ void launch_gi_preview(const CameraDev& c, const SceneDev& s, int cur, u32 seed,
 void launch_gi_resolving(const CameraDev& c, const SceneDev& s, int cur, const float4* in, cudaStream_t st);
 void launch_di_sample_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed_sampling, u32 seed_temporal, u32 frame, const LightGridDev* lg, cudaStream_t st);
 void launch_di_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
-void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf, cudaStream_t st);
+void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_a, u32 seed_b, u32 frame, bool nmap, const LightGridDev* lg, const TexFilterDev* tf,
+                              const EnvMapDev* em, cudaStream_t st);
 void launch_gi_spatial_fused(const CameraDev& c, const SceneDev& s, int cur, u32 seed_pick, u32 seed_sample, u32 frame, cudaStream_t st);
 void launch_gi_preview_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 seed, const float4* in, const float4* source, cudaStream_t st);
 void launch_math_shading(int op, const float* a, const float* b, float* out, long n, cudaStream_t st);   // test hook: this build's sin/cos/exp/pow/sqrt/div

@@ -795,6 +795,73 @@ ST_DEV float3 atmosphere_sample(const SceneDev& sc, float3 sun_dir, float3 ray_d
     return lum;
 }
 
+// ---- Environment map (st_set_environment_map; DESIGN.md §2 "Environment map") --------------------------------------------------
+// The lookup uses the x*() primitives only, so the sky it gives is the same in the strict and the fast-shading builds.
+// acos_det / atan2_det's Cephes kernels through the x*() primitives (st_device_math ops 8 and 9)
+ST_DEV float asin_core_x(float x) {
+    const float z = xmul(x, x);
+    float p = 4.2163199048e-2f;
+    p = xadd(xmul(p, z), 2.4181311049e-2f); p = xadd(xmul(p, z), 4.5470025998e-2f); p = xadd(xmul(p, z), 7.4953002686e-2f);
+    p = xadd(xmul(p, z), 1.6666752422e-1f);
+    return xadd(xmul(xmul(p, z), x), x);
+}
+ST_DEV float acos_x(float x) {
+    if (!(x == x)) return x;
+    if (x < -1.0f || x > 1.0f) return fnan();
+    if (x > 0.5f) return xmul(2.0f, asin_core_x(xsqrt(xmul(0.5f, xsub(1.0f, x)))));
+    if (x < -0.5f) return xsub(kPi, xmul(2.0f, asin_core_x(xsqrt(xmul(0.5f, xadd(1.0f, x))))));
+    if (x >= 0.0f) return xsub(kHalfPi, asin_core_x(x));
+    return xadd(kHalfPi, asin_core_x(-x));
+}
+ST_DEV float atan_core_x(float x) {   // x >= 0
+    float y;
+    if (x > 2.414213562373095f) { y = kHalfPi; x = -xdiv(1.0f, x); }
+    else if (x > 0.4142135623730950f) { y = 0.7853981633974483f; x = xdiv(xsub(x, 1.0f), xadd(x, 1.0f)); }
+    else y = 0.0f;
+    const float z = xmul(x, x);
+    float p = 8.05374449538e-2f;
+    p = xsub(xmul(p, z), 1.38776856032e-1f); p = xadd(xmul(p, z), 1.99777106478e-1f); p = xsub(xmul(p, z), 3.33329491539e-1f);
+    return xadd(y, xadd(xmul(xmul(p, z), x), x));
+}
+ST_DEV float atan2_x(float y, float x) {
+    if (!(x == x) || !(y == y)) return fnan();
+    if (y == 0.0f) {
+        if (x > 0.0f || (x == 0.0f && !(fbits(x) >> 31))) return y;
+        return cpsign(kPi, y);
+    }
+    if (x == 0.0f) return cpsign(kHalfPi, y);
+    float a = atan_core_x(xdiv(fabs_(y), fabs_(x)));
+    if (x < 0.0f) a = xsub(kPi, a);
+    return cpsign(a, y);
+}
+// The map's radiance along d (as the pass has it, not renormalised): theta = acos(d.y), phi = atan2(d.x, -d.z); u = (phi + rotation)
+// / 2 pi + 0.5, v = theta / pi; columns floor(u W - 0.5) and the next, wrapped modulo W, rows floor(v H - 0.5) and the next, clamped;
+// blended as lut_fetch blends, times the intensity.  A non-finite u or v gives 0.
+ST_DEV float3 env_sample(const EnvMapDev& em, float3 d) {
+    const float theta = acos_x(rclamp(d.y, -1.0f, 1.0f)), phi = atan2_x(d.x, -d.z);
+    const float u = xadd(xmul(xadd(phi, em.rotation), 0.15915494309189535f), 0.5f), v = xmul(theta, 0.3183098861837907f);
+    if (!(fabs_(u) < finf()) || !(fabs_(v) < finf())) return f3s(0.0f);
+    const float s = xsub(xmul(u, (float)em.w), 0.5f), t = xsub(xmul(v, (float)em.h), 0.5f);
+    const float sx = floorf(s), sy = floorf(t);
+    const float tx = xsub(s, sx), ty = xsub(t, sy);
+    const int W = (int)em.w, H = (int)em.h;
+    int x0 = to_i32_sat(sx) % W; if (x0 < 0) x0 += W;
+    const int x1 = x0 + 1 == W ? 0 : x0 + 1;
+    const int iy = to_i32_sat(sy);
+    const int y0 = max(0, min(iy, H - 1)), y1 = max(0, min(iy + 1, H - 1));
+    const float3 a = xyz(ldg4(em.texels + (size_t)y0 * W + x0)), b = xyz(ldg4(em.texels + (size_t)y0 * W + x1));
+    const float3 c = xyz(ldg4(em.texels + (size_t)y1 * W + x0)), e = xyz(ldg4(em.texels + (size_t)y1 * W + x1));
+    const float3 top = f3(xadd(a.x, xmul(xsub(b.x, a.x), tx)), xadd(a.y, xmul(xsub(b.y, a.y), tx)), xadd(a.z, xmul(xsub(b.z, a.z), tx)));
+    const float3 bot = f3(xadd(c.x, xmul(xsub(e.x, c.x), tx)), xadd(c.y, xmul(xsub(e.y, c.y), tx)), xadd(c.z, xmul(xsub(e.z, c.z), tx)));
+    const float3 r = f3(xadd(top.x, xmul(xsub(bot.x, top.x), ty)), xadd(top.y, xmul(xsub(bot.y, top.y), ty)), xadd(top.z, xmul(xsub(bot.z, top.z), ty)));
+    return xscale(r, em.intensity);
+}
+// The sky radiance along `dir` at the four sites that evaluate it: the map when the ENVM instantiation runs, else atmosphere_sample
+template <bool ENVM>
+ST_DEV float3 sky_radiance(const SceneDev& sc, const EnvMapDev& em, float3 sun_dir, float3 dir) {
+    return ENVM ? env_sample(em, dir) : atmosphere_sample(sc, sun_dir, dir);
+}
+
 // ---- Reservoirs (reservoir.rs, reservoir/{di,gi,ephemeral,mis}.rs) ------------------------------------------
 struct DiRes { float m, w; float pdf, confidence; u32 light_id; float3 light_point; bool occluded; };
 ST_DEV DiRes di_zero() { DiRes r; r.m = 0.f; r.w = 0.f; r.pdf = 0.f; r.confidence = 0.f; r.light_id = 0u; r.light_point = f3s(0.f); r.occluded = false; return r; }

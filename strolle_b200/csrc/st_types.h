@@ -76,6 +76,15 @@ struct TexFilterDev {
 // texels apart from `src`, in the atlas for k = 0, else in the pool)
 struct MipJob { uint32_t src, src_stride, src_w, src_h, dst, dst_w, dst_h, from_atlas; };
 
+// st_set_environment_map (DESIGN.md §2 "Environment map"): an equirectangular map of linear RGB in place of the procedural sky.
+// Uploaded by st_set_environment_map, taken at st_tick; passed by value to the ENVM instantiations of the sky-evaluating kernels only.
+struct EnvMapDev {
+    const float4* texels;   // w x h, row-major, row 0 the zenith; alpha unused
+    uint32_t w, h;
+    float intensity;        // radiance scale
+    float rotation;         // radians in [0, 2 pi), added to the azimuth
+};
+
 // Per-camera device buffers: the logical buffers of
 // strolle/src/camera_controller/buffers.rs:53-339 as linear row-major float4
 // arrays indexed by full-frame coordinates (each GPU of a strip-partitioned run

@@ -43,6 +43,7 @@ STAT_BVH_REFITS = 9            # refit ticks (OPT_BVH_REFIT) since the engine wa
 STAT_LIGHT_GRID_BUILDS = 10    # light grid builds (OPT_LIGHT_GRID) since the engine was created
 STAT_TEXTURE_MIP_BUILDS = 11   # mip-chain builds (OPT_TEXTURE_FILTER) since the engine was created
 STAT_TAA_RESOLVES = 12         # temporal resolve launches (OPT_TEMPORAL_AA) since the engine was created
+STAT_ENVIRONMENT_MAP_LAUNCHES = 13   # launches of the environment-mapped kernel variants (set_environment_map) since creation
 
 
 class StrolleError(RuntimeError):
@@ -97,6 +98,7 @@ def load_library():
         "st_insert_image": [P, u64, C.c_void_p, u32, u32], "st_remove_image": [P, u64], "st_set_material_textures": [P, u64, C.POINTER(_MaterialTextures)],
         "st_insert_instance": [P, u64, u64, u64, f32p], "st_remove_instance": [P, u64],
         "st_insert_light": [P, u64, C.POINTER(_Light)], "st_remove_light": [P, u64], "st_update_sun": [P, C.c_float, C.c_float],
+        "st_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float],
         "st_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_update_camera": [P, i32, C.POINTER(_Camera)], "st_delete_camera": [P, i32],
         "st_tick": [P], "st_render_camera": [P, i32, P, C.c_int], "st_copy_output": [P, i32, P, C.c_int], "st_synchronize": [P],
         "st_set_seed_base": [P, u32], "st_set_blue_noise": [P, C.c_void_p],
@@ -126,6 +128,7 @@ def load_library():
         "st_multi_insert_image": [P, u64, C.c_void_p, u32, u32], "st_multi_remove_image": [P, u64], "st_multi_set_material_textures": [P, u64, C.POINTER(_MaterialTextures)],
         "st_multi_insert_instance": [P, u64, u64, u64, f32p], "st_multi_remove_instance": [P, u64],
         "st_multi_insert_light": [P, u64, C.POINTER(_Light)], "st_multi_remove_light": [P, u64], "st_multi_update_sun": [P, C.c_float, C.c_float],
+        "st_multi_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float],
         "st_multi_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_multi_update_camera": [P, i32, C.POINTER(_Camera)], "st_multi_delete_camera": [P, i32],
         "st_multi_tick": [P], "st_multi_render_camera": [P, i32, P, C.c_int], "st_multi_synchronize": [P],
         "st_multi_set_option": [P, C.c_int, C.c_int], "st_multi_set_seed_base": [P, u32], "st_multi_set_blue_noise": [P, C.c_void_p],
@@ -222,6 +225,18 @@ class BvhBuilder:
             pass
 
 
+def _envmap_texels(rgba):
+    """An H x W x 3 or H x W x 4 map as the contiguous H x W x 4 float32 texels st_set_environment_map takes (None stays None)."""
+    if rgba is None:
+        return None
+    a = np.asarray(rgba, dtype=np.float32)
+    if a.ndim != 3 or a.shape[2] not in (3, 4):
+        raise ValueError("environment map: an H x W x 3 or H x W x 4 array")
+    if a.shape[2] == 3:
+        a = np.concatenate([a, np.ones(a.shape[:2] + (1,), np.float32)], axis=2)
+    return np.ascontiguousarray(a)
+
+
 class Engine:
     """strolle::Engine on one GPU (CUDA device `device`)."""
 
@@ -300,6 +315,13 @@ class Engine:
 
     def update_sun(self, azimuth, altitude):
         self._check(self.lib.st_update_sun(self._h, azimuth, altitude))
+
+    def set_environment_map(self, rgba=None, intensity=1.0, rotation=0.0):
+        """Lights the scene from an equirectangular map (H x W x 4 or H x W x 3 linear RGB, row 0 the zenith) in place of the
+        procedural sky, from the next tick; None clears it (include/strolle_b200.h st_set_environment_map)."""
+        t = _envmap_texels(rgba)
+        w, h = (0, 0) if t is None else (t.shape[1], t.shape[0])
+        self._check(self.lib.st_set_environment_map(self._h, None if t is None else t.ctypes.data, w, h, intensity, rotation))
 
     # ---- cameras ----------------------------------------------------------------------------
     @staticmethod
@@ -399,7 +421,7 @@ class Engine:
                # the fast-shading build's forms (ST_OPT_SHADING_FAST_MATH): SFU sin / cos / exp / pow, sqrt.approx, div.full, and the
                # Cephes acos / atan2 compiled with FMA contraction, sqrt.approx and div.full
                "sin_fast": 16, "cos_fast": 17, "exp_fast": 18, "pow_fast": 19, "sqrt_fast": 20, "div_fast": 21, "acos_fast": 22,
-               "atan2_fast": 23}
+               "atan2_fast": 23, "acos_env": 8, "atan2_env": 9}
         a = _f(a)
         b = _f(b) if b is not None else np.zeros_like(a)
         out = np.empty_like(a)
@@ -562,6 +584,12 @@ class MultiEngine:
 
     def update_sun(self, azimuth, altitude):
         self._check(self.lib.st_multi_update_sun(self._h, azimuth, altitude))
+
+    def set_environment_map(self, rgba=None, intensity=1.0, rotation=0.0):
+        """Engine.set_environment_map on every member."""
+        t = _envmap_texels(rgba)
+        w, h = (0, 0) if t is None else (t.shape[1], t.shape[0])
+        self._check(self.lib.st_multi_set_environment_map(self._h, None if t is None else t.ctypes.data, w, h, intensity, rotation))
 
     def create_camera(self, mode, denoise, ref_depth, w, h, transform16, projection16):
         c = Engine._cam(mode, denoise, ref_depth, w, h, transform16, projection16)

@@ -624,6 +624,8 @@ def apply(engine, scene):
     for h, kind, params in scene["lights"]:
         engine.insert_light(h, kind, params)
     engine.update_sun(*scene["sun"])
+    if "environment_map" in scene:
+        engine.set_environment_map(**scene["environment_map"])
     c = scene["camera"]
     return engine.create_camera(c["mode"], c["denoise"], c["ref_depth"], c["w"], c["h"], c["transform"], c["projection"])
 
@@ -651,3 +653,56 @@ def aa_edges(width=96, height=64, mode=MODE_IMAGE, denoise=True, ref_depth=1):
     cam = dict(mode=mode, denoise=denoise, ref_depth=ref_depth, w=width, h=height, transform=look_at_transform((0.0, 0.0, 0.0), (0.0, 0.0, -1.0)),
                projection=perspective_infinite_reverse_rh(math.pi / 4.0, width / height, 0.1))
     return dict(name="aa_edges", meshes=meshes, materials=materials, instances=instances, lights=[], sun=(0.0, -1.0), camera=cam)
+
+
+def courtyard_sky(width=256, height=128, sun_disc=True):
+    """An equirectangular test sky (height x width x 4 linear RGB, row 0 the zenith), generated rather than loaded: a horizon gradient
+    (bright near the horizon, deep blue at the zenith, dark brown below), tinted by one colour per azimuth quadrant, and a small disc
+    of radiance ~50 (a firefly source, placed so that it straddles the u = 0 / 1 seam)."""
+    v = (np.arange(height, dtype=np.float64) + 0.5) / height
+    u = (np.arange(width, dtype=np.float64) + 0.5) / width
+    uu, vv = np.meshgrid(u, v)
+    alt = 0.5 - vv   # +0.5 at the zenith, -0.5 at the nadir (in units of pi)
+    sky = np.where(alt[..., None] >= 0, (1.0 - 2.0 * alt[..., None]) * np.array([1.1, 1.0, 0.9]) + 2.0 * alt[..., None] * np.array([0.15, 0.3, 0.9]),
+                   np.array([0.25, 0.18, 0.12]) * (1.0 + 2.0 * alt[..., None]))
+    quadrant = np.floor(uu * 4.0).astype(int) % 4
+    tint = np.array([[1.0, 0.85, 0.85], [0.85, 1.0, 0.85], [0.85, 0.85, 1.0], [1.0, 1.0, 0.8]])[quadrant]
+    rgb = sky * tint
+    if sun_disc:
+        # the disc: centred on the seam (u = 0), 20 degrees above the horizon, 4 degrees across
+        du = np.minimum(uu, 1.0 - uu) * 2.0 * math.pi
+        dv = (vv - (0.5 - 20.0 / 180.0)) * math.pi
+        rgb[(du * du + dv * dv) < math.radians(2.0) ** 2] = (50.0, 47.0, 42.0)
+    out = np.ones((height, width, 4), np.float32)
+    out[..., :3] = rgb
+    return out
+
+
+def env_courtyard_motion(t):
+    """Frame t's camera transform and moving-crate affine for env_courtyard: the camera orbits slowly, the crate slides."""
+    a = 0.05 * t
+    eye = (3.5 * math.sin(a), 1.4, 3.5 * math.cos(a))
+    crate = np.array([1, 0, 0, 0, 1, 0, 0, 0, 1, -0.8 + 0.07 * t, 0.0, 0.6], np.float32)
+    return look_at_transform(eye, (0.0, 0.8, 0.0)), crate
+
+
+def env_courtyard(width=320, height=180, mode=MODE_IMAGE, denoise=True, ref_depth=1):
+    """Exercises the environment map (st_set_environment_map): a ground plane and a few occluders (two walls, a pillar, a crate that
+    moves), open to the sky, lit by one dim point light and the map (`environment_map`: courtyard_sky at intensity 1.5).  The sun is
+    below the horizon (altitude -1.2): the map is the only sky light, and K13's sky-draw probability would be 0 without a map."""
+    materials = {130: (material((0.55, 0.5, 0.45, 1.0)), False), 131: (material((0.8, 0.75, 0.7, 1.0), perceptual_roughness=0.6), False),
+                 132: (material((0.3, 0.35, 0.5, 1.0), perceptual_roughness=0.3, metallic=0.8), False),
+                 133: (material((0.7, 0.4, 0.2, 1.0)), False)}
+    meshes = {230: np.stack(_quad((-20, 0, -20), (20, 0, -20), (20, 0, 20), (-20, 0, 20), (0, 1, 0))),
+              231: np.stack(_box((-2.5, 0.0, -2.2), (1.5, 1.8, -1.9))),
+              232: np.stack(_box((1.9, 0.0, -2.0), (2.2, 1.2, 1.0))),
+              233: np.stack(_box((-0.2, 0.0, -0.9), (0.2, 2.4, -0.5))),
+              234: np.stack(_box((-0.35, 0.0, -0.35), (0.35, 0.7, 0.35)))}
+    cam_xf, crate = env_courtyard_motion(0)
+    instances = [(330, 230, 130, IDENTITY_AFFINE), (331, 231, 131, IDENTITY_AFFINE), (332, 232, 131, IDENTITY_AFFINE),
+                 (333, 233, 132, IDENTITY_AFFINE), (334, 234, 133, crate)]
+    lights = [(430, LIGHT_POINT, point_light((-1.0, 2.0, 1.0), 0.1, (1.5, 1.4, 1.2), 15.0))]
+    cam = dict(mode=mode, denoise=denoise, ref_depth=ref_depth, w=width, h=height, transform=cam_xf,
+               projection=perspective_infinite_reverse_rh(math.pi / 3.0, width / height, 0.1))
+    return dict(name="env_courtyard", meshes=meshes, materials=materials, instances=instances, lights=lights, sun=(0.0, -1.2), camera=cam,
+                environment_map=dict(rgba=courtyard_sky(), intensity=1.5, rotation=0.0))

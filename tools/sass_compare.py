@@ -1,6 +1,6 @@
 """Compare per-kernel SASS of two libstrolle_b200.so builds: every kernel of the old build against the same kernel (for a kernel that
-gained `bool NMAP` / `bool LGRID` / `bool TEXF` template parameters: its all-<false> instantiation, whose trailing LightGridDev and
-TexFilterDev arguments are unused) of the new one.  Compared: the full instruction text (opcodes,
+gained `bool NMAP` / `bool LGRID` / `bool TEXF` / `bool ENVM` template parameters: its all-<false> instantiation, whose trailing
+LightGridDev, TexFilterDev and EnvMapDev arguments are unused) of the new one.  Compared: the full instruction text (opcodes,
 registers, immediates, constant-bank operands); normalised: the code-offset comments, branch targets and relocated symbol names."""
 import re, subprocess, sys
 
@@ -25,14 +25,21 @@ def kernels(lib):
     dem = subprocess.run(["c++filt"], input="\n".join(funcs), capture_output=True, text=True).stdout.split("\n")
     NM = ("k_prim_gbuffer", "k_gi_sampling_a", "k_ref_tracing", "k_gi_sampling_fused")                          # bool NMAP
     LG = {"k_di_sampling": 0, "k_di_sample_temporal": 0, "k_gi_sampling_b": 0, "k_ref_shading": 0, "k_gi_sampling_fused": 1}   # bool LGRID, its position
+    EM = ("k_di_resolving", "k_gi_sampling_b", "k_gi_sampling_fused", "k_ref_shading")                          # bool ENVM, the last
     def base(d):
         m = re.search(r"::(\w+)<", d)
-        return m.group(1) if m and (m.group(1) in NM or m.group(1) in LG) else None
+        return m.group(1) if m and (m.group(1) in NM or m.group(1) in LG or m.group(1) in EM) else None
     def targs(d): return d.split("(")[0].split("<", 1)[1].rstrip(">").split(", ")
-    def norm(d):   # the name the kernel had before it gained TEXF, LGRID (and NMAP): all-false instantiations lose their template arguments
+    def norm(d):   # the name the kernel had before it gained ENVM, TEXF, LGRID (and NMAP): all-false instantiations lose their template arguments
         k = base(d)
         if k is None: return d
         args = targs(d)
+        if "EnvMapDev)" in d:   # bool ENVM, the last template argument
+            if args[-1] == "true": return d
+            del args[-1]
+            head = d.split("(")[0]
+            d = head.split("<")[0] + "<" + ", ".join(args) + ">" + re.sub(r", \w+::EnvMapDev\)", ")", d[len(head):])
+            if not args: d = re.sub(r"<>", "", d, count=1)
         if "TexFilterDev)" in d:   # bool TEXF, the last template argument
             if args[-1] == "true": return d
             del args[-1]
@@ -59,5 +66,5 @@ for k, body in sorted(old.items()):
         if "-v" in sys.argv:
             import difflib
             print("\n".join(list(difflib.unified_diff(body, new[k], lineterm="", n=1))[:60]))
-print(f"{same} kernels identical, {diff} differ; {len(old)} kernels in the old build, {len(new)} (+{len(nmap)} NMAP / LGRID / TEXF instantiations) in the new")
-for k in sorted(nmap): print("  NMAP / LGRID / TEXF:", k)
+print(f"{same} kernels identical, {diff} differ; {len(old)} kernels in the old build, {len(new)} (+{len(nmap)} NMAP / LGRID / TEXF / ENVM instantiations) in the new")
+for k in sorted(nmap): print("  NMAP / LGRID / TEXF / ENVM:", k)
