@@ -167,7 +167,9 @@ int st_read_buffer(st_engine* e, st_camera_handle camera, const char* name, floa
  * RGBA8 texels of the pool (byte 0 = red).  The pool holds levels 1.. of every live image in insertion order, level after level,
  * each row-major; level k + 1 is max(1, w_k >> 1) x max(1, h_k >> 1).  While the frames render with an environment map (set, and
  * taken by a tick), "environment_map" as 32-bit words: {W, H, intensity bits, rotation bits (reduced)}, then the W x H x 4 floats of
- * the texels as uploaded. */
+ * the texels as uploaded.  While ST_OPT_ENVIRONMENT_MAP_SAMPLING is on, a map is set and a tick has built its distribution,
+ * "environment_map_distribution" as 32-bit words: {W, H, total bits}, then the H floats of the marginal CDF, then the H x W floats of
+ * the conditional CDFs, row by row (the total is the marginal's last value; 0 or not finite: the frames do not use it). */
 int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap_floats, size_t* count);
 int st_bvh_depth(st_engine* e, int* depth);
 uint32_t st_frame(st_engine* e);
@@ -197,7 +199,17 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18, ST_OPT_ENVIRONMENT_MAP_SAMPLING = 19 };
+/* ST_OPT_ENVIRONMENT_MAP_SAMPLING (default 0; 1 = on, anything else is ST_ERR_INVALID): while an environment map is set
+ * (st_set_environment_map), the GI bounce and the GI sky draw aim at the map's bright texels.  A tick that uploads a map with other
+ * texels, or that finds the option turned on, builds on the device a distribution over the texels (weight: the largest RGB channel of
+ * the texel's 3x3 neighbourhood times sin theta; f32 running sums, row by row, then over the rows); the distribution is freed when
+ * the map is cleared or the option turns off.  With it, K12's bounce direction comes with probability 1/2 from the map and otherwise
+ * from the BRDF, weighted by the mixture's density; K13's sky draw at a bounce hit comes from the map, weighted by its density.  Only
+ * how directions are drawn changes, not what is estimated: the frame's expectation is the option-off one, with less variance where
+ * the map's light is concentrated.  With no map, or a map whose total weight is 0 or not finite, every buffer is the option-off one.
+ * Takes effect at the next st_tick; ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS counts the builds; st_read_scene
+ * ("environment_map_distribution") returns the distribution (DESIGN.md §2 "Environment map sampling"). */
 /* ST_OPT_TEXTURE_FILTER (default 0; 1 = on, anything else is ST_ERR_INVALID): material textures are filtered through per-image mip
  * chains with a ray-cone level of detail, instead of the nearest texel of level 0 (the reference's sampler, so 0 keeps parity).
  * Level 0 is the image's atlas rect; levels 1.. (each texel the 2x2 box of the level above, averaged in linear light through the
@@ -315,7 +327,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_LIGHT_GRID_BUILDS = 10 /* light grid builds (ST_OPT_LIGHT_GRID) since creation */,
        ST_STAT_TEXTURE_MIP_BUILDS = 11 /* mip-chain builds (ST_OPT_TEXTURE_FILTER) since creation */,
        ST_STAT_TAA_RESOLVES = 12 /* temporal resolve launches (ST_OPT_TEMPORAL_AA) since creation */,
-       ST_STAT_ENVIRONMENT_MAP_LAUNCHES = 13 /* launches of the environment-mapped kernel variants (st_set_environment_map) since creation */ };
+       ST_STAT_ENVIRONMENT_MAP_LAUNCHES = 13 /* launches of the environment-mapped kernel variants (st_set_environment_map) since creation */,
+       ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14 /* environment-map distribution builds (ST_OPT_ENVIRONMENT_MAP_SAMPLING) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,

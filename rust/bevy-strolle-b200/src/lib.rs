@@ -52,6 +52,8 @@ pub struct StrolleSun {
 /// pixel centre, as the reference does); needs one GPU.
 /// `environment_map`: light the scene from an equirectangular HDR map in place of the procedural sky (None, the default, keeps the
 /// reference's sky); put the sun (`StrolleSun`) below the horizon to light from the map alone.
+/// `environment_map_sampling`: aim the GI bounce and sky draw at the environment map's bright texels (false, the default, draws
+/// from the BRDF and the uniform hemisphere, as the reference does) - for HDRIs with a small, bright sun.
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
@@ -60,6 +62,7 @@ pub struct StrolleSettings {
     pub texture_filter: bool,
     pub temporal_aa: bool,
     pub environment_map: Option<st::EnvironmentMap>,
+    pub environment_map_sampling: bool,
 }
 
 #[derive(Clone, Debug)]
@@ -105,6 +108,7 @@ impl Plugin for StrollePlugin {
         engine.set_light_grid(settings.light_grid).expect("strolle_b200: ST_OPT_LIGHT_GRID");
         engine.set_texture_filter(settings.texture_filter).expect("strolle_b200: ST_OPT_TEXTURE_FILTER");
         engine.set_temporal_aa(settings.temporal_aa).expect("strolle_b200: ST_OPT_TEMPORAL_AA");
+        engine.set_environment_map_sampling(settings.environment_map_sampling).expect("strolle_b200: ST_OPT_ENVIRONMENT_MAP_SAMPLING");
         sync::set_environment_map(&mut engine, settings.environment_map.as_ref());
         render_app.insert_resource(EngineResource(engine));
     }

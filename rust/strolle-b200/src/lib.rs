@@ -465,6 +465,14 @@ impl<P: Params> Engine<P> {
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_TEMPORAL_AA, on as c_int) })
     }
 
+    /// Draws the GI bounce and the GI sky draw from the environment map's distribution, where its light is
+    /// (`ST_OPT_ENVIRONMENT_MAP_SAMPLING`; off, the default, draws from the BRDF and the uniform hemisphere, as the reference does).
+    /// Changes only the noise, not the expected frame; has an effect only while a map is set.  Takes effect with the next frame's
+    /// scene update.
+    pub fn set_environment_map_sampling(&mut self, on: bool) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_ENVIRONMENT_MAP_SAMPLING, on as c_int) })
+    }
+
     /// Lights the scene from an equirectangular environment map in place of the procedural sky (`st_set_environment_map`; `None`,
     /// the default, keeps the reference's procedural sky).  The sun light still follows `update_sun`: to light from the map alone,
     /// put the sun below the horizon.  Takes effect with the next frame's scene update.

@@ -497,6 +497,11 @@ struct st_engine {
     // instantiation
     std::vector<float4> h_envm; uint32_t envm_w = 0, envm_h = 0; float envm_intensity = 0.0f, envm_rotation = 0.0f;
     bool envm_set = false, envm_dirty = false, envm_frame = false; EnvMapDev envm{}; DevMem d_envm; uint64_t envm_launches = 0;
+    // ST_OPT_ENVIRONMENT_MAP_SAMPLING: `envm_sampling` = the option, `envs_built` = d_envs holds the distribution of the map as st_tick
+    // took it (envm.cdf / envm.total), `envs_frame` = the frame's GI sampling kernels run their ENV_SAMPLED instantiation
+    // `envm_new_texels` = the map set since the last tick has other texels than the one before (a new intensity or rotation alone keeps
+    // the distribution)
+    bool envm_sampling = false, envs_built = false, envs_frame = false, envm_new_texels = false; DevMem d_envs; uint64_t envs_builds = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -749,6 +754,28 @@ static int upload(st_engine* e, DevMem& d, const void* src, size_t bytes) {
     return ST_OK;
 }
 
+// ---- ST_OPT_ENVIRONMENT_MAP_SAMPLING (DESIGN.md §2 "Environment map sampling") ------------------------------------------------
+// Builds the distribution of the map st_tick took (e->envm) into d_envs: each row's sin(pi (i + 0.5) / H), evaluated in double and
+// rounded to f32, goes up into the marginal's slots, the kernels leave the CDFs there; the total comes back to the host, which picks
+// the instantiation from it.
+static int build_env_distribution(st_engine* e) {
+    const uint32_t W = e->envm.w, H = e->envm.h;
+    std::vector<float> sin_theta(H);
+    for (uint32_t i = 0; i < H; i++) sin_theta[i] = (float)std::sin(3.141592653589793 * ((double)i + 0.5) / (double)H);
+    int rc = e->d_envs.ensure(sizeof(float) * ((size_t)H + (size_t)W * H));
+    if (rc) return rc;
+    float* cdf = (float*)e->d_envs.p;
+    CK(cudaMemcpyAsync(cdf, sin_theta.data(), sizeof(float) * H, cudaMemcpyHostToDevice, e->stream));
+    launch_envdist_build(e->envm.texels, W, H, cdf, e->stream);
+    CK(cudaGetLastError());
+    float total = 0.0f;
+    CK(cudaMemcpyAsync(&total, cdf + H - 1, sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    e->envm.cdf = cdf; e->envm.total = total;
+    e->envs_built = true; e->envs_builds++;
+    return ST_OK;
+}
+
 // ---- ST_OPT_BVH_REFIT ------------------------------------------------------------------------------------
 static const st_engine::Range* range_of(const st_engine* e, st_handle inst) {
     for (const auto& r : e->tri_ranges) if (r.handle == inst) return &r;
@@ -988,7 +1015,9 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     const bool tfon = e->texf_frame;   // filtered material textures (ST_OPT_TEXTURE_FILTER)
     const TexFilterDev tfd = e->texf;
     const bool emon = e->envm_frame;   // the environment map in place of the procedural sky (st_set_environment_map)
-    const EnvMapDev emd = e->envm;
+    EnvMapDev emd = e->envm;
+    if (!e->envs_frame) emd.cdf = nullptr;   // ST_OPT_ENVIRONMENT_MAP_SAMPLING: K12 / K13 draw from the map's distribution
+    const bool eson = emon && e->envs_frame;
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
     auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
@@ -1048,7 +1077,11 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
                     });
                     return;
                 }
-                add(P_GI_SAMPLING_A, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, nm, tfon ? &tfd : nullptr, s); });
+                add(P_GI_SAMPLING_A, [=](cudaStream_t s) {
+                    if (nm) e->normal_map_launches++;
+                    if (eson) e->envm_launches++;
+                    (fs ? stf::launch_gi_sampling_a : st::launch_gi_sampling_a)(cam, sc, cur, sa, f, nm, tfon ? &tfd : nullptr, eson ? &emd : nullptr, s);
+                });
                 add(P_GI_SAMPLING_B, [=](cudaStream_t s) { if (emon) e->envm_launches++; (fs ? stf::launch_gi_sampling_b : st::launch_gi_sampling_b)(cam, sc, cur, sb, f, lgon ? &lgd : nullptr, emon ? &emd : nullptr, s); });
             };
             if (tracing) {
@@ -1494,7 +1527,7 @@ void st_engine_destroy(st_engine* e) {
     if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
     for (CameraSlot* c : e->cameras) { for (int k = 0; k < 2; k++) { if (c->side[k]) { cudaStreamSynchronize(c->side[k]); cudaStreamDestroy(c->side[k]); } if (c->ev_pushed[k]) cudaEventDestroy(c->ev_pushed[k]); } if (c->ev_produced) cudaEventDestroy(c->ev_produced);
         c->arena.release(); c->svgf_pairs.release(); c->rgba8.release(); for (int k = 0; k < 2; k++) { if (c->ev_ready[k]) cudaEventDestroy(c->ev_ready[k]); if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]); } delete c; }
-    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake, &e->d_lgrid, &e->d_texf_pool, &e->d_texf_table, &e->d_texf_jobs, &e->d_envm};
+    DevMem* all[] = {&e->d_triangles, &e->d_bvh, &e->d_materials, &e->d_lights, &e->d_noise, &e->d_tlut, &e->d_slut, &e->d_skylut, &e->d_scratch, &e->d_raycount, &e->d_matpacked, &e->d_unpacklut, &e->d_atlas, &e->d_srgb, &e->d_tri_instance, &e->d_instance_xforms, &e->d_tile_errors, &e->d_plan, &e->d_bake, &e->d_lgrid, &e->d_texf_pool, &e->d_texf_table, &e->d_texf_jobs, &e->d_envm, &e->d_envs};
     for (DevMem* d : all) d->release();
     for (auto& m : e->d_meshes) m.second.release();
     for (int k = 0; k < 2; k++) { if (e->staging[k]) cudaFreeHost(e->staging[k]); if (e->staging_ev[k]) cudaEventDestroy(e->staging_ev[k]); }
@@ -1826,8 +1859,15 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
             e->envm.texels = (const float4*)e->d_envm.p; e->envm.w = e->envm_w; e->envm.h = e->envm_h;
             e->envm.intensity = e->envm_intensity; e->envm.rotation = e->envm_rotation;
         } else { e->d_envm.release(); e->envm = EnvMapDev{}; }
+        if (e->envm_new_texels || !e->envm_set) e->envs_built = false;
+        e->envm_new_texels = false;
     }
     e->envm_frame = e->envm_set;
+    // ST_OPT_ENVIRONMENT_MAP_SAMPLING: the distribution follows the map just uploaded, exists only while the option is on and a map is
+    // set, and is used only where it has a finite, positive total
+    if (!(e->envm_sampling && e->envm_set)) { e->d_envs.release(); e->envs_built = false; e->envm.cdf = nullptr; e->envm.total = 0.0f; }
+    else if (!e->envs_built) { if ((rc = build_env_distribution(e))) return rc; }
+    e->envs_frame = e->envs_built && e->envm.total > 0.0f && e->envm.total < INFINITY;
     // ST_OPT_TEMPORAL_AA: the history exists only while the option is on, and starts over when it turns on
     if (e->temporal_aa != e->taa_frame) for (CameraSlot* c : e->cameras) { c->taa.release(); c->taa_hist[0] = c->taa_hist[1] = nullptr; }
     e->taa_frame = e->temporal_aa;
@@ -1981,6 +2021,21 @@ int st_read_scene(st_engine* e, const char* name, float* dst, size_t cap, size_t
         }
         return ST_OK;
     }
+    if (s == "environment_map_distribution") {   // {W, H, total bits}, the marginal CDF, the conditional CDFs (include/strolle_b200.h)
+        if (!e->envs_built) return fail(ST_ERR_NOT_FOUND, "no environment map distribution: ST_OPT_ENVIRONMENT_MAP_SAMPLING is off, no map is set or no st_tick has built it");
+        const size_t n = (size_t)e->envm.h + (size_t)e->envm.w * e->envm.h;
+        *count = 3 + n;
+        if (dst) {
+            uint32_t head[3] = {e->envm.w, e->envm.h, 0u};
+            std::memcpy(head + 2, &e->envm.total, 4);
+            std::memcpy(dst, head, 4 * std::min<size_t>(cap, 3));
+            if (cap > 3) {
+                CK(cudaStreamSynchronize(e->stream));
+                CK(cudaMemcpy(dst + 3, e->envm.cdf, 4 * std::min(cap - 3, n), cudaMemcpyDeviceToHost));
+            }
+        }
+        return ST_OK;
+    }
     if (s == "texture_mips") {   // {pool texels, materials}, the table, the pool (include/strolle_b200.h)
         if (!e->texf_built) return fail(ST_ERR_NOT_FOUND, "no mip chains: ST_OPT_TEXTURE_FILTER is off or no st_tick has built them");
         std::vector<uint32_t> w = {(uint32_t)e->texf_pool_texels, (uint32_t)e->h_materials.size()};
@@ -2054,6 +2109,7 @@ int st_set_environment_map(st_engine* e, const float* rgba32f, uint32_t width, u
     double r = std::fmod((double)rotation, two_pi);
     if (r < 0.0) r += two_pi;
     if (r >= two_pi) r = 0.0;
+    if (!(e->envm_set && width == e->envm_w && height == e->envm_h && std::memcmp(e->h_envm.data(), rgba32f, n * sizeof(float4)) == 0)) e->envm_new_texels = true;
     e->h_envm.resize(n);
     std::memcpy(e->h_envm.data(), rgba32f, n * sizeof(float4));
     e->envm_w = width; e->envm_h = height; e->envm_intensity = intensity; e->envm_rotation = (float)r;
@@ -2101,6 +2157,10 @@ int st_set_option(st_engine* e, int option, int value) {
     if (option == ST_OPT_TEXTURE_FILTER) {   // takes effect at the next st_tick
         if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_TEXTURE_FILTER: 0 (nearest level-0 texel) or 1 (filtered)");
         e->texture_filter = value == 1; return ST_OK;
+    }
+    if (option == ST_OPT_ENVIRONMENT_MAP_SAMPLING) {   // takes effect at the next st_tick
+        if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_ENVIRONMENT_MAP_SAMPLING: 0 (BRDF and uniform draws) or 1 (draws from the map)");
+        e->envm_sampling = value != 0; return ST_OK;
     }
     if (option == ST_OPT_TEMPORAL_AA) {   // takes effect at the next st_tick
         if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_TEMPORAL_AA: 0 (off) or 1 (jitter + temporal resolve)");
@@ -2153,6 +2213,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_TEXTURE_MIP_BUILDS) { *value = e->texture_mip_builds; return ST_OK; }
     if (stat == ST_STAT_TAA_RESOLVES) { *value = e->taa_resolves; return ST_OK; }
     if (stat == ST_STAT_ENVIRONMENT_MAP_LAUNCHES) { *value = e->envm_launches; return ST_OK; }
+    if (stat == ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS) { *value = e->envs_builds; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
         CK(cudaSetDevice(e->device)); CK(cudaStreamSynchronize(e->stream));
         uint64_t total = 0;

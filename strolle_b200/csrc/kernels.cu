@@ -512,9 +512,11 @@ __global__ void __launch_bounds__(ST_BLOCK) k_gi_reprojection(KPARAMS, int cur) 
 // returns false where the kernel leaves without writing its three scratch texels (gi_d0: ray direction + pdf, gi_d1/gi_d2: the packed
 // G-buffer entry of what the ray hit)
 // TEXF: the bounce hit's textures are filtered, with a fresh cone from the segment's origin
-template <bool NMAP, bool TEXF>
+// ENVM == ENV_SAMPLED (ST_OPT_ENVIRONMENT_MAP_SAMPLING): on tracing frames one extra draw first picks, with probability 1/2, a direction
+// from the map's distribution, else the BRDF's (its draws unchanged); gi_d0.w is then q / kappa (env_mixture_pdf) in place of the pdf
+template <bool NMAP, bool TEXF, int ENVM>
 ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4* t0, float4* t1, float4* t2,
-                               const TexFilterDev& tf) {
+                               const TexFilterDev& tf, const EnvMapDev& em) {
     bool tracing = gi_tracing_frame(frame);
     uint2 sp = tracing ? checker(g.x, g.y, frame / 2u) : checker(g.x, g.y, frame);
     if (!cam_contains_u(cam.curr, sp.x, sp.y)) return false;
@@ -524,9 +526,17 @@ ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const T
         Rng rng = rng_make(seed, sp.x, sp.y);
         Hit hit = load_hit_lut(sc, cam.curr, cam.prim_gbuffer_d0[cur], cam.prim_gbuffer_d1[cur], cam, sp.x, sp.y);
         if (!hit_some(hit)) return false;
-        BrdfS s = brdf_layered_sample(hit.g, rng, -hit.dir);
-        gi_r = ray_make(hit.point, s.dir);
-        gi_pdf_ = s.pdf;
+        if (ENVM == ENV_SAMPLED) {
+            float3 dir;
+            if (rng_f(rng) < 0.5f) { const float xi1 = rng_f(rng), xi2 = rng_f(rng); dir = env_draw(em, xi1, xi2); }
+            else dir = brdf_layered_sample(hit.g, rng, -hit.dir).dir;
+            gi_r = ray_make(hit.point, dir);
+            gi_pdf_ = env_mixture_pdf(em, hit.g, -hit.dir, dir);
+        } else {
+            BrdfS s = brdf_layered_sample(hit.g, rng, -hit.dir);
+            gi_r = ray_make(hit.point, s.dir);
+            gi_pdf_ = s.pdf;
+        }
     } else {
         GiRes res = gi_load(cam.gi_reservoirs[2], idx);
         if (res.m == 0.0f) return false;
@@ -554,21 +564,23 @@ ST_DEV bool gi_sampling_a_pair(const CameraDev& cam, const SceneDev& sc, const T
     *t0 = f4(gi_r.d, gi_pdf_);
     return true;
 }
-template <bool NMAP, bool TEXF>
-__global__ void ST_LB_GI_SAMPLING_A k_gi_sampling_a(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ TexFilterDev tf) {
+template <bool NMAP, bool TEXF, int ENVM>
+__global__ void ST_LB_GI_SAMPLING_A k_gi_sampling_a(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ TexFilterDev tf, const __grid_constant__ EnvMapDev em) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
-    if (!gi_sampling_a_pair<NMAP, TEXF>(cam, sc, stk, cur, seed, frame, g, &t0, &t1, &t2, tf)) return;
+    if (!gi_sampling_a_pair<NMAP, TEXF, ENVM>(cam, sc, stk, cur, seed, frame, g, &t0, &t1, &t2, tf, em)) return;
     size_t gi = pix(cam, g.x, g.y);
     cam.gi_d0[gi] = t0; cam.gi_d1[gi] = t1; cam.gi_d2[gi] = t2;
 }
 
 // K13 gi_sampling_b::main (gi_sampling_b.rs:4-235); LGRID: the light candidates come from the light grid's list for the bounce hit
 // (the sky-or-light draw still tests the global light count, so the RNG sequence keeps its shape); ENVM: the missed bounce and the sky
-// draw see the map, and the sky draw's probability is 0.25 whatever the sun's altitude (the map does not darken with the sun)
-template <bool LGRID, bool ENVM>
+// draw see the map, and the sky draw's probability is 0.25 whatever the sun's altitude (the map does not darken with the sun);
+// ENVM == ENV_SAMPLED: the sky draw takes its direction from the map's distribution with the same two draws, and its value is
+// L max(n.w, 0) / (2 pi p_env) (no shadow ray where n.w <= 0)
+template <bool LGRID, int ENVM>
 ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const TraceStack& stk, int cur, u32 seed, u32 frame, Px g, float4 d0, float4 d1, float4 d2, const LightGridDev& lg,
                                const EnvMapDev& em) {
     bool tracing = gi_tracing_frame(frame);
@@ -593,13 +605,23 @@ ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const T
     const u32 SKY = 0xffffffffu;
     float3 sun_dir = world_sun_dir(sc.world);
     u32 light_id; float light_pdf; float3 light_rad; float3 light_dir = f3s(0.f);
-    if (!hit_some(gh)) { light_id = SKY; light_pdf = 1.0f; light_rad = sky_radiance<ENVM>(sc, em, sun_dir, gh.dir); }
+    bool sky_below = false;   // ENV_SAMPLED: the sky draw points below the bounce hit's surface
+    if (!hit_some(gh)) { light_id = SKY; light_pdf = 1.0f; light_rad = sky_radiance<ENVM != ENV_NONE>(sc, em, sun_dir, gh.dir); }
     else {
-        float atm_pdf = (!ENVM && sc.world.sun_altitude <= -1.0f) ? 0.0f : 0.25f;
+        float atm_pdf = (ENVM == ENV_NONE && sc.world.sun_altitude <= -1.0f) ? 0.0f : 0.25f;
         if (sc.world.light_count == 0u || rng_f(rng) < atm_pdf) {
             light_id = SKY; light_pdf = atm_pdf;
-            light_dir = rng_hemisphere(rng, gh.g.normal);
-            light_rad = sky_radiance<ENVM>(sc, em, sun_dir, light_dir) * dot(gh.g.normal, light_dir);
+            if (ENVM == ENV_SAMPLED) {
+                const float xi1 = rng_f(rng), xi2 = rng_f(rng);
+                light_dir = env_draw(em, xi1, xi2);
+                const float c = xdot(gh.g.normal, light_dir);
+                sky_below = !(c > 0.0f);
+                const float p = sky_below ? 0.0f : env_pdf(em, light_dir);
+                light_rad = p > 0.0f ? xscale(env_sample(em, light_dir), xdiv(c, xmul(6.283185307179586f, p))) : f3s(0.0f);
+            } else {
+                light_dir = rng_hemisphere(rng, gh.g.normal);
+                light_rad = sky_radiance<ENVM != ENV_NONE>(sc, em, sun_dir, light_dir) * dot(gh.g.normal, light_dir);
+            }
         } else {
             EphRes er = LGRID ? ephemeral_build_list(rng, sc, gh, lgrid_list(lg, gh.point)) : ephemeral_build(rng, sc, gh);
             if (er.w > 0.0f) { light_id = er.light_id; light_pdf = (1.0f / er.w) * (1.0f - atm_pdf); light_rad = er.rad.radiance * (f3s(1.0f) + er.rad.spec); }
@@ -610,8 +632,11 @@ ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const T
     if (light_pdf > 0.0f) {
         float vis;
         if (hit_some(gh)) {
-            Ray r = (light_id == SKY) ? ray_make(gh.point, light_dir) : light_ray_wnoise(light_load(sc, light_id), rng, gh.point);
-            vis = trace_any(r, sc, stk) ? 0.0f : 1.0f;
+            if (ENVM == ENV_SAMPLED && sky_below) vis = 0.0f;
+            else {
+                Ray r = (light_id == SKY) ? ray_make(gh.point, light_dir) : light_ray_wnoise(light_load(sc, light_id), rng, gh.point);
+                vis = trace_any(r, sc, stk) ? 0.0f : 1.0f;
+            }
         } else vis = 1.0f;
         radiance = light_rad * vis / light_pdf;
     } else radiance = f3s(0.f);
@@ -627,7 +652,7 @@ ST_DEV void gi_sampling_b_pair(const CameraDev& cam, const SceneDev& sc, const T
     }
     gi_store(res, cam.gi_reservoirs[1], idx);
 }
-template <bool LGRID, bool ENVM>
+template <bool LGRID, int ENVM>
 __global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, u32 frame, const __grid_constant__ LightGridDev lg, const __grid_constant__ EnvMapDev em) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
@@ -637,14 +662,14 @@ __global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_b(KPARAMS, int cur, u32 seed, 
 }
 // K12 + K13 in one launch (ST_OPT_FUSED_PASSES): the bounce ray is traced and shaded by the same thread; the hit still goes through
 // GBufferEntry's pack / unpack (its 8-bit quantisation is part of the result), just not through memory.
-template <bool NMAP, bool LGRID, bool TEXF, bool ENVM>
+template <bool NMAP, bool LGRID, bool TEXF, int ENVM>
 __global__ void ST_LB_GI_SAMPLING_B k_gi_sampling_fused(KPARAMS, int cur, u32 seed_a, u32 seed_b, u32 frame, const __grid_constant__ LightGridDev lg,
                                                         const __grid_constant__ TexFilterDev tf, const __grid_constant__ EnvMapDev em) {
     ST_TRACE_STACK();
     Px g = pixel_half(cam);
     if (!g.in) return;
     float4 t0, t1, t2;
-    if (!gi_sampling_a_pair<NMAP, TEXF>(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2, tf)) return;
+    if (!gi_sampling_a_pair<NMAP, TEXF, ENVM == ENV_SAMPLED ? ENV_SAMPLED : ENV_NONE>(cam, sc, stk, cur, seed_a, frame, g, &t0, &t1, &t2, tf, em)) return;
     gi_sampling_b_pair<LGRID, ENVM>(cam, sc, stk, cur, seed_b, frame, g, t0, t1, t2, lg, em);
 }
 
@@ -1799,13 +1824,18 @@ void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, const E
     if (em) k_di_resolving<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, *em); else k_di_resolving<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, EnvMapDev{});
 }
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st) { k_gi_reprojection<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur); }
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st) {
-    if (tf) {
-        if (nmap) HALF_LAUNCH((k_gi_sampling_a<true, true>), c, st, c, s, cur, seed, frame, *tf); else HALF_LAUNCH((k_gi_sampling_a<false, true>), c, st, c, s, cur, seed, frame, *tf);
-    } else {
-        const TexFilterDev none{};
-        if (nmap) HALF_LAUNCH((k_gi_sampling_a<true, false>), c, st, c, s, cur, seed, frame, none); else HALF_LAUNCH((k_gi_sampling_a<false, false>), c, st, c, s, cur, seed, frame, none);
-    }
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, const EnvMapDev* em,
+                          cudaStream_t st) {
+    const TexFilterDev tnone{};
+    const TexFilterDev& t = tf ? *tf : tnone;
+    const EnvMapDev enone{};
+    const EnvMapDev& m = em ? *em : enone;
+#define ST_GSA(N_, T_, E_) HALF_LAUNCH((k_gi_sampling_a<N_, T_, E_>), c, st, c, s, cur, seed, frame, t, m)
+#define ST_GSA_E(N_, T_) do { if (em && em->cdf) ST_GSA(N_, T_, ENV_SAMPLED); else ST_GSA(N_, T_, ENV_NONE); } while (0)
+    if (tf) { if (nmap) ST_GSA_E(true, true); else ST_GSA_E(false, true); }
+    else { if (nmap) ST_GSA_E(true, false); else ST_GSA_E(false, false); }
+#undef ST_GSA_E
+#undef ST_GSA
 }
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, const EnvMapDev* em, cudaStream_t st) {
     const LightGridDev none{};
@@ -1813,8 +1843,9 @@ void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 se
     const EnvMapDev enone{};
     const EnvMapDev& m = em ? *em : enone;
 #define ST_GSB(L_, E_) HALF_LAUNCH((k_gi_sampling_b<L_, E_>), c, st, c, s, cur, seed, frame, g, m)
-    if (em) { if (lg) ST_GSB(true, true); else ST_GSB(false, true); }
-    else { if (lg) ST_GSB(true, false); else ST_GSB(false, false); }
+#define ST_GSB_E(L_) do { if (!em) ST_GSB(L_, ENV_NONE); else if (em->cdf) ST_GSB(L_, ENV_SAMPLED); else ST_GSB(L_, ENV_MAP); } while (0)
+    if (lg) ST_GSB_E(true); else ST_GSB_E(false);
+#undef ST_GSB_E
 #undef ST_GSB
 }
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st) { k_gi_temporal<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, cur, seed, frame, inline_reprojection); }
@@ -1836,7 +1867,7 @@ void launch_gi_sampling_fused(const CameraDev& c, const SceneDev& s, int cur, u3
     const EnvMapDev enone{};
     const EnvMapDev& m = em ? *em : enone;
 #define ST_GSF(N_, L_, T_, E_) HALF_LAUNCH((k_gi_sampling_fused<N_, L_, T_, E_>), c, st, c, s, cur, seed_a, seed_b, frame, g, t, m)
-#define ST_GSF_E(N_, L_, T_) do { if (em) ST_GSF(N_, L_, T_, true); else ST_GSF(N_, L_, T_, false); } while (0)
+#define ST_GSF_E(N_, L_, T_) do { if (!em) ST_GSF(N_, L_, T_, ENV_NONE); else if (em->cdf) ST_GSF(N_, L_, T_, ENV_SAMPLED); else ST_GSF(N_, L_, T_, ENV_MAP); } while (0)
     if (tf) {
         if (lg) { if (nmap) ST_GSF_E(true, true, true); else ST_GSF_E(false, true, true); }
         else { if (nmap) ST_GSF_E(true, false, true); else ST_GSF_E(false, false, true); }
@@ -2107,6 +2138,59 @@ void launch_math(int op, const float* a, const float* b, float* out, long n, cud
     if (op == 7) k_math_log2<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, out, n);
     else if (op == 8 || op == 9) k_math_envm<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n);
     else k_math<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(op, a, b, out, n);
+}
+// ST_OPT_ENVIRONMENT_MAP_SAMPLING (DESIGN.md §2 "Environment map sampling"): one warp per row i.  Texel (i, j)'s weight is the
+// largest RGB channel over rows i-1..i+1 (clamped) and columns j-1..j+1 (wrapped), times the row's sin theta (cdf[i] on entry); the
+// row's conditional CDF is the f32 running sum of its weights in column order.  Every lane adds the 32 weights of a chunk in order,
+// so the sum is the sequential one.
+__device__ __forceinline__ float envdist_max3(float4 t) { return fmaxf(fmaxf(t.x, t.y), t.z); }
+__device__ __forceinline__ float envdist_scan32(float w, float* acc, u32 n) {   // the running sum at this lane, over lanes 0..n-1
+    const u32 lane = threadIdx.x & 31u;
+    float mine = 0.0f;
+    for (u32 q = 0; q < n; q++) {
+        const float x = __shfl_sync(0xffffffffu, w, q);
+        *acc = xadd(*acc, x);
+        if (lane == q) mine = *acc;
+    }
+    return mine;
+}
+__global__ void __launch_bounds__(256) k_envdist_rows(const float4* __restrict__ texels, u32 w, u32 h, float* __restrict__ cdf) {
+    const u32 i = blockIdx.x * 8u + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+    if (i >= h) return;
+    const float sin_theta = cdf[i];
+    const u32 r0 = i ? i - 1u : 0u, r2 = i + 1u < h ? i + 1u : h - 1u;
+    float* row = cdf + h + (size_t)i * w;
+    float acc = 0.0f;
+    for (u32 base = 0; base < w; base += 32u) {
+        const u32 j = base + lane;
+        float wt = 0.0f;
+        if (j < w) {
+            const u32 jl = j ? j - 1u : w - 1u, jr = j + 1u < w ? j + 1u : 0u;
+            float m = 0.0f;
+            for (u32 r : {r0, i, r2}) {
+                const float4* t = texels + (size_t)r * w;
+                m = fmaxf(m, fmaxf(envdist_max3(__ldg(t + jl)), fmaxf(envdist_max3(__ldg(t + j)), envdist_max3(__ldg(t + jr)))));
+            }
+            wt = xmul(m, sin_theta);
+        }
+        const float c = envdist_scan32(wt, &acc, min(32u, w - base));
+        if (j < w) row[j] = c;
+    }
+}
+// The marginal CDF: the f32 running sum of the rows' last conditional values, in row order, by one warp.
+__global__ void __launch_bounds__(32) k_envdist_marginal(u32 w, u32 h, float* __restrict__ cdf) {
+    const u32 lane = threadIdx.x & 31u;
+    float acc = 0.0f;
+    for (u32 base = 0; base < h; base += 32u) {
+        const u32 i = base + lane;
+        const float r = i < h ? cdf[h + (size_t)i * w + w - 1u] : 0.0f;
+        const float c = envdist_scan32(r, &acc, min(32u, h - base));
+        if (i < h) cdf[i] = c;
+    }
+}
+void launch_envdist_build(const float4* texels, uint32_t w, uint32_t h, float* cdf, cudaStream_t st) {
+    k_envdist_rows<<<(h + 7u) / 8u, 256, 0, st>>>(texels, w, h, cdf);
+    k_envdist_marginal<<<1, 32, 0, st>>>(w, h, cdf);
 }
 void launch_light_grid_build(const LightGridDev& lg, const GpuLight* lights, cudaStream_t st) {
     const u32 ncell = lg.dims[0] * lg.dims[1] * lg.dims[2];

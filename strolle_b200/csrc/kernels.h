@@ -8,7 +8,8 @@ typedef uint32_t u32;
 
 // nmap: the NMAP instantiation (normal-mapped shading normal, ST_OPT_NORMAL_MAPS) of the kernels that shade a closest hit;
 // tf (non-null): their TEXF instantiation (filtered material textures, ST_OPT_TEXTURE_FILTER); em (non-null): the ENVM instantiation
-// of the kernels that evaluate the sky (K10, K13 and the fused K12 + K13, K2: the environment map of st_set_environment_map)
+// of the kernels that evaluate the sky (K10, K13 and the fused K12 + K13, K2: the environment map of st_set_environment_map); K12, K13
+// and the fused K12 + K13 run their ENV_SAMPLED instantiation when em->cdf is non-null (ST_OPT_ENVIRONMENT_MAP_SAMPLING)
 void launch_prim_gbuffer(const CameraDev& c, const SceneDev& s, int cur, int with_reprojection, bool nmap, const TexFilterDev* tf, cudaStream_t st);
 void launch_frame_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
 void launch_di_sampling(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, cudaStream_t st);
@@ -18,7 +19,7 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st);
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);
@@ -51,6 +52,9 @@ void launch_trace_stream_any(const SceneDev& s, const float4* rays, long n, u32*
 void launch_math(int op, const float* a, const float* b, float* out, long n, cudaStream_t st);
 // ST_OPT_LIGHT_GRID: fills lg.counts / lg.lists (dims.x * dims.y * dims.z cells, then the outside list) from the device lights
 void launch_light_grid_build(const LightGridDev& lg, const GpuLight* lights, cudaStream_t st);
+// ST_OPT_ENVIRONMENT_MAP_SAMPLING: the distribution of `texels` (w x h) into `cdf` (h + w h floats, DESIGN.md §2 "Environment map
+// sampling"); cdf[0 .. h) holds each row's sin theta on entry (k_envdist_rows reads it before k_envdist_marginal overwrites it)
+void launch_envdist_build(const float4* texels, uint32_t w, uint32_t h, float* cdf, cudaStream_t st);
 // ST_OPT_TEXTURE_FILTER: k_texture_mips for level k + 1 over jobs [first[k], first[k + 1]) with blocks[k] x 256 threads, k < levels,
 // in launches of at most 65535 jobs; returns the first launch error
 cudaError_t launch_texture_mips(const MipJob* jobs, const u32* first, const u32* blocks, int levels, const uchar4* atlas, uchar4* pool, const float* srgb, cudaStream_t st);
@@ -119,7 +123,7 @@ void launch_spatial_trace(const CameraDev& c, const SceneDev& s, const float4* d
 void launch_di_spatial_sample(const CameraDev& c, const SceneDev& s, u32 seed, u32 frame, cudaStream_t st);
 void launch_di_resolving(const CameraDev& c, const SceneDev& s, int cur, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_reprojection(const CameraDev& c, const SceneDev& s, int cur, cudaStream_t st);
-void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, cudaStream_t st);
+void launch_gi_sampling_a(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, bool nmap, const TexFilterDev* tf, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_sampling_b(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, const LightGridDev* lg, const EnvMapDev* em, cudaStream_t st);
 void launch_gi_temporal(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, int inline_reprojection, cudaStream_t st);
 void launch_gi_spatial_pick(const CameraDev& c, const SceneDev& s, int cur, u32 seed, u32 frame, cudaStream_t st);

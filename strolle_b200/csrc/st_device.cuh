@@ -862,6 +862,104 @@ ST_DEV float3 sky_radiance(const SceneDev& sc, const EnvMapDev& em, float3 sun_d
     return ENVM ? env_sample(em, dir) : atmosphere_sample(sc, sun_dir, dir);
 }
 
+// ---- Environment map sampling (ST_OPT_ENVIRONMENT_MAP_SAMPLING; DESIGN.md §2 "Environment map sampling") ------------------------
+// The draw and its density use the x*() primitives only, as the lookup does, so both builds give the same bits.
+// The strict build's sincos_det (Cephes, three-part pi/4 reduction) through the x*() primitives
+ST_DEV void sincos_x(float xx, float* s_out, float* c_out) {
+    float x = fabs_(xx);
+    u32 j = to_u32_sat(xmul(1.27323954473516f, x));
+    float y = (float)j;
+    if (j & 1u) { j += 1u; y = xadd(y, 1.0f); }
+    j &= 7u;
+    x = xsub(xsub(xsub(x, xmul(y, 0.78515625f)), xmul(y, 2.4187564849853515625e-4f)), xmul(y, 3.77489497744594108e-8f));
+    const float z = xmul(x, x);
+    const float ps = xadd(xmul(xmul(xsub(xmul(xadd(xmul(-1.9515295891e-4f, z), 8.3321608736e-3f), z), 1.6666654611e-1f), z), x), x);
+    const float pc = xadd(xsub(xmul(xmul(xadd(xmul(xsub(xmul(2.443315711809948e-5f, z), 1.388731625493765e-3f), z), 4.166664568298827e-2f), z), z),
+                               xmul(0.5f, z)), 1.0f);
+    float s = (j == 0u) ? ps : (j == 2u) ? pc : (j == 4u) ? -ps : -pc;
+    const float c = (j == 0u) ? pc : (j == 2u) ? -ps : (j == 4u) ? -pc : ps;
+    if (fbits(xx) & 0x80000000u) s = -s;
+    *s_out = s; *c_out = c;
+}
+// The first index i < n with cdf[i] > t or cdf[i] == last (the second clause catches t == last, reached by a draw of exactly 1).
+ST_DEV u32 env_cdf_find(const float* cdf, u32 n, float t, float last) {
+    u32 lo = 0u, hi = n - 1u;
+    while (lo < hi) {
+        const u32 mid = (lo + hi) >> 1;
+        const float c = __ldg(cdf + mid);
+        if (c > t || c == last) hi = mid; else lo = mid + 1u;
+    }
+    return lo;
+}
+// A direction drawn with density env_pdf: the row from the marginal CDF at xi1 * total, the column from that row's conditional CDF
+// at xi2 * (the row's last value), each offset inside its cell the remainder over the cell's CDF difference (below 1);
+// u = (j + du) / W, v = (i + dv) / H, phi = (u - 0.5) 2 pi - rotation, theta = pi v, d = (sin theta sin phi, cos theta,
+// -sin theta cos phi): the exact inverse of the lookup's theta = acos(d.y), phi = atan2(d.x, -d.z).
+ST_DEV float3 env_draw(const EnvMapDev& em, float xi1, float xi2) {
+    const u32 W = em.w, H = em.h;
+    const float below_one = 0.99999994039535522f;   // the largest float below 1
+    const float* M = em.cdf;
+    const float t = xmul(xi1, em.total);
+    const u32 i = env_cdf_find(M, H, t, em.total);
+    const float m0 = i ? __ldg(M + i - 1u) : 0.0f, m1 = __ldg(M + i);
+    const float dv = fminf(xdiv(xsub(t, m0), xsub(m1, m0)), below_one);
+    const float* C = em.cdf + H + (size_t)i * W;
+    const float rt = __ldg(C + W - 1u);
+    const float t2 = xmul(xi2, rt);
+    const u32 j = env_cdf_find(C, W, t2, rt);
+    const float c0 = j ? __ldg(C + j - 1u) : 0.0f, c1 = __ldg(C + j);
+    const float du = fminf(xdiv(xsub(t2, c0), xsub(c1, c0)), below_one);
+    const float u = xdiv(xadd((float)j, du), (float)W), v = xdiv(xadd((float)i, dv), (float)H);
+    const float phi = xsub(xmul(xsub(u, 0.5f), 6.283185307179586f), em.rotation), theta = xmul(kPi, v);
+    float st, ct, sp, cp;
+    sincos_x(theta, &st, &ct); sincos_x(phi, &sp, &cp);
+    return f3(xmul(st, sp), ct, -xmul(st, cp));
+}
+// The solid-angle density of env_draw at d: u, v as env_sample computes them, the cell (floor(u W) wrapped, floor(v H) clamped),
+// p = ((row's marginal CDF difference / total) (cell's conditional CDF difference / the row's last value)) (W H) / (2 pi^2 sin theta),
+// sin theta = sqrt(max(0, 1 - d.y^2)); 0 where the cell cannot be drawn, +inf where sin theta = 0.
+ST_DEV float env_pdf(const EnvMapDev& em, float3 d) {
+    const float theta = acos_x(rclamp(d.y, -1.0f, 1.0f)), phi = atan2_x(d.x, -d.z);
+    const float u = xadd(xmul(xadd(phi, em.rotation), 0.15915494309189535f), 0.5f), v = xmul(theta, 0.3183098861837907f);
+    if (!(fabs_(u) < finf()) || !(fabs_(v) < finf())) return 0.0f;
+    const int W = (int)em.w, H = (int)em.h;
+    int j = to_i32_sat(floorf(xmul(u, (float)W))) % W; if (j < 0) j += W;
+    const int i = max(0, min(to_i32_sat(floorf(xmul(v, (float)H))), H - 1));
+    const float* M = em.cdf;
+    const float* C = em.cdf + H + (size_t)i * W;
+    const float pr = xsub(__ldg(M + i), i ? __ldg(M + i - 1) : 0.0f), pc = xsub(__ldg(C + j), j ? __ldg(C + j - 1) : 0.0f);
+    if (!(pr > 0.0f) || !(pc > 0.0f)) return 0.0f;
+    const float st = xsqrt(fmaxf(0.0f, xsub(1.0f, xmul(d.y, d.y))));
+    if (st == 0.0f) return finf();
+    const float prob = xmul(xdiv(pr, em.total), xdiv(pc, __ldg(C + W - 1)));
+    return xdiv(xmul(prob, xmul((float)W, (float)H)), xmul(19.739208802178716f, st));
+}
+// K12's one-sample mixture (ENV_SAMPLED): q(w) / kappa(w) for a bounce direction w at a surface g seen along v.  q = 1/2 p_bsdf +
+// 1/2 p_env with p_bsdf = (1 - m) / 2 pi [n.w > 0] + m p_ggx(w); kappa = (1 - m)^2 / 2 [n.w > 0] + m^2 [p_ggx(w) > 0] is what the
+// reference's per-branch pdfs estimate; +inf where kappa = 0 (the candidate then carries w = 0).
+ST_DEV float env_mixture_pdf(const EnvMapDev& em, const GBuf& g, float3 v, float3 w) {
+    const float m = g.metallic;
+    const float3 n = g.normal;
+    const bool up = xdot(n, w) > 0.0f;
+    float pg = 0.0f;
+    if (m > 0.0f) {
+        const float a = gbuf_clamped_roughness(g), a2 = xmul(a, a);
+        const float3 h = xnorm(xadd3(w, v));
+        const float n_dot_h = sat(xdot(n, h)), h_dot_v = sat(xdot(h, v));
+        if (n_dot_h > 0.0f && h_dot_v > 0.0f) {
+            const float dd = xadd(xmul(xsub(xmul(n_dot_h, a2), n_dot_h), n_dot_h), 1.0f);
+            const float dist = xdiv(a2, xmul(xmul(kPi, dd), dd));
+            pg = xdiv(xmul(dist, n_dot_h), xmul(4.0f, h_dot_v));
+        }
+    }
+    const float om = xsub(1.0f, m);
+    const float kappa = xadd(up ? xmul(xmul(om, om), 0.5f) : 0.0f, pg > 0.0f ? xmul(m, m) : 0.0f);
+    if (!(kappa > 0.0f)) return finf();
+    const float pb = xadd(up ? xmul(om, 0.15915494309189535f) : 0.0f, xmul(m, pg));
+    const float q = xadd(xmul(0.5f, pb), xmul(0.5f, env_pdf(em, w)));
+    return xdiv(q, kappa);
+}
+
 // ---- Reservoirs (reservoir.rs, reservoir/{di,gi,ephemeral,mis}.rs) ------------------------------------------
 struct DiRes { float m, w; float pdf, confidence; u32 light_id; float3 light_point; bool occluded; };
 ST_DEV DiRes di_zero() { DiRes r; r.m = 0.f; r.w = 0.f; r.pdf = 0.f; r.confidence = 0.f; r.light_id = 0u; r.light_point = f3s(0.f); r.occluded = false; return r; }

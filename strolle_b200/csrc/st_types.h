@@ -83,7 +83,14 @@ struct EnvMapDev {
     uint32_t w, h;
     float intensity;        // radiance scale
     float rotation;         // radians in [0, 2 pi), added to the azimuth
+    // ST_OPT_ENVIRONMENT_MAP_SAMPLING (DESIGN.md §2 "Environment map sampling"): the marginal CDF (h floats) followed by the h
+    // conditional CDFs (w floats each), and the marginal's last value; cdf is null (and the sampled instantiations do not run)
+    // while the option is off or the map has no distribution
+    const float* cdf;
+    float total;
 };
+// The three instantiations of the GI sampling kernels (K12, K13 and both fused) by what their sky is
+enum EnvMode { ENV_NONE = 0, ENV_MAP = 1, ENV_SAMPLED = 2 };
 
 // Per-camera device buffers: the logical buffers of
 // strolle/src/camera_controller/buffers.rs:53-339 as linear row-major float4

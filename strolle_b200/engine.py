@@ -30,6 +30,7 @@ OPT_BVH_REFIT = 15           # N > 0: up to N ticks in a row that only move inst
 OPT_LIGHT_GRID = 16          # N in 1..64: light candidates from a world-space grid of N cells along its longest axis (0 = every slot)
 OPT_TEXTURE_FILTER = 17      # 1: material textures filtered through per-image mip chains with a ray-cone level of detail (0 = nearest texel)
 OPT_TEMPORAL_AA = 18         # 1: sub-pixel camera jitter + temporal resolve in place of the composition (0 = one centred ray per pixel)
+OPT_ENVIRONMENT_MAP_SAMPLING = 19   # 1: the GI bounce and sky draw aim at the environment map's bright texels (0 = BRDF / uniform draws)
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
 STAT_WAVELET_TILED_ERRORS = 2
@@ -44,6 +45,7 @@ STAT_LIGHT_GRID_BUILDS = 10    # light grid builds (OPT_LIGHT_GRID) since the en
 STAT_TEXTURE_MIP_BUILDS = 11   # mip-chain builds (OPT_TEXTURE_FILTER) since the engine was created
 STAT_TAA_RESOLVES = 12         # temporal resolve launches (OPT_TEMPORAL_AA) since the engine was created
 STAT_ENVIRONMENT_MAP_LAUNCHES = 13   # launches of the environment-mapped kernel variants (set_environment_map) since creation
+STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14   # environment-map distribution builds (OPT_ENVIRONMENT_MAP_SAMPLING) since creation
 
 
 class StrolleError(RuntimeError):

@@ -706,3 +706,37 @@ def env_courtyard(width=320, height=180, mode=MODE_IMAGE, denoise=True, ref_dept
                projection=perspective_infinite_reverse_rh(math.pi / 3.0, width / height, 0.1))
     return dict(name="env_courtyard", meshes=meshes, materials=materials, instances=instances, lights=lights, sun=(0.0, -1.2), camera=cam,
                 environment_map=dict(rgba=courtyard_sky(), intensity=1.5, rotation=0.0))
+
+
+def sunlit_sky(width=2048, height=1024, sun_radiance=2.0e5, sun_altitude_deg=40.0, sun_u=0.3):
+    """An equirectangular test sky (height x width x 4 linear RGB, row 0 the zenith) for environment-map sampling: a dim gradient
+    (about 0.2 to 0.5 above the horizon, a dark ground below) and a sun disc 0.5 degrees across of radiance `sun_radiance` at
+    `sun_altitude_deg` and column `sun_u`.  At the defaults the disc carries about 90% of the irradiance of an open horizontal
+    surface."""
+    v = (np.arange(height, dtype=np.float64) + 0.5) / height
+    u = (np.arange(width, dtype=np.float64) + 0.5) / width
+    uu, vv = np.meshgrid(u, v)
+    alt = 0.5 - vv
+    rgb = np.where(alt[..., None] >= 0, 0.2 + 0.3 * (1.0 - 2.0 * alt[..., None]) * np.array([1.0, 0.95, 0.85]),
+                   np.array([0.04, 0.035, 0.03]))
+    theta, phi = vv * math.pi, (uu - 0.5) * 2.0 * math.pi
+    d = np.stack([np.sin(theta) * np.sin(phi), np.cos(theta), -np.sin(theta) * np.cos(phi)], -1)
+    st, sp = math.radians(90.0 - sun_altitude_deg), (sun_u - 0.5) * 2.0 * math.pi
+    s = np.array([math.sin(st) * math.sin(sp), math.cos(st), -math.sin(st) * math.cos(sp)])
+    rgb[(d @ s) >= math.cos(math.radians(0.25))] = sun_radiance * np.array([1.0, 0.96, 0.9])
+    out = np.ones((height, width, 4), np.float32)
+    out[..., :3] = rgb
+    return out
+
+
+def env_sunlit(width=320, height=180, mode=MODE_IMAGE, denoise=True, ref_depth=1, sky_width=2048, sky_height=1024):
+    """Exercises environment-map sampling (ST_OPT_ENVIRONMENT_MAP_SAMPLING): a ground plane and one occluder (a wall that casts the
+    sun's shadow), no lights, lit only by sunlit_sky (the analytic sun is below the horizon).  The camera is still."""
+    materials = {140: (material((0.6, 0.58, 0.55, 1.0)), False), 141: (material((0.7, 0.45, 0.3, 1.0), perceptual_roughness=0.5), False)}
+    meshes = {240: np.stack(_quad((-30, 0, -30), (30, 0, -30), (30, 0, 30), (-30, 0, 30), (0, 1, 0))),
+              241: np.stack(_box((-1.5, 0.0, -1.2), (1.5, 1.6, -0.9)))}
+    instances = [(340, 240, 140, IDENTITY_AFFINE), (341, 241, 141, IDENTITY_AFFINE)]
+    cam = dict(mode=mode, denoise=denoise, ref_depth=ref_depth, w=width, h=height, transform=look_at_transform((0.0, 2.2, 4.5), (0.0, 0.3, -0.5)),
+               projection=perspective_infinite_reverse_rh(math.pi / 3.0, width / height, 0.1))
+    return dict(name="env_sunlit", meshes=meshes, materials=materials, instances=instances, lights=[], sun=(0.0, -1.2), camera=cam,
+                environment_map=dict(rgba=sunlit_sky(sky_width, sky_height), intensity=1.0, rotation=0.0))

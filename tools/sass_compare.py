@@ -1,6 +1,7 @@
 """Compare per-kernel SASS of two libstrolle_b200.so builds: every kernel of the old build against the same kernel (for a kernel that
 gained `bool NMAP` / `bool LGRID` / `bool TEXF` / `bool ENVM` template parameters: its all-<false> instantiation, whose trailing
-LightGridDev, TexFilterDev and EnvMapDev arguments are unused) of the new one.  Compared: the full instruction text (opcodes,
+LightGridDev, TexFilterDev and EnvMapDev arguments are unused) of the new one.  The GI sampling kernels' ENVM is an int (EnvMode):
+0 compares as false, 1 (the map) as true, 2 (the map sampled, ST_OPT_ENVIRONMENT_MAP_SAMPLING) is new.  Compared: the full instruction text (opcodes,
 registers, immediates, constant-bank operands); normalised: the code-offset comments, branch targets and relocated symbol names."""
 import re, subprocess, sys
 
@@ -25,7 +26,7 @@ def kernels(lib):
     dem = subprocess.run(["c++filt"], input="\n".join(funcs), capture_output=True, text=True).stdout.split("\n")
     NM = ("k_prim_gbuffer", "k_gi_sampling_a", "k_ref_tracing", "k_gi_sampling_fused")                          # bool NMAP
     LG = {"k_di_sampling": 0, "k_di_sample_temporal": 0, "k_gi_sampling_b": 0, "k_ref_shading": 0, "k_gi_sampling_fused": 1}   # bool LGRID, its position
-    EM = ("k_di_resolving", "k_gi_sampling_b", "k_gi_sampling_fused", "k_ref_shading")                          # bool ENVM, the last
+    EM = ("k_di_resolving", "k_gi_sampling_a", "k_gi_sampling_b", "k_gi_sampling_fused", "k_ref_shading")       # bool / int ENVM, the last
     def base(d):
         m = re.search(r"::(\w+)<", d)
         return m.group(1) if m and (m.group(1) in NM or m.group(1) in LG or m.group(1) in EM) else None
@@ -34,6 +35,11 @@ def kernels(lib):
         k = base(d)
         if k is None: return d
         args = targs(d)
+        if "EnvMapDev)" in d and args[-1] in ("0", "1", "2"):   # int ENVM: ENV_NONE / ENV_MAP as the bool it replaced
+            args[-1] = {"0": "false", "1": "true", "2": "2"}[args[-1]]
+            head = d.split("(")[0]
+            d = head.split("<")[0] + "<" + ", ".join(args) + ">" + d[len(head):]
+            if args[-1] == "2": return d
         if "EnvMapDev)" in d:   # bool ENVM, the last template argument
             if args[-1] == "true": return d
             del args[-1]
@@ -53,7 +59,7 @@ def kernels(lib):
         name = head.split("<")[0]
         if all(a == "false" for a in args): return re.sub(r"^void ", "", name) + d[len(head):]
         return name + "<" + ", ".join(args) + ">" + d[len(head):]
-    return {norm(d): funcs[m] for d, m in zip(dem, funcs)}, {d for d in dem if base(d) and "true" in targs(d)}
+    return {norm(d): funcs[m] for d, m in zip(dem, funcs)}, {d for d in dem if base(d) and ({"true", "1", "2"} & set(targs(d)))}
 
 old, _ = kernels(sys.argv[1])
 new, nmap = kernels(sys.argv[2])
