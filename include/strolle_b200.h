@@ -125,6 +125,14 @@ int st_update_sun(st_engine* e, float azimuth, float altitude);
  * `rotation` is reduced into [0, 2 pi) in double, then rounded to f32.  Takes effect at the next st_tick, which uploads the texels;
  * ST_STAT_ENVIRONMENT_MAP_LAUNCHES counts the launches that evaluate it (DESIGN.md §2 "Environment map"). */
 int st_set_environment_map(st_engine* e, const float* rgba32f, uint32_t width, uint32_t height, float intensity, float rotation);
+/* The exposure of the tonemapped Rgba8 store (ST_OPT_TONEMAPPING, ST_OPT_AUTO_EXPOSURE), in stops: the stored value is scene value x
+ * 2^(compensation - ev).  `ev`: the manual exposure; `compensation`: added in both modes; `ev_min` <= `ev_max`: the clamp on the
+ * metered EV; `low` < `high` in [0, 1]: the metered fraction of the counted pixels (the darkest `low` and the brightest 1 - `high` are
+ * dropped); `speed_up`, `speed_down` >= 0: the largest EV change per frame, up and down.  Every field must be finite. */
+typedef struct st_exposure { float ev, compensation, ev_min, ev_max, low, high, speed_up, speed_down; } st_exposure;
+/* NULL restores the defaults {0, 0, -8, 8, 0.1, 0.9, 0.05, 1/60}.  The whole call is validated first: ST_ERR_INVALID, and no change,
+ * when a field is out of range.  Takes effect at the next st_tick. */
+int st_set_exposure(st_engine* e, const st_exposure* exposure);
 
 /* Engine::create_camera / update_camera / delete_camera (lib.rs:252-294) */
 int st_create_camera(st_engine* e, const st_camera* camera, st_camera_handle* out);
@@ -199,7 +207,24 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18, ST_OPT_ENVIRONMENT_MAP_SAMPLING = 19 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18, ST_OPT_ENVIRONMENT_MAP_SAMPLING = 19, ST_OPT_TONEMAPPING = 20, ST_OPT_AUTO_EXPOSURE = 21 };
+/* ST_OPT_TONEMAPPING (default 0; 0..4, anything else is ST_ERR_INVALID): the display transform of the Rgba8UnormSrgb store.  0 keeps
+ * today's store (clamp to [0, 1], sRGB OETF, round).  Otherwise each channel c of `output` becomes max(c, 0) (NaN -> 0) times
+ * 2^(compensation - ev), goes through T, and is then stored as at 0.  T is 1: the identity (exposure only), 2: Reinhard on luminance,
+ * x / (1 + L(x)), L = 0.2126 r + 0.7152 g + 0.0722 b, 3: ACES fitted (Hill's fit, as Bevy's AcesFitted), 4: AgX (the minimal AgX with
+ * its 6th-order contrast polynomial, output as linear light).  It applies to st_render_camera / st_copy_output with
+ * ST_FORMAT_RGBA8_SRGB and to the strip gathers; the Rgba32F frame and `output` stay the linear, scene-referred frame.
+ * CameraMode::BvhHeatmap keeps today's store.  Takes effect at the next st_tick (DESIGN.md §2 "Exposure and tonemapping"). */
+/* ST_OPT_AUTO_EXPOSURE (default 0; 1 = on, anything else is ST_ERR_INVALID; it has an effect only while ST_OPT_TONEMAPPING is not 0):
+ * each camera meters its frame and adapts its own EV instead of taking st_exposure.ev.  After the frame is composed (timed as
+ * P_COMPOSITION) a histogram of log2 L of `output` (256 bins of 1/8 stop over [-16, 16), pixels with a finite L > 0) is metered: the
+ * pixels sorted by bin, the window [floor(low N), ceil(high N)) of the N counted is kept, its mean bin centre l gives the target
+ * clamp(l - log2 0.18, ev_min, ev_max), and the EV moves toward it by at most speed_up per frame up and speed_down down (a first frame
+ * jumps to it).  The metering runs once per rendered frame: st_copy_output does not meter.  The state is allocated while the camera
+ * meters and restarts (a first frame) when metering turns on and when the camera is reallocated; st_read_buffer("exposure") returns it
+ * as 32-bit words {ev, target (f32 bits), counted, kept, frames} then the 256 bin counts of the last frame.  The heat map is not
+ * metered.  While it is on, st_render_strips and st_multi_render_camera over more than one member return ST_ERR_INVALID.
+ * ST_STAT_EXPOSURE_METERINGS counts the metering launches.  Takes effect at the next st_tick. */
 /* ST_OPT_ENVIRONMENT_MAP_SAMPLING (default 0; 1 = on, anything else is ST_ERR_INVALID): while an environment map is set
  * (st_set_environment_map), the GI bounce and the GI sky draw aim at the map's bright texels.  A tick that uploads a map with other
  * texels, or that finds the option turned on, builds on the device a distribution over the texels (weight: the largest RGB channel of
@@ -328,7 +353,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_TEXTURE_MIP_BUILDS = 11 /* mip-chain builds (ST_OPT_TEXTURE_FILTER) since creation */,
        ST_STAT_TAA_RESOLVES = 12 /* temporal resolve launches (ST_OPT_TEMPORAL_AA) since creation */,
        ST_STAT_ENVIRONMENT_MAP_LAUNCHES = 13 /* launches of the environment-mapped kernel variants (st_set_environment_map) since creation */,
-       ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14 /* environment-map distribution builds (ST_OPT_ENVIRONMENT_MAP_SAMPLING) since creation */ };
+       ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14 /* environment-map distribution builds (ST_OPT_ENVIRONMENT_MAP_SAMPLING) since creation */,
+       ST_STAT_EXPOSURE_METERINGS = 15 /* metering launches (ST_OPT_AUTO_EXPOSURE) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,
@@ -429,6 +455,7 @@ int st_multi_tick(st_multi* m);
 int st_multi_render_camera(st_multi* m, st_camera_handle camera, void* host_out, int format);
 int st_multi_synchronize(st_multi* m);
 int st_multi_set_option(st_multi* m, int option, int value);
+int st_multi_set_exposure(st_multi* m, const st_exposure* exposure);
 int st_multi_set_seed_base(st_multi* m, uint32_t base);
 int st_multi_set_blue_noise(st_multi* m, const uint8_t* rgba8_256x256);
 int st_multi_read_buffer(st_multi* m, st_camera_handle camera, const char* name, float* dst, size_t cap_floats, size_t* count);

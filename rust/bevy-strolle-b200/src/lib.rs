@@ -54,6 +54,10 @@ pub struct StrolleSun {
 /// reference's sky); put the sun (`StrolleSun`) below the horizon to light from the map alone.
 /// `environment_map_sampling`: aim the GI bounce and sky draw at the environment map's bright texels (false, the default, draws
 /// from the BRDF and the uniform hemisphere, as the reference does) - for HDRIs with a small, bright sun.
+/// `tonemapping`: expose and tonemap the frame for display (`Tonemapping::None`, the default, clamps linear light, as the reference
+/// does); with any other value the views receive `Rgba8UnormSrgb` frames instead of linear `Rgba32Float` ones.
+/// `auto_exposure`: meter each camera's frame and adapt its exposure (false, the default, takes `exposure.ev`); needs one GPU.
+/// `exposure`: the manual EV, the compensation and the metering's window, clamp and speeds.
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
@@ -63,6 +67,9 @@ pub struct StrolleSettings {
     pub temporal_aa: bool,
     pub environment_map: Option<st::EnvironmentMap>,
     pub environment_map_sampling: bool,
+    pub tonemapping: st::Tonemapping,
+    pub auto_exposure: bool,
+    pub exposure: st::Exposure,
 }
 
 #[derive(Clone, Debug)]
@@ -109,7 +116,11 @@ impl Plugin for StrollePlugin {
         engine.set_texture_filter(settings.texture_filter).expect("strolle_b200: ST_OPT_TEXTURE_FILTER");
         engine.set_temporal_aa(settings.temporal_aa).expect("strolle_b200: ST_OPT_TEMPORAL_AA");
         engine.set_environment_map_sampling(settings.environment_map_sampling).expect("strolle_b200: ST_OPT_ENVIRONMENT_MAP_SAMPLING");
+        engine.set_tonemapping(settings.tonemapping).expect("strolle_b200: ST_OPT_TONEMAPPING");
+        engine.set_auto_exposure(settings.auto_exposure).expect("strolle_b200: ST_OPT_AUTO_EXPOSURE");
+        engine.set_exposure(&settings.exposure).expect("strolle_b200: st_set_exposure");
         sync::set_environment_map(&mut engine, settings.environment_map.as_ref());
+        render_app.world.resource_mut::<sync::Synced>().tonemapped = settings.tonemapping != st::Tonemapping::None;
         render_app.insert_resource(EngineResource(engine));
     }
 }

@@ -23,6 +23,8 @@ pub(crate) struct SyncedCamera {
 #[derive(Default, Resource)]
 pub(crate) struct Synced {
     pub cameras: HashMap<Entity, SyncedCamera>,
+    /// StrolleSettings::tonemapping is set: the views receive display-referred Rgba8UnormSrgb frames
+    pub tonemapped: bool,
 }
 
 struct PendingCamera {
@@ -269,7 +271,8 @@ fn apply(mut engine: ResMut<EngineResource>, mut pending: ResMut<Pending>, mut s
         let Some((_, view)) = views.iter().find(|(e, _)| *e == cam.entity) else { continue };
         let Some(size) = view.physical_viewport_size else { continue };
         let position = view.viewport.as_ref().map(|v| v.physical_position).unwrap_or_default();
-        let viewport = st::CameraViewport { format: st::ViewportFormat::Rgba32Float, size, position };
+        let format = if synced.tonemapped { st::ViewportFormat::Rgba8UnormSrgb } else { st::ViewportFormat::Rgba32Float };
+        let viewport = st::CameraViewport { format, size, position };
         let camera = st::Camera { mode: cam.mode.unwrap_or_default(), viewport: viewport.clone(), transform: cam.transform, projection: cam.projection };
         alive.insert(cam.entity);
         match synced.cameras.get_mut(&cam.entity) {

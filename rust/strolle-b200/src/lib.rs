@@ -271,6 +271,46 @@ impl Default for CameraMode {
     }
 }
 
+/// The display transform of `Rgba8UnormSrgb` frames (`ST_OPT_TONEMAPPING`), applied after the exposure.
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub enum Tonemapping {
+    /// Linear light clamped to [0, 1] (the reference's store).
+    #[default]
+    None = 0,
+    /// The exposure only.
+    Exposure = 1,
+    /// Reinhard on luminance, x / (1 + L(x)).
+    Reinhard = 2,
+    /// Hill's fit of ACES, as Bevy's `AcesFitted`.
+    AcesFitted = 3,
+    /// The minimal AgX with its 6th-order contrast polynomial.
+    AgX = 4,
+}
+
+/// The exposure of tonemapped frames, in stops (`st_exposure`): the stored value is the scene value times 2^(compensation - ev).
+#[derive(Clone, Copy, Debug, PartialEq)]
+pub struct Exposure {
+    /// Manual exposure (auto exposure off).
+    pub ev: f32,
+    /// Added in both modes.
+    pub compensation: f32,
+    /// Clamp on the metered EV.
+    pub ev_min: f32,
+    pub ev_max: f32,
+    /// The metered fraction of the pixels: the darkest `low` and the brightest `1 - high` are dropped.
+    pub low: f32,
+    pub high: f32,
+    /// Largest EV change per frame, up and down.
+    pub speed_up: f32,
+    pub speed_down: f32,
+}
+
+impl Default for Exposure {
+    fn default() -> Self {
+        Self { ev: 0.0, compensation: 0.0, ev_min: -8.0, ev_max: 8.0, low: 0.1, high: 0.9, speed_up: 0.05, speed_down: 1.0 / 60.0 }
+    }
+}
+
 /// The two formats the engine composes into (`CameraViewport::format`, `camera.rs:170-185`)
 #[derive(Clone, Copy, Debug, PartialEq, Eq)]
 pub enum ViewportFormat {
@@ -471,6 +511,30 @@ impl<P: Params> Engine<P> {
     /// scene update.
     pub fn set_environment_map_sampling(&mut self, on: bool) -> Result<(), Error> {
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_ENVIRONMENT_MAP_SAMPLING, on as c_int) })
+    }
+
+    /// The display transform of `Rgba8UnormSrgb` frames (`ST_OPT_TONEMAPPING`; `Tonemapping::None`, the default, clamps linear light
+    /// to [0, 1], as the reference does).  `Rgba32Float` frames stay linear and scene-referred.  Takes effect with the next frame's
+    /// scene update.
+    pub fn set_tonemapping(&mut self, t: Tonemapping) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_TONEMAPPING, t as c_int) })
+    }
+
+    /// Each camera meters its frame and adapts its own EV (`ST_OPT_AUTO_EXPOSURE`; off, the default, takes `Exposure::ev`).  Has an
+    /// effect only while the tonemapping is not `Tonemapping::None`; needs an engine over one device: row strips over several refuse
+    /// to render while it is on.  Takes effect with the next frame's scene update.
+    pub fn set_auto_exposure(&mut self, on: bool) -> Result<(), Error> {
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_AUTO_EXPOSURE, on as c_int) })
+    }
+
+    /// The exposure of tonemapped frames (`st_set_exposure`); refused as a whole when a field is out of range.  Takes effect with the
+    /// next frame's scene update.
+    pub fn set_exposure(&mut self, e: &Exposure) -> Result<(), Error> {
+        let x = sys::st_exposure {
+            ev: e.ev, compensation: e.compensation, ev_min: e.ev_min, ev_max: e.ev_max, low: e.low, high: e.high, speed_up: e.speed_up,
+            speed_down: e.speed_down,
+        };
+        check(unsafe { sys::st_multi_set_exposure(self.raw, &x) })
     }
 
     /// Lights the scene from an equirectangular environment map in place of the procedural sky (`st_set_environment_map`; `None`,

@@ -385,6 +385,10 @@ static uint32_t dispatch_seed(uint32_t base, uint32_t frame, uint32_t k) {
     return (w >> 22) ^ w;
 }
 
+// st_set_exposure(e, NULL): manual EV 0, no compensation, metered EV clamped to [-8, 8] from the 10th to the 90th percentile, at most
+// 0.05 EV up and 1/60 EV down per frame
+static const ExposureDev kExposureDefaults = {0.0f, 0.0f, -8.0f, 8.0f, 0.1f, 0.9f, 0.05f, 1.0f / 60.0f};
+
 struct CameraSlot {
     bool alive = false;
     st_camera desc;
@@ -397,6 +401,7 @@ struct CameraSlot {
     DevMem svgf_pairs; float4* pair[2] = {nullptr, nullptr};   // interleaved {DI, GI} records of the wide-stride à-trous iterations (ST_OPT_WAVELET_PAIRED); private scratch, never exchanged
     DevMem rgba8; int rgba8_slot = 0;
     DevMem taa; float4* taa_hist[2] = {nullptr, nullptr};   // ST_OPT_TEMPORAL_AA history {tonemapped rgb, count}, a / b by frame parity; zero-filled
+    DevMem expo;   // ST_OPT_AUTO_EXPOSURE metering state (kExposureWords words, kernels.h), zero-filled: the next metering is a first frame
     // asynchronous RGBA8 read-back: slot k of the staging buffer is converted on the engine stream (ev_ready[k]) and copied to
     // the host on the copy stream (ev_copied[k]); the engine stream only waits for ev_copied[k] before reusing slot k
     cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
@@ -502,6 +507,10 @@ struct st_engine {
     // `envm_new_texels` = the map set since the last tick has other texels than the one before (a new intensity or rotation alone keeps
     // the distribution)
     bool envm_sampling = false, envs_built = false, envs_frame = false, envm_new_texels = false; DevMem d_envs; uint64_t envs_builds = 0;
+    // ST_OPT_TONEMAPPING / ST_OPT_AUTO_EXPOSURE / st_set_exposure: the options and settings as set, and as st_tick took them for the frame
+    int tonemapping = 0, tm_frame = 0; bool auto_exposure = false, ae_frame = false; uint64_t exposure_meterings = 0;
+    int sm_count = 0;   // multiprocessors of `device` (the histogram's grid)
+    ExposureDev exposure = kExposureDefaults, expo_frame = kExposureDefaults;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -988,6 +997,7 @@ static int allocate_camera(st_engine* e, CameraSlot* cs) {
     d.w = (int)cs->desc.width; d.h = (int)cs->desc.height; d.y0 = 0; d.y1 = d.h;
     d.own_y0 = 0; d.own_y1 = d.h; d.mirror_up = 0; d.mirror_dn = 0; d.need_rows = nullptr; d.gi_mirror_reach = 128; d.di_mirror_reach = 128;
     cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr;   // ST_OPT_TEMPORAL_AA: history restarts (allocated zeroed at the next resolve)
+    cs->expo.release();   // ST_OPT_AUTO_EXPOSURE: the next metering is a first frame
     return ST_OK;
 }
 
@@ -997,6 +1007,9 @@ static int allocate_camera(st_engine* e, CameraSlot* cs) {
 // those buffers has to travel.  All zero = every pass runs on [y0, y1).
 struct StripExt { int gbuffer = 0, variance = 0, wavelet[5] = {0, 0, 0, 0, 0}; int preview_mirror[2] = {0, 0}; bool still = false; /* nothing moved: no rows of last frame are pulled */ };
 static CameraDev grown(const CameraDev& c, int rows) { CameraDev g = c; g.y0 = std::max(0, c.y0 - rows); g.y1 = std::min(c.h, c.y1 + rows); return g; }
+// ST_OPT_AUTO_EXPOSURE: whether the camera's frames are metered (the heat map's false colours are stored as they are)
+static bool meters(const st_engine* e, const CameraSlot* cs) { return e->tm_frame != 0 && e->ae_frame && cs->desc.mode != ST_MODE_BVH_HEATMAP; }
+static int ensure_exposure_state(st_engine* e, CameraSlot* cs) { return (meters(e, cs) && !cs->expo.p) ? cs->expo.ensure(kExposureWords * 4) : ST_OK; }
 static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* steps, const StripExt* ext = nullptr) {
     GpuCamera jc, jp; float4 jit;
     const bool taa = taa_cameras(e, cs, &jc, &jp, &jit);   // ST_OPT_TEMPORAL_AA: every pass sees the jittered cameras
@@ -1020,6 +1033,11 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     const bool eson = emon && e->envs_frame;
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
     auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
+    auto meter = [&]() {   // ST_OPT_AUTO_EXPOSURE: the histogram of the frame's `output` and the adaptation, once per rendered frame
+        if (!meters(e, cs)) return;
+        uint32_t* state = (uint32_t*)cs->expo.p; const ExposureDev ep = e->expo_frame; const int sms = e->sm_count;
+        add(P_COMPOSITION, [=](cudaStream_t s) { e->exposure_meterings++; launch_exposure_histogram(cam, state, ep, sms, s); });
+    };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
     const float4* gi_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_GI_DIFFUSE)) ? cam.gi_diff_curr_colors : cam.gi_diff_samples;
     if (d.mode == ST_MODE_BVH_HEATMAP) {
@@ -1035,6 +1053,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         }
         add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, nullptr, nullptr, s); });
         add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, 6u, di_final, gi_final, s); });
+        meter();
         return;
     }
     const bool needs_di = d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE || d.mode == ST_MODE_DI_SPECULAR;
@@ -1148,9 +1167,11 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     if (taa) {   // the resolve composes the frame itself; history a / b alternate with the frame parity like the G-buffer
         const float4* hin = cs->taa_hist[cur ^ 1]; float4* hout = cs->taa_hist[cur];
         add(P_COMPOSITION, [=](cudaStream_t s) { e->taa_resolves++; launch_taa_resolve(cam, sc, cur, mode, di_final, gi_final, hin, hout, jit, s); });
+        meter();
         return;
     }
     add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, mode, di_final, gi_final, s); });
+    meter();
 }
 
 
@@ -1509,6 +1530,7 @@ int st_engine_create(int device, st_engine** out) {
     CK(cudaSetDevice(device));
     st_engine* e = new st_engine();
     e->device = device;
+    CK(cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, device));
     CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
     std::memset(&e->world, 0, sizeof e->world);
     e->h_lights.push_back(make_sun(make_float4(0, 0, 0, 25.0f), make_float4(0, 0, 0, std::numeric_limits<float>::infinity())));   // Lights::new (lights.rs:33-50)
@@ -1718,7 +1740,7 @@ int st_delete_camera(st_engine* e, st_camera_handle h) {
     if (e->copy_stream) CK(cudaStreamSynchronize(e->copy_stream));
     for (int k = 0; k < 2; k++) if (cs->side[k]) CK(cudaStreamSynchronize(cs->side[k]));
     cs->alive = false; cs->arena.release(); cs->svgf_pairs.release(); cs->pair[0] = cs->pair[1] = nullptr; cs->rgba8.release();
-    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr;
+    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr; cs->expo.release();
     return ST_OK;
 }
 int st_camera_set_strip(st_engine* e, st_camera_handle h, int y0, int y1) {
@@ -1871,6 +1893,9 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
     // ST_OPT_TEMPORAL_AA: the history exists only while the option is on, and starts over when it turns on
     if (e->temporal_aa != e->taa_frame) for (CameraSlot* c : e->cameras) { c->taa.release(); c->taa_hist[0] = c->taa_hist[1] = nullptr; }
     e->taa_frame = e->temporal_aa;
+    // ST_OPT_AUTO_EXPOSURE: the metering state exists only while the camera meters, and starts over when metering turns on
+    if ((e->tonemapping != 0 && e->auto_exposure) != (e->tm_frame != 0 && e->ae_frame)) for (CameraSlot* c : e->cameras) c->expo.release();
+    e->tm_frame = e->tonemapping; e->ae_frame = e->auto_exposure; e->expo_frame = e->exposure;
     e->frame += 1;
     if (too_deep) return fail(ST_ERR_LIMIT, "BVH deeper than the 24-entry traversal stack (strolle-gpu/src/lib.rs:72-76): the scene is not drawn until it changes");
     return ST_OK;
@@ -1900,6 +1925,7 @@ int st_render_range(st_engine* e, st_camera_handle h, int first, int last) {
     CK(cudaSetDevice(e->device));
     int rc = ensure_luts(e); if (rc) return rc;
     if ((rc = ensure_taa_history(e, cs))) return rc;
+    if ((rc = ensure_exposure_state(e, cs))) return rc;
     std::vector<Step> steps; build_schedule(e, cs, &steps);
     if (last < 0 || last >= (int)steps.size()) last = (int)steps.size() - 1;
     for (int i = std::max(first, 0); i <= last; i++) e->run_timed(steps[i].pass, steps[i].run, steps[i].sub);
@@ -1911,6 +1937,16 @@ int st_render_camera(st_engine* e, st_camera_handle h, void* host_out, int forma
     if (host_out) return st_copy_output(e, h, host_out, format);
     return ST_OK;
 }
+// The Rgba8 store of rows [cd.y0, cd.y1) into dst8: today's k_output_rgba8, or with ST_OPT_TONEMAPPING the exposed and tonemapped store
+static int store_rgba8(st_engine* e, CameraSlot* cs, const CameraDev& cd, uchar4* dst8) {
+    const SceneDev sc = e->scene();
+    const int op = cs->desc.mode == ST_MODE_BVH_HEATMAP ? 0 : e->tm_frame;
+    if (op == 0) { e->run_timed(P_COMPOSITION, [=](cudaStream_t s) { launch_output_rgba8(cd, sc, dst8, s); }); return ST_OK; }
+    int rc = ensure_exposure_state(e, cs); if (rc) return rc;
+    const uint32_t* state = meters(e, cs) ? (const uint32_t*)cs->expo.p : nullptr; const ExposureDev ep = e->expo_frame;
+    e->run_timed(P_COMPOSITION, [=](cudaStream_t s) { launch_output_display(cd, sc, op, state, ep, dst8, s); });
+    return ST_OK;
+}
 // Converts rows [y0, y1) of the composed frame to `format` and copies them to the same rows of `host_out` (a full-frame buffer).
 static int copy_rows_out(st_engine* e, CameraSlot* cs, void* host_out, int format, int y0, int y1) {
     const size_t W = cs->desc.width, n = W * cs->desc.height;
@@ -1919,14 +1955,14 @@ static int copy_rows_out(st_engine* e, CameraSlot* cs, void* host_out, int forma
     else if (format == ST_FORMAT_RGBA8_SRGB) {
         int rc2 = cs->rgba8.ensure(2 * n * 4); if (rc2) return rc2;
         cs->rgba8_slot ^= 1;
-        SceneDev sc = e->scene(); uchar4* dst8 = (uchar4*)cs->rgba8.p + (cs->rgba8_slot ? n : 0); CameraDev cd = cs->dev; cd.y0 = y0; cd.y1 = y1;
+        uchar4* dst8 = (uchar4*)cs->rgba8.p + (cs->rgba8_slot ? n : 0); CameraDev cd = cs->dev; cd.y0 = y0; cd.y1 = y1;
         const int k = cs->rgba8_slot;
         if (e->async_output) {   // conversion on the engine stream, copy on the copy stream: the next frame's passes do not queue behind the copy
             if (!e->copy_stream) CK(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
             if (!cs->ev_ready[k]) { CK(cudaEventCreateWithFlags(&cs->ev_ready[k], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&cs->ev_copied[k], cudaEventDisableTiming)); }
             else CK(cudaStreamWaitEvent(e->stream, cs->ev_copied[k], 0));   // slot k's previous copy must have left the staging buffer
         }
-        e->run_timed(P_COMPOSITION, [=](cudaStream_t s) { launch_output_rgba8(cd, sc, dst8, s); });
+        if ((rc2 = store_rgba8(e, cs, cd, dst8))) return rc2;
         if (e->async_output) {
             CK(cudaEventRecord(cs->ev_ready[k], e->stream));
             CK(cudaStreamWaitEvent(e->copy_stream, cs->ev_ready[k], 0));
@@ -1961,6 +1997,12 @@ int st_read_buffer(st_engine* e, st_camera_handle h, const char* name, float* ds
         const bool taa = taa_cameras(e, cs, &jc, &jp, &jit);   // ST_OPT_TEMPORAL_AA: the cameras the frame renders through
         const GpuCamera& c = !std::strcmp(name, "curr_camera") ? (taa ? jc : cs->dev.curr) : (taa ? jp : cs->dev.prev);
         *count = 40; if (dst) std::memcpy(dst, &c, 4 * std::min<size_t>(cap, 40)); return ST_OK;
+    }
+    if (!std::strcmp(name, "exposure")) {   // ST_OPT_AUTO_EXPOSURE: {ev, target, counted, kept, frames}, then the last frame's 256 bins
+        if (!cs->expo.p) return fail(ST_ERR_NOT_FOUND, "no exposure state: the camera does not meter (ST_OPT_TONEMAPPING and ST_OPT_AUTO_EXPOSURE)");
+        *count = 5 + kExposureBins;
+        if (dst) { CK(cudaStreamSynchronize(e->stream)); CK(cudaMemcpy(dst, cs->expo.p, 4 * std::min(cap, *count), cudaMemcpyDeviceToHost)); }
+        return ST_OK;
     }
     if (!std::strcmp(name, "taa_history_a") || !std::strcmp(name, "taa_history_b")) {
         const float4* p = cs->taa_hist[name[12] == 'a' ? 0 : 1];
@@ -2166,8 +2208,31 @@ int st_set_option(st_engine* e, int option, int value) {
         if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_TEMPORAL_AA: 0 (off) or 1 (jitter + temporal resolve)");
         e->temporal_aa = value == 1; return ST_OK;
     }
+    if (option == ST_OPT_TONEMAPPING) {   // takes effect at the next st_tick
+        if (value < 0 || value > 4) return fail(ST_ERR_INVALID, "ST_OPT_TONEMAPPING: 0 (off), 1 (exposure only), 2 (Reinhard), 3 (ACES fitted) or 4 (AgX)");
+        e->tonemapping = value; return ST_OK;
+    }
+    if (option == ST_OPT_AUTO_EXPOSURE) {   // takes effect at the next st_tick
+        if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_AUTO_EXPOSURE: 0 (manual EV) or 1 (metered)");
+        e->auto_exposure = value == 1; return ST_OK;
+    }
     if (option == ST_OPT_BVH_REFIT) { if (value < 0) return fail(ST_ERR_INVALID, "ST_OPT_BVH_REFIT: 0 or a positive budget"); e->bvh_refit = value; return ST_OK; }
     return fail(ST_ERR_INVALID, "unknown option");
+}
+static int exposure_from(const st_exposure* x, ExposureDev* out) {
+    if (!x) { *out = kExposureDefaults; return ST_OK; }
+    const float f[8] = {x->ev, x->compensation, x->ev_min, x->ev_max, x->low, x->high, x->speed_up, x->speed_down};
+    for (float v : f) if (!std::isfinite(v)) return fail(ST_ERR_INVALID, "st_set_exposure: every field must be finite");
+    if (!(x->ev_min <= x->ev_max)) return fail(ST_ERR_INVALID, "st_set_exposure: ev_min <= ev_max");
+    if (!(0.0f <= x->low && x->low < x->high && x->high <= 1.0f)) return fail(ST_ERR_INVALID, "st_set_exposure: 0 <= low < high <= 1");
+    if (!(x->speed_up >= 0.0f && x->speed_down >= 0.0f)) return fail(ST_ERR_INVALID, "st_set_exposure: speed_up, speed_down >= 0");
+    *out = {x->ev, x->compensation, x->ev_min, x->ev_max, x->low, x->high, x->speed_up, x->speed_down};
+    return ST_OK;
+}
+int st_set_exposure(st_engine* e, const st_exposure* x) {   // takes effect at the next st_tick
+    if (!e) return fail(ST_ERR_INVALID, "null engine");
+    ExposureDev v; int rc = exposure_from(x, &v); if (rc) return rc;
+    e->exposure = v; return ST_OK;
 }
 // ---- host-side BVH builder without a device (test / tool hook; strolle/src/bvh/builder.rs, serializer.rs) ----
 struct st_bvh_builder { BvhBuild b; BvhOut flat; };
@@ -2212,6 +2277,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_LIGHT_GRID_BUILDS) { *value = e->light_grid_builds; return ST_OK; }
     if (stat == ST_STAT_TEXTURE_MIP_BUILDS) { *value = e->texture_mip_builds; return ST_OK; }
     if (stat == ST_STAT_TAA_RESOLVES) { *value = e->taa_resolves; return ST_OK; }
+    if (stat == ST_STAT_EXPOSURE_METERINGS) { *value = e->exposure_meterings; return ST_OK; }
     if (stat == ST_STAT_ENVIRONMENT_MAP_LAUNCHES) { *value = e->envm_launches; return ST_OK; }
     if (stat == ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS) { *value = e->envs_builds; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
@@ -2439,10 +2505,14 @@ int st_plan_strip_order(const int* schedule, int n, int dma, char* out, size_t c
 }
 // The resolve would need the neighbours' rows of last frame's history and a composed halo row: not supported (yet) for strips
 static const char* const kTaaStripsError = "ST_OPT_TEMPORAL_AA: row strips are not supported; render the camera on one engine (st_render_camera)";
+// Metering needs the whole frame's histogram (a reduction across the strips): not supported (yet) for strips.  A fixed exposure is per pixel.
+static const char* const kAutoExposureStripsError = "ST_OPT_AUTO_EXPOSURE: row strips are not supported; use a fixed exposure or render the camera on one engine";
+static bool auto_exposure_on(const st_engine* e) { return (e->tonemapping != 0 && e->auto_exposure) || (e->tm_frame != 0 && e->ae_frame); }
 int st_render_strips(st_engine* e, st_camera_handle h, void* host_out, int format, int temporal_reach, int gather) {
     CameraSlot* cs = e ? get_camera(e, h) : nullptr;
     if (!cs) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
+    if (auto_exposure_on(e)) return fail(ST_ERR_INVALID, kAutoExposureStripsError);
     CK(cudaSetDevice(e->device));
     int rc = enqueue_strip_frame(e, cs, temporal_reach); if (rc) return rc;
     if (!gather) return ST_OK;
@@ -2461,8 +2531,8 @@ int st_render_strips(st_engine* e, st_camera_handle h, void* host_out, int forma
     else if (format == ST_FORMAT_RGBA8_SRGB) {
         if ((rc = cs->rgba8.ensure(2 * n * 4))) return rc;
         cs->rgba8_slot ^= 1;
-        SceneDev sc = e->scene(); uchar4* dst8 = (uchar4*)cs->rgba8.p + (cs->rgba8_slot ? n : 0); CameraDev cd = cs->dev;
-        e->run_timed(P_COMPOSITION, [=](cudaStream_t s) { launch_output_rgba8(cd, sc, dst8, s); });
+        uchar4* dst8 = (uchar4*)cs->rgba8.p + (cs->rgba8_slot ? n : 0); CameraDev cd = cs->dev;
+        if ((rc = store_rgba8(e, cs, cd, dst8))) return rc;
         base = (char*)dst8; px_bytes = 4; dt = ncclUint8; per_px = 4;
     } else return fail(ST_ERR_INVALID, "unsupported output format");
     if (peer) {
@@ -2600,6 +2670,10 @@ int st_multi_set_environment_map(st_multi* m, const float* rgba32f, uint32_t wid
     ST_MULTI_ALL(st_set_environment_map(e, rgba32f, width, height, intensity, rotation));
 }
 int st_multi_set_option(st_multi* m, int option, int value) { ST_MULTI_ALL(st_set_option(e, option, value)); }
+int st_multi_set_exposure(st_multi* m, const st_exposure* x) {
+    ExposureDev v; int rc = exposure_from(x, &v); if (rc) return rc;   // validated once: a refused call changes no member
+    ST_MULTI_ALL(st_set_exposure(e, x));
+}
 int st_multi_set_seed_base(st_multi* m, uint32_t base) { ST_MULTI_ALL(st_set_seed_base(e, base)); }
 int st_multi_set_blue_noise(st_multi* m, const uint8_t* rgba) { ST_MULTI_ALL(st_set_blue_noise(e, rgba)); }
 int st_multi_tick(st_multi* m) { ST_MULTI_ALL(st_tick(e)); }
@@ -2640,6 +2714,7 @@ int st_multi_render_camera(st_multi* m, st_camera_handle h, void* host_out, int 
     const size_t n = m->e.size();
     if (n == 1) return st_render_camera(m->e[0], m->cams[h][0], host_out, format);
     for (st_engine* e : m->e) if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
+    for (st_engine* e : m->e) if (auto_exposure_on(e)) return fail(ST_ERR_INVALID, kAutoExposureStripsError);
     std::vector<CameraSlot*> cs(n);
     for (size_t i = 0; i < n; i++) {   // first-use allocations and LUT generation synchronise their device: do them before anything can wait on a peer
         cs[i] = get_camera(m->e[i], m->cams[h][i]);

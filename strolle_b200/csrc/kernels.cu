@@ -1402,6 +1402,172 @@ __global__ void __launch_bounds__(ST_BLOCK) k_output_rgba8(KPARAMS, uchar4* __re
     out[i] = make_uchar4((unsigned char)q[0], (unsigned char)q[1], (unsigned char)q[2], 255);
 }
 
+// ---- ST_OPT_TONEMAPPING / ST_OPT_AUTO_EXPOSURE (DESIGN.md §2 "Exposure and tonemapping") --------------------------------------------
+// Every f32 step is one IEEE operation in the order written (strict build only); oracle_exposure/exposure.cpp restates it operation for
+// operation.  The metering's doubles use + - * / floor ceil only, which are correctly rounded on the host and the device alike.
+// The histogram's shape (DESIGN.md §4 "Exposure and tonemapping" compares the variants; tools/exposure_variants.py builds them): threads
+// per CTA, CTAs per SM, lanes merged per bin with __match_any_sync (1) or a shared atomicAdd per lane (0), the metering in the last CTA
+// (0) or in a second one-CTA launch (1).  The defaults are the fastest measured.
+#ifndef ST_EXPO_THREADS
+#define ST_EXPO_THREADS 512
+#endif
+#ifndef ST_EXPO_CTAS_PER_SM
+#define ST_EXPO_CTAS_PER_SM 4
+#endif
+#ifndef ST_EXPO_AGGREGATE
+#define ST_EXPO_AGGREGATE 1
+#endif
+#ifndef ST_EXPO_METER_LAUNCH
+#define ST_EXPO_METER_LAUNCH 0
+#endif
+#define EXPO_THREADS ST_EXPO_THREADS
+#define EXPO_WARPS (EXPO_THREADS / 32)
+ST_DEV float expo_luminance(float r, float g, float b) { return (0.2126f * r + 0.7152f * g) + 0.0722f * b; }
+// The histogram bin of luminance L (256 bins of 1/8 stop over log2 L in [-16, 16)), or -1 where the pixel does not count
+ST_DEV int expo_bin(float L) {
+    if (!(L > 0.0f) || L == finf()) return -1;
+    const float y = (log2_x(L) + 16.0f) * 8.0f;
+    return y < 0.0f ? 0 : (y >= 256.0f ? 255 : (int)y);
+}
+// The metering and adaptation of DESIGN.md §2, by one thread over the frame's 256 bin counts
+ST_DEV void expo_meter(const u32* bins, u32* state, const ExposureDev& p) {
+    unsigned long long n = 0;
+    for (int b = 0; b < kExposureBins; b++) n += bins[b];
+    const double lo = floor((double)p.low * (double)n), hi = ceil((double)p.high * (double)n);
+    double start = 0.0, kept = 0.0, sum = 0.0;
+    for (int b = 0; b < kExposureBins; b++) {
+        const double end = start + (double)bins[b];
+        const double a = start > lo ? start : lo, z = end < hi ? end : hi;
+        if (z > a) { kept = kept + (z - a); sum = sum + (z - a) * (-16.0 + ((double)b + 0.5) / 8.0); }
+        start = end;
+    }
+    const bool first = state[4] == 0u;
+    const float prev = __uint_as_float(state[0]);
+    float target;
+    if (kept > 0.0) {
+        double t = sum / kept - (-2.4739311883324122);   // - log2(0.18): an average of mid-grey meters EV 0
+        t = t < (double)p.ev_min ? (double)p.ev_min : t;
+        t = t > (double)p.ev_max ? (double)p.ev_max : t;
+        target = (float)t;
+    } else if (first) target = rclamp(0.0f, p.ev_min, p.ev_max);
+    else target = prev;
+    float ev = target;
+    if (!first) {
+        const float d = target - prev;
+        if (d > p.speed_up) ev = prev + p.speed_up;
+        else if (d < -p.speed_down) ev = prev - p.speed_down;
+    }
+    state[0] = __float_as_uint(ev); state[1] = __float_as_uint(target);
+    state[2] = (u32)n; state[3] = (u32)kept; state[4] = state[4] + 1u;
+}
+// One thread per pixel over grid-stride rounds.  Lanes of a warp that fall into one bin (a sky, a flat wall) are merged by
+// __match_any_sync and counted once, by their lowest lane, into the warp's own shared sub-histogram; each CTA then adds its non-zero
+// bins to the accumulator with one global atomic each.  The last CTA to finish (ticket after a fence) meters.
+__global__ void __launch_bounds__(EXPO_THREADS) k_exposure_histogram(const float4* __restrict__ output, u32 n, u32* __restrict__ state, ExposureDev p) {
+    __shared__ u32 s_hist[EXPO_WARPS][kExposureBins];
+    __shared__ bool s_last;
+    const u32 lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    for (u32 k = threadIdx.x; k < EXPO_WARPS * kExposureBins; k += EXPO_THREADS) (&s_hist[0][0])[k] = 0u;
+    __syncthreads();
+    for (u32 base = blockIdx.x * EXPO_THREADS; base < n; base += gridDim.x * EXPO_THREADS) {   // base is uniform: whole warps take part
+        const u32 i = base + threadIdx.x;
+        int bin = -1;
+        if (i < n) { const float4 c = output[i]; bin = expo_bin(expo_luminance(c.x, c.y, c.z)); }
+#if ST_EXPO_AGGREGATE
+        const u32 same = __match_any_sync(0xffffffffu, bin);
+        if (bin >= 0 && lane == (u32)(__ffs(same) - 1)) s_hist[warp][bin] += (u32)__popc(same);   // the warp's own row: no other writer
+        __syncwarp();
+#else
+        if (bin >= 0) atomicAdd(&s_hist[warp][bin], 1u);
+        (void)lane;
+#endif
+    }
+    __syncthreads();
+    for (u32 b = threadIdx.x; b < kExposureBins; b += EXPO_THREADS) {
+        u32 c = 0;
+#pragma unroll
+        for (int w = 0; w < EXPO_WARPS; w++) c += s_hist[w][b];
+        if (c) atomicAdd(&state[kExposureAccum + b], c);
+    }
+#if ST_EXPO_METER_LAUNCH
+    (void)s_last; (void)p;
+#else
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(&state[kExposureTicket], 1u) == gridDim.x - 1u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    u32* bins = &s_hist[0][0];   // the frame's counts; the accumulator is left zero for the next frame
+    for (u32 b = threadIdx.x; b < kExposureBins; b += EXPO_THREADS) { bins[b] = atomicExch(&state[kExposureAccum + b], 0u); state[5 + b] = bins[b]; }
+    __syncthreads();
+    if (threadIdx.x == 0) { expo_meter(bins, state, p); state[kExposureTicket] = 0u; }
+#endif
+}
+#if ST_EXPO_METER_LAUNCH
+__global__ void __launch_bounds__(kExposureBins) k_exposure_meter(u32* __restrict__ state, ExposureDev p) {
+    __shared__ u32 bins[kExposureBins];
+    bins[threadIdx.x] = state[kExposureAccum + threadIdx.x];
+    state[kExposureAccum + threadIdx.x] = 0u; state[5 + threadIdx.x] = bins[threadIdx.x];
+    __syncthreads();
+    if (threadIdx.x == 0) expo_meter(bins, state, p);
+}
+#endif
+
+// The display transforms T of ST_OPT_TONEMAPPING 2..4 (1 is the identity)
+ST_DEV float3 expo_mat(const float m[9], float3 v) {
+    return f3((m[0] * v.x + m[1] * v.y) + m[2] * v.z, (m[3] * v.x + m[4] * v.y) + m[5] * v.z, (m[6] * v.x + m[7] * v.y) + m[8] * v.z);
+}
+ST_DEV float expo_aces_rrt_odt(float v) { return (v * (v + 0.0245786f) - 0.000090537f) / (v * (0.983729f * v + 0.4329510f) + 0.238081f); }
+ST_DEV float expo_agx_curve(float v) {
+    float l = v > 0.0f ? log2_x(v) : -12.47393f;
+    l = l < -12.47393f ? -12.47393f : l;
+    l = l > 4.026069f ? 4.026069f : l;
+    const float x = (l + 12.47393f) / 16.499999f;
+    const float x2 = x * x, x4 = x2 * x2;
+    return (((((15.5f * x4 * x2 - 40.14f * x4 * x) + 31.96f * x4) - 6.868f * x2 * x) + 0.4298f * x2) + 0.1191f * x) - 0.00232f;
+}
+template <int OP>
+ST_DEV float3 expo_transform(float3 x) {
+    if (OP == 2) { const float d = 1.0f + expo_luminance(x.x, x.y, x.z); return f3(x.x / d, x.y / d, x.z / d); }
+    if (OP == 3) {
+        const float A[9] = {0.59719f, 0.35458f, 0.04823f, 0.07600f, 0.90834f, 0.01566f, 0.02840f, 0.13383f, 0.83777f};
+        const float B[9] = {1.60475f, -0.53108f, -0.07367f, -0.10208f, 1.10813f, -0.00605f, -0.00327f, -0.07276f, 1.07602f};
+        const float3 v = expo_mat(A, x);
+        return expo_mat(B, f3(expo_aces_rrt_odt(v.x), expo_aces_rrt_odt(v.y), expo_aces_rrt_odt(v.z)));
+    }
+    if (OP == 4) {
+        const float M[9] = {0.842479062253094f, 0.0784335999999992f, 0.0792237451477643f, 0.0423282422610123f, 0.878468636469772f, 0.0791661274605434f,
+                            0.0423756549057051f, 0.0784336f, 0.879142973793104f};
+        const float MI[9] = {1.19687900512017f, -0.0980208811401368f, -0.0990297440797205f, -0.0528968517574562f, 1.15190312990417f, -0.0989611768448433f,
+                             -0.0529716355144438f, -0.0980434501171241f, 1.15107367264116f};
+        const float3 v = expo_mat(M, x);
+        const float3 u = expo_mat(MI, f3(expo_agx_curve(v.x), expo_agx_curve(v.y), expo_agx_curve(v.z)));
+        return f3(pow_det(u.x > 0.0f ? u.x : 0.0f, 2.2f), pow_det(u.y > 0.0f ? u.y : 0.0f, 2.2f), pow_det(u.z > 0.0f ? u.z : 0.0f, 2.2f));
+    }
+    return x;
+}
+// The Rgba8UnormSrgb store of k_output_rgba8 after exposure and T
+template <int OP>
+__global__ void __launch_bounds__(ST_BLOCK) k_output_display(KPARAMS, uchar4* __restrict__ out, const u32* __restrict__ state, ExposureDev ep) {
+    Px p = pixel_full(cam);
+    if (!p.in) return;
+    size_t i = pix(cam, p.x, p.y);
+    const float ev = state ? __uint_as_float(state[0]) : ep.ev;
+    const float s = pow_det(2.0f, ep.compensation - ev);
+    const float4 c = cam.output[i];
+    const float3 t = expo_transform<OP>(f3((c.x > 0.0f ? c.x : 0.0f) * s, (c.y > 0.0f ? c.y : 0.0f) * s, (c.z > 0.0f ? c.z : 0.0f) * s));
+    float v[3] = {t.x, t.y, t.z};
+    u32 q[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        float x = sat(v[k]);
+        float e = (x <= 0.0031308f) ? 12.92f * x : 1.055f * pow_det(x, 1.0f / 2.4f) - 0.055f;
+        q[k] = to_u32_sat(sat(e) * 255.0f + 0.5f);
+    }
+    out[i] = make_uchar4((unsigned char)q[0], (unsigned char)q[1], (unsigned char)q[2], 255);
+}
+
 // K1 ref_tracing::main (ref_tracing.rs:4-60); NMAP: the packed normal is the mapped one, which K2 shades with and nudges along
 template <bool NMAP>
 __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
@@ -2095,6 +2261,22 @@ void launch_taa_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 mode
     k_taa_resolve<<<grid, TAA_TW * TAA_TH, 0, st>>>(c, s, cur, mode, di_diff, gi_diff, hist_in, hist_out, jit);
 }
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st) { k_output_rgba8<<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out); }
+void launch_exposure_histogram(const CameraDev& c, u32* state, ExposureDev p, int sms, cudaStream_t st) {
+    const u32 n = (u32)c.w * (u32)c.h;
+    const u32 ctas = std::max(1u, std::min((n + EXPO_THREADS - 1) / EXPO_THREADS, (u32)ST_EXPO_CTAS_PER_SM * (u32)sms));
+    k_exposure_histogram<<<ctas, EXPO_THREADS, 0, st>>>(c.output, n, state, p);
+#if ST_EXPO_METER_LAUNCH
+    k_exposure_meter<<<1, kExposureBins, 0, st>>>(state, p);
+#endif
+}
+void launch_output_display(const CameraDev& c, const SceneDev& s, int op, const u32* state, ExposureDev p, uchar4* out, cudaStream_t st) {
+    switch (op) {
+    case 1: k_output_display<1><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p); break;
+    case 2: k_output_display<2><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p); break;
+    case 3: k_output_display<3><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p); break;
+    default: k_output_display<4><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p); break;
+    }
+}
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {
     if (nmap) k_ref_tracing<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); else k_ref_tracing<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth);
 }

@@ -44,6 +44,17 @@ void launch_composition(const CameraDev& c, const SceneDev& s, int cur, u32 mode
 void launch_taa_resolve(const CameraDev& c, const SceneDev& s, int cur, u32 mode, const float4* di_diff, const float4* gi_diff, const float4* hist_in, float4* hist_out,
                         float4 jit, cudaStream_t st);
 void launch_output_rgba8(const CameraDev& c, const SceneDev& s, uchar4* out, cudaStream_t st);
+// ST_OPT_TONEMAPPING / ST_OPT_AUTO_EXPOSURE (DESIGN.md §2 "Exposure and tonemapping"; strict build only).  The per-camera metering state,
+// 32-bit words: {ev, target (f32 bits), counted, kept, frames}, the 256 bins of the last metered frame, the last-CTA ticket, then (at
+// kExposureAccum) the 256 bins the next histogram accumulates into, zero between launches.
+struct ExposureDev { float ev, compensation, ev_min, ev_max, low, high, speed_up, speed_down; };
+enum { kExposureBins = 256, kExposureTicket = 5 + kExposureBins, kExposureAccum = 264, kExposureWords = kExposureAccum + kExposureBins };
+// The log-luminance histogram of c.output (the whole frame) into state[kExposureAccum ..] over a grid sized from the device's `sms`
+// multiprocessors; the last CTA to finish meters it, adapts the EV (state[0]) and zeroes the accumulator and the ticket for the next frame.
+void launch_exposure_histogram(const CameraDev& c, u32* state, ExposureDev p, int sms, cudaStream_t st);
+// The Rgba8 store of rows [c.y0, c.y1) through exposure 2^(compensation - ev) and the display transform `op` (1..4); ev = state[0]
+// when `state` is non-null (auto exposure), p.ev otherwise
+void launch_output_display(const CameraDev& c, const SceneDev& s, int op, const u32* state, ExposureDev p, uchar4* out, cudaStream_t st);
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st);
 void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, const EnvMapDev* em, cudaStream_t st);
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st);

@@ -31,6 +31,9 @@ OPT_LIGHT_GRID = 16          # N in 1..64: light candidates from a world-space g
 OPT_TEXTURE_FILTER = 17      # 1: material textures filtered through per-image mip chains with a ray-cone level of detail (0 = nearest texel)
 OPT_TEMPORAL_AA = 18         # 1: sub-pixel camera jitter + temporal resolve in place of the composition (0 = one centred ray per pixel)
 OPT_ENVIRONMENT_MAP_SAMPLING = 19   # 1: the GI bounce and sky draw aim at the environment map's bright texels (0 = BRDF / uniform draws)
+OPT_TONEMAPPING = 20         # Rgba8 display transform: 0 off (today's store), 1 exposure only, 2 Reinhard, 3 ACES fitted, 4 AgX
+OPT_AUTO_EXPOSURE = 21       # 1: each camera meters its frame and adapts its EV (0 = the manual ev of set_exposure); needs OPT_TONEMAPPING
+TONEMAP_OFF, TONEMAP_EXPOSURE, TONEMAP_REINHARD, TONEMAP_ACES, TONEMAP_AGX = 0, 1, 2, 3, 4
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
 STAT_WAVELET_TILED_ERRORS = 2
@@ -46,6 +49,7 @@ STAT_TEXTURE_MIP_BUILDS = 11   # mip-chain builds (OPT_TEXTURE_FILTER) since the
 STAT_TAA_RESOLVES = 12         # temporal resolve launches (OPT_TEMPORAL_AA) since the engine was created
 STAT_ENVIRONMENT_MAP_LAUNCHES = 13   # launches of the environment-mapped kernel variants (set_environment_map) since creation
 STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14   # environment-map distribution builds (OPT_ENVIRONMENT_MAP_SAMPLING) since creation
+STAT_EXPOSURE_METERINGS = 15   # metering launches (OPT_AUTO_EXPOSURE) since creation
 
 
 class StrolleError(RuntimeError):
@@ -75,6 +79,31 @@ class _Light(C.Structure):
                 ("direction", C.c_float * 3), ("angle", C.c_float)]
 
 
+class _Exposure(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("ev", "compensation", "ev_min", "ev_max", "low", "high", "speed_up", "speed_down")]
+
+
+EXPOSURE_DEFAULTS = dict(ev=0.0, compensation=0.0, ev_min=-8.0, ev_max=8.0, low=0.1, high=0.9, speed_up=0.05, speed_down=1.0 / 60.0)
+
+
+def _exposure(fields):
+    """st_exposure from keyword fields over the defaults; None (no fields) stands for NULL."""
+    if fields is None:
+        return None
+    unknown = set(fields) - set(EXPOSURE_DEFAULTS)
+    if unknown:
+        raise TypeError(f"set_exposure: unknown fields {sorted(unknown)}")
+    v = dict(EXPOSURE_DEFAULTS, **fields)
+    return C.byref(_Exposure(*[v[n] for n, _ in _Exposure._fields_]))
+
+
+def parse_exposure(words):
+    """read_buffer(cam, "exposure") as a dict: ev, target (float32), counted, kept, frames and the 256 bins of the last frame."""
+    w = np.asarray(words, np.float32).view(np.uint32)
+    return dict(ev=w[0:1].view(np.float32)[0], target=w[1:2].view(np.float32)[0], counted=int(w[2]), kept=int(w[3]), frames=int(w[4]),
+                bins=w[5:261].astype(np.int64))
+
+
 class _Camera(C.Structure):
     _fields_ = [("mode", C.c_int32), ("denoise", C.c_int32), ("ref_depth", C.c_int32), ("width", C.c_uint32), ("height", C.c_uint32),
                 ("transform", C.c_float * 16), ("projection", C.c_float * 16)]
@@ -100,7 +129,7 @@ def load_library():
         "st_insert_image": [P, u64, C.c_void_p, u32, u32], "st_remove_image": [P, u64], "st_set_material_textures": [P, u64, C.POINTER(_MaterialTextures)],
         "st_insert_instance": [P, u64, u64, u64, f32p], "st_remove_instance": [P, u64],
         "st_insert_light": [P, u64, C.POINTER(_Light)], "st_remove_light": [P, u64], "st_update_sun": [P, C.c_float, C.c_float],
-        "st_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float],
+        "st_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_set_exposure": [P, C.c_void_p],
         "st_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_update_camera": [P, i32, C.POINTER(_Camera)], "st_delete_camera": [P, i32],
         "st_tick": [P], "st_render_camera": [P, i32, P, C.c_int], "st_copy_output": [P, i32, P, C.c_int], "st_synchronize": [P],
         "st_set_seed_base": [P, u32], "st_set_blue_noise": [P, C.c_void_p],
@@ -130,7 +159,7 @@ def load_library():
         "st_multi_insert_image": [P, u64, C.c_void_p, u32, u32], "st_multi_remove_image": [P, u64], "st_multi_set_material_textures": [P, u64, C.POINTER(_MaterialTextures)],
         "st_multi_insert_instance": [P, u64, u64, u64, f32p], "st_multi_remove_instance": [P, u64],
         "st_multi_insert_light": [P, u64, C.POINTER(_Light)], "st_multi_remove_light": [P, u64], "st_multi_update_sun": [P, C.c_float, C.c_float],
-        "st_multi_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float],
+        "st_multi_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_multi_set_exposure": [P, C.c_void_p],
         "st_multi_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_multi_update_camera": [P, i32, C.POINTER(_Camera)], "st_multi_delete_camera": [P, i32],
         "st_multi_tick": [P], "st_multi_render_camera": [P, i32, P, C.c_int], "st_multi_synchronize": [P],
         "st_multi_set_option": [P, C.c_int, C.c_int], "st_multi_set_seed_base": [P, u32], "st_multi_set_blue_noise": [P, C.c_void_p],
@@ -324,6 +353,12 @@ class Engine:
         t = _envmap_texels(rgba)
         w, h = (0, 0) if t is None else (t.shape[1], t.shape[0])
         self._check(self.lib.st_set_environment_map(self._h, None if t is None else t.ctypes.data, w, h, intensity, rotation))
+
+    def set_exposure(self, **fields):
+        """The exposure of the tonemapped Rgba8 store, from the next tick: ev, compensation, ev_min, ev_max, low, high, speed_up,
+        speed_down (fields not given take their defaults, EXPOSURE_DEFAULTS; no fields restores them all).  Refused as a whole when a
+        field is out of range (include/strolle_b200.h st_set_exposure)."""
+        self._check(self.lib.st_set_exposure(self._h, _exposure(fields or None)))
 
     # ---- cameras ----------------------------------------------------------------------------
     @staticmethod
@@ -615,6 +650,9 @@ class MultiEngine:
 
     def set_option(self, option, value):
         self._check(self.lib.st_multi_set_option(self._h, option, int(value)))
+
+    def set_exposure(self, **fields):
+        self._check(self.lib.st_multi_set_exposure(self._h, _exposure(fields or None)))
 
     def read_buffer(self, cam, name):
         """The whole frame's buffer, each strip read from the member that owns it."""
