@@ -133,6 +133,15 @@ typedef struct st_exposure { float ev, compensation, ev_min, ev_max, low, high, 
 /* NULL restores the defaults {0, 0, -8, 8, 0.1, 0.9, 0.05, 1/60}.  The whole call is validated first: ST_ERR_INVALID, and no change,
  * when a field is out of range.  Takes effect at the next st_tick. */
 int st_set_exposure(st_engine* e, const st_exposure* exposure);
+/* The glow of ST_OPT_BLOOM (DESIGN.md §2 "Bloom").  `intensity`: the glow's share of the stored value, in [0, 1] with `mode` 0
+ * (energy-conserving: (1 - intensity) x + intensity B) or >= 0 with `mode` 1 (additive: x + intensity B); `scatter` in [0, 1]: how far
+ * the glow spreads (level k of the pyramid weighs (1 - scatter) scatter^k, the last level scatter^(L-1)); `threshold` >= 0: the exposed
+ * brightness max(r, g, b) where the glow starts (0: every pixel glows), with a soft knee of width threshold x `softness`, `softness` in
+ * [0, 1]; `levels` in 1..8: the pyramid's depth L, level 0 at half resolution.  Every float field must be finite. */
+typedef struct st_bloom { float intensity, scatter, threshold, softness; int32_t levels, mode; } st_bloom;
+/* NULL restores the defaults {0.15, 0.7, 0, 0, 7, 0}.  The whole call is validated first: ST_ERR_INVALID, and no change, when a field
+ * is out of range.  Takes effect at the next st_tick. */
+int st_set_bloom(st_engine* e, const st_bloom* bloom);
 
 /* Engine::create_camera / update_camera / delete_camera (lib.rs:252-294) */
 int st_create_camera(st_engine* e, const st_camera* camera, st_camera_handle* out);
@@ -207,7 +216,22 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18, ST_OPT_ENVIRONMENT_MAP_SAMPLING = 19, ST_OPT_TONEMAPPING = 20, ST_OPT_AUTO_EXPOSURE = 21 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18, ST_OPT_ENVIRONMENT_MAP_SAMPLING = 19, ST_OPT_TONEMAPPING = 20, ST_OPT_AUTO_EXPOSURE = 21, ST_OPT_BLOOM = 22 };
+/* ST_OPT_BLOOM (default 0; 1 = on, anything else is ST_ERR_INVALID): the Rgba8UnormSrgb store gains a glow around bright light
+ * (st_set_bloom).  After the frame is composed and metered (timed as P_COMPOSITION), once per rendered frame, a pyramid of `output` is
+ * built: each channel cleared to 0 where it is not finite and > 0, times the exposure 2^(compensation - ev) while ST_OPT_TONEMAPPING is
+ * not 0 (1 otherwise), through the soft-knee threshold, then L levels down (Jimenez's 13-tap filter, Karis-weighted on the first) and
+ * back up (3 x 3 tent).  The store composites the glow B of level 0, brought to full resolution by the same tent, into the value it
+ * would store (mode 0: (1 - intensity) x + intensity B, mode 1: x + intensity B), before T and today's store; st_copy_output
+ * composites from the stored pyramid and never rebuilds it.  It applies to st_render_camera / st_copy_output with
+ * ST_FORMAT_RGBA8_SRGB and the one-member st_multi_render_camera, with every ST_OPT_TONEMAPPING value; the Rgba32F frame and `output`
+ * stay the linear, scene-referred frame, and CameraMode::BvhHeatmap is not bloomed.  The pyramid is allocated (zero-filled: a copy
+ * before the first pyramid composites no glow) while the camera blooms, freed when the option turns off, and reallocated when the
+ * camera is reallocated or `levels` changes.  st_read_buffer("bloom") returns it as the last rendered frame left it, as 32-bit words:
+ * {L, w_0, h_0, .., w_7, h_7, 0, 0, 0} (level k is max(1, W >> (k + 1)) x max(1, H >> (k + 1)); zero past level L - 1), then
+ * {r, g, b, 0} float texels, row-major: the down levels 0 .. L - 1, then the up levels 0 .. L - 2 (up_{L-1} is down_{L-1}).
+ * While it is on, as set or as taken by the last st_tick, st_render_strips and st_multi_render_camera over more than one member return
+ * ST_ERR_INVALID.  ST_STAT_BLOOM_PYRAMIDS counts the pyramid builds.  Takes effect at the next st_tick. */
 /* ST_OPT_TONEMAPPING (default 0; 0..4, anything else is ST_ERR_INVALID): the display transform of the Rgba8UnormSrgb store.  0 keeps
  * today's store (clamp to [0, 1], sRGB OETF, round).  Otherwise each channel c of `output` becomes max(c, 0) (NaN -> 0) times
  * 2^(compensation - ev), goes through T, and is then stored as at 0.  T is 1: the identity (exposure only), 2: Reinhard on luminance,
@@ -354,7 +378,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_TAA_RESOLVES = 12 /* temporal resolve launches (ST_OPT_TEMPORAL_AA) since creation */,
        ST_STAT_ENVIRONMENT_MAP_LAUNCHES = 13 /* launches of the environment-mapped kernel variants (st_set_environment_map) since creation */,
        ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14 /* environment-map distribution builds (ST_OPT_ENVIRONMENT_MAP_SAMPLING) since creation */,
-       ST_STAT_EXPOSURE_METERINGS = 15 /* metering launches (ST_OPT_AUTO_EXPOSURE) since creation */ };
+       ST_STAT_EXPOSURE_METERINGS = 15 /* metering launches (ST_OPT_AUTO_EXPOSURE) since creation */,
+       ST_STAT_BLOOM_PYRAMIDS = 16 /* pyramid builds (ST_OPT_BLOOM) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,
@@ -456,6 +481,7 @@ int st_multi_render_camera(st_multi* m, st_camera_handle camera, void* host_out,
 int st_multi_synchronize(st_multi* m);
 int st_multi_set_option(st_multi* m, int option, int value);
 int st_multi_set_exposure(st_multi* m, const st_exposure* exposure);
+int st_multi_set_bloom(st_multi* m, const st_bloom* bloom);
 int st_multi_set_seed_base(st_multi* m, uint32_t base);
 int st_multi_set_blue_noise(st_multi* m, const uint8_t* rgba8_256x256);
 int st_multi_read_buffer(st_multi* m, st_camera_handle camera, const char* name, float* dst, size_t cap_floats, size_t* count);

@@ -58,6 +58,8 @@ pub struct StrolleSun {
 /// does); with any other value the views receive `Rgba8UnormSrgb` frames instead of linear `Rgba32Float` ones.
 /// `auto_exposure`: meter each camera's frame and adapt its exposure (false, the default, takes `exposure.ev`); needs one GPU.
 /// `exposure`: the manual EV, the compensation and the metering's window, clamp and speeds.
+/// `bloom`: a glow around light brighter than the display shows (None, the default, stores no glow); with `Some` the views receive
+/// `Rgba8UnormSrgb` frames, with or without tonemapping; needs one GPU.
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
@@ -70,6 +72,7 @@ pub struct StrolleSettings {
     pub tonemapping: st::Tonemapping,
     pub auto_exposure: bool,
     pub exposure: st::Exposure,
+    pub bloom: Option<st::Bloom>,
 }
 
 #[derive(Clone, Debug)]
@@ -119,8 +122,9 @@ impl Plugin for StrollePlugin {
         engine.set_tonemapping(settings.tonemapping).expect("strolle_b200: ST_OPT_TONEMAPPING");
         engine.set_auto_exposure(settings.auto_exposure).expect("strolle_b200: ST_OPT_AUTO_EXPOSURE");
         engine.set_exposure(&settings.exposure).expect("strolle_b200: st_set_exposure");
+        engine.set_bloom(settings.bloom.as_ref()).expect("strolle_b200: st_set_bloom");
         sync::set_environment_map(&mut engine, settings.environment_map.as_ref());
-        render_app.world.resource_mut::<sync::Synced>().tonemapped = settings.tonemapping != st::Tonemapping::None;
+        render_app.world.resource_mut::<sync::Synced>().tonemapped = settings.tonemapping != st::Tonemapping::None || settings.bloom.is_some();
         render_app.insert_resource(EngineResource(engine));
     }
 }

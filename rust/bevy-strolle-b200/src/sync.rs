@@ -23,7 +23,7 @@ pub(crate) struct SyncedCamera {
 #[derive(Default, Resource)]
 pub(crate) struct Synced {
     pub cameras: HashMap<Entity, SyncedCamera>,
-    /// StrolleSettings::tonemapping is set: the views receive display-referred Rgba8UnormSrgb frames
+    /// StrolleSettings::tonemapping or StrolleSettings::bloom is set: the views receive display-referred Rgba8UnormSrgb frames
     pub tonemapped: bool,
 }
 

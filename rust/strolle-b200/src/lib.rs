@@ -311,6 +311,39 @@ impl Default for Exposure {
     }
 }
 
+/// How the glow enters the stored value (`st_bloom::mode`).
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub enum BloomMode {
+    /// (1 - intensity) x + intensity B: a constant frame stays constant; `intensity` in [0, 1].
+    #[default]
+    EnergyConserving = 0,
+    /// x + intensity B; `intensity` >= 0.
+    Additive = 1,
+}
+
+/// The glow around bright light in `Rgba8UnormSrgb` frames (`st_bloom`, `ST_OPT_BLOOM`): a downsample / upsample pyramid of the
+/// exposed frame, composited before the display transform.
+#[derive(Clone, Copy, Debug, PartialEq)]
+pub struct Bloom {
+    /// The glow's share of the stored value.
+    pub intensity: f32,
+    /// How far the glow spreads, in [0, 1]: level k of the pyramid weighs (1 - scatter) scatter^k.
+    pub scatter: f32,
+    /// The exposed brightness (largest channel) where the glow starts; 0 lets every pixel glow.
+    pub threshold: f32,
+    /// The soft knee's width as a fraction of the threshold, in [0, 1].
+    pub softness: f32,
+    /// The pyramid's depth, 1..=8; level 0 is half resolution.
+    pub levels: i32,
+    pub mode: BloomMode,
+}
+
+impl Default for Bloom {
+    fn default() -> Self {
+        Self { intensity: 0.15, scatter: 0.7, threshold: 0.0, softness: 0.0, levels: 7, mode: BloomMode::EnergyConserving }
+    }
+}
+
 /// The two formats the engine composes into (`CameraViewport::format`, `camera.rs:170-185`)
 #[derive(Clone, Copy, Debug, PartialEq, Eq)]
 pub enum ViewportFormat {
@@ -535,6 +568,20 @@ impl<P: Params> Engine<P> {
             speed_down: e.speed_down,
         };
         check(unsafe { sys::st_multi_set_exposure(self.raw, &x) })
+    }
+
+    /// A glow around bright light in `Rgba8UnormSrgb` frames (`ST_OPT_BLOOM` and `st_set_bloom`; `None`, the default, stores no glow).
+    /// It works with every tonemapping, `Tonemapping::None` included; `Rgba32Float` frames stay linear and without glow.  Needs an
+    /// engine over one device: row strips over several refuse to render while it is on.  Refused as a whole when a field is out of
+    /// range.  Takes effect with the next frame's scene update.
+    pub fn set_bloom(&mut self, bloom: Option<&Bloom>) -> Result<(), Error> {
+        if let Some(b) = bloom {
+            let x = sys::st_bloom {
+                intensity: b.intensity, scatter: b.scatter, threshold: b.threshold, softness: b.softness, levels: b.levels, mode: b.mode as i32,
+            };
+            check(unsafe { sys::st_multi_set_bloom(self.raw, &x) })?;
+        }
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_BLOOM, bloom.is_some() as c_int) })
     }
 
     /// Lights the scene from an equirectangular environment map in place of the procedural sky (`st_set_environment_map`; `None`,

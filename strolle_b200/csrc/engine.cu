@@ -388,6 +388,8 @@ static uint32_t dispatch_seed(uint32_t base, uint32_t frame, uint32_t k) {
 // st_set_exposure(e, NULL): manual EV 0, no compensation, metered EV clamped to [-8, 8] from the 10th to the 90th percentile, at most
 // 0.05 EV up and 1/60 EV down per frame
 static const ExposureDev kExposureDefaults = {0.0f, 0.0f, -8.0f, 8.0f, 0.1f, 0.9f, 0.05f, 1.0f / 60.0f};
+// st_set_bloom(e, NULL): 15 % energy-conserving glow, scatter 0.7, no threshold, 7 levels
+static const BloomDev kBloomDefaults = {0.15f, 0.7f, 0.0f, 0.0f, 7, 0};
 
 struct CameraSlot {
     bool alive = false;
@@ -402,6 +404,7 @@ struct CameraSlot {
     DevMem rgba8; int rgba8_slot = 0;
     DevMem taa; float4* taa_hist[2] = {nullptr, nullptr};   // ST_OPT_TEMPORAL_AA history {tonemapped rgb, count}, a / b by frame parity; zero-filled
     DevMem expo;   // ST_OPT_AUTO_EXPOSURE metering state (kExposureWords words, kernels.h), zero-filled: the next metering is a first frame
+    DevMem bloom;  // ST_OPT_BLOOM pyramid (bloom_layout, kernels.h), zero-filled: a store before the first pyramid composites no glow
     // asynchronous RGBA8 read-back: slot k of the staging buffer is converted on the engine stream (ev_ready[k]) and copied to
     // the host on the copy stream (ev_copied[k]); the engine stream only waits for ev_copied[k] before reusing slot k
     cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
@@ -511,6 +514,8 @@ struct st_engine {
     int tonemapping = 0, tm_frame = 0; bool auto_exposure = false, ae_frame = false; uint64_t exposure_meterings = 0;
     int sm_count = 0;   // multiprocessors of `device` (the histogram's grid)
     ExposureDev exposure = kExposureDefaults, expo_frame = kExposureDefaults;
+    // ST_OPT_BLOOM / st_set_bloom: the option and settings as set, and as st_tick took them for the frame
+    bool bloom = false, bloom_frame = false; BloomDev bloom_set = kBloomDefaults, bloom_cfg = kBloomDefaults; uint64_t bloom_pyramids = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -998,6 +1003,7 @@ static int allocate_camera(st_engine* e, CameraSlot* cs) {
     d.own_y0 = 0; d.own_y1 = d.h; d.mirror_up = 0; d.mirror_dn = 0; d.need_rows = nullptr; d.gi_mirror_reach = 128; d.di_mirror_reach = 128;
     cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr;   // ST_OPT_TEMPORAL_AA: history restarts (allocated zeroed at the next resolve)
     cs->expo.release();   // ST_OPT_AUTO_EXPOSURE: the next metering is a first frame
+    cs->bloom.release();  // ST_OPT_BLOOM: the pyramid is reallocated (zeroed) at the new size
     return ST_OK;
 }
 
@@ -1010,6 +1016,21 @@ static CameraDev grown(const CameraDev& c, int rows) { CameraDev g = c; g.y0 = s
 // ST_OPT_AUTO_EXPOSURE: whether the camera's frames are metered (the heat map's false colours are stored as they are)
 static bool meters(const st_engine* e, const CameraSlot* cs) { return e->tm_frame != 0 && e->ae_frame && cs->desc.mode != ST_MODE_BVH_HEATMAP; }
 static int ensure_exposure_state(st_engine* e, CameraSlot* cs) { return (meters(e, cs) && !cs->expo.p) ? cs->expo.ensure(kExposureWords * 4) : ST_OK; }
+// ST_OPT_BLOOM: whether the camera's Rgba8 frames are bloomed (not the heat map's), and its pyramid's levels
+static bool blooms(const st_engine* e, const CameraSlot* cs) { return e->bloom_frame && cs->desc.mode != ST_MODE_BVH_HEATMAP; }
+static BloomLevels bloom_levels(const st_engine* e, const CameraSlot* cs) {
+    BloomLevels lv; bloom_layout((int)cs->desc.width, (int)cs->desc.height, e->bloom_cfg.levels, cs->bloom.p, &lv); return lv;
+}
+static int ensure_bloom_state(st_engine* e, CameraSlot* cs) {
+    if (!blooms(e, cs) || cs->bloom.p) return ST_OK;
+    BloomLevels lv;
+    int rc = cs->bloom.ensure(bloom_layout((int)cs->desc.width, (int)cs->desc.height, e->bloom_cfg.levels, nullptr, &lv)); if (rc) return rc;
+    uint32_t head[kBloomHeaderWords] = {};
+    head[0] = (uint32_t)lv.levels;
+    for (int k = 0; k < lv.levels; k++) { head[1 + 2 * k] = (uint32_t)lv.w[k]; head[2 + 2 * k] = (uint32_t)lv.h[k]; }
+    CK(cudaMemcpy(cs->bloom.p, head, sizeof head, cudaMemcpyHostToDevice));   // the allocation synchronised the device: nothing reads it yet
+    return ST_OK;
+}
 static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* steps, const StripExt* ext = nullptr) {
     GpuCamera jc, jp; float4 jit;
     const bool taa = taa_cameras(e, cs, &jc, &jp, &jit);   // ST_OPT_TEMPORAL_AA: every pass sees the jittered cameras
@@ -1038,6 +1059,12 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         uint32_t* state = (uint32_t*)cs->expo.p; const ExposureDev ep = e->expo_frame; const int sms = e->sm_count;
         add(P_COMPOSITION, [=](cudaStream_t s) { e->exposure_meterings++; launch_exposure_histogram(cam, state, ep, sms, s); });
     };
+    auto pyramid = [&]() {   // ST_OPT_BLOOM: the pyramid of the frame's `output`, after the metering, once per rendered frame
+        if (!blooms(e, cs)) return;
+        const BloomLevels lv = bloom_levels(e, cs); const uint32_t* state = meters(e, cs) ? (const uint32_t*)cs->expo.p : nullptr;
+        const ExposureDev ep = e->expo_frame; const int tm = e->tm_frame; const BloomDev bp = e->bloom_cfg;
+        add(P_COMPOSITION, [=](cudaStream_t s) { e->bloom_pyramids++; launch_bloom_pyramid(cam, lv, state, ep, tm, bp, s); });
+    };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
     const float4* gi_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_GI_DIFFUSE)) ? cam.gi_diff_curr_colors : cam.gi_diff_samples;
     if (d.mode == ST_MODE_BVH_HEATMAP) {
@@ -1053,7 +1080,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         }
         add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, nullptr, nullptr, s); });
         add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, 6u, di_final, gi_final, s); });
-        meter();
+        meter(); pyramid();
         return;
     }
     const bool needs_di = d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE || d.mode == ST_MODE_DI_SPECULAR;
@@ -1167,11 +1194,11 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     if (taa) {   // the resolve composes the frame itself; history a / b alternate with the frame parity like the G-buffer
         const float4* hin = cs->taa_hist[cur ^ 1]; float4* hout = cs->taa_hist[cur];
         add(P_COMPOSITION, [=](cudaStream_t s) { e->taa_resolves++; launch_taa_resolve(cam, sc, cur, mode, di_final, gi_final, hin, hout, jit, s); });
-        meter();
+        meter(); pyramid();
         return;
     }
     add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, mode, di_final, gi_final, s); });
-    meter();
+    meter(); pyramid();
 }
 
 
@@ -1740,7 +1767,7 @@ int st_delete_camera(st_engine* e, st_camera_handle h) {
     if (e->copy_stream) CK(cudaStreamSynchronize(e->copy_stream));
     for (int k = 0; k < 2; k++) if (cs->side[k]) CK(cudaStreamSynchronize(cs->side[k]));
     cs->alive = false; cs->arena.release(); cs->svgf_pairs.release(); cs->pair[0] = cs->pair[1] = nullptr; cs->rgba8.release();
-    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr; cs->expo.release();
+    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr; cs->expo.release(); cs->bloom.release();
     return ST_OK;
 }
 int st_camera_set_strip(st_engine* e, st_camera_handle h, int y0, int y1) {
@@ -1896,6 +1923,9 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
     // ST_OPT_AUTO_EXPOSURE: the metering state exists only while the camera meters, and starts over when metering turns on
     if ((e->tonemapping != 0 && e->auto_exposure) != (e->tm_frame != 0 && e->ae_frame)) for (CameraSlot* c : e->cameras) c->expo.release();
     e->tm_frame = e->tonemapping; e->ae_frame = e->auto_exposure; e->expo_frame = e->exposure;
+    // ST_OPT_BLOOM: the pyramid exists only while the option is on, and is reallocated (zeroed) when its number of levels changes
+    if (e->bloom != e->bloom_frame || e->bloom_set.levels != e->bloom_cfg.levels) for (CameraSlot* c : e->cameras) c->bloom.release();
+    e->bloom_frame = e->bloom; e->bloom_cfg = e->bloom_set;
     e->frame += 1;
     if (too_deep) return fail(ST_ERR_LIMIT, "BVH deeper than the 24-entry traversal stack (strolle-gpu/src/lib.rs:72-76): the scene is not drawn until it changes");
     return ST_OK;
@@ -1926,6 +1956,7 @@ int st_render_range(st_engine* e, st_camera_handle h, int first, int last) {
     int rc = ensure_luts(e); if (rc) return rc;
     if ((rc = ensure_taa_history(e, cs))) return rc;
     if ((rc = ensure_exposure_state(e, cs))) return rc;
+    if ((rc = ensure_bloom_state(e, cs))) return rc;
     std::vector<Step> steps; build_schedule(e, cs, &steps);
     if (last < 0 || last >= (int)steps.size()) last = (int)steps.size() - 1;
     for (int i = std::max(first, 0); i <= last; i++) e->run_timed(steps[i].pass, steps[i].run, steps[i].sub);
@@ -1941,6 +1972,14 @@ int st_render_camera(st_engine* e, st_camera_handle h, void* host_out, int forma
 static int store_rgba8(st_engine* e, CameraSlot* cs, const CameraDev& cd, uchar4* dst8) {
     const SceneDev sc = e->scene();
     const int op = cs->desc.mode == ST_MODE_BVH_HEATMAP ? 0 : e->tm_frame;
+    if (blooms(e, cs)) {   // ST_OPT_BLOOM: composited from the stored pyramid, never rebuilt here
+        int rc = ensure_exposure_state(e, cs); if (rc) return rc;
+        if ((rc = ensure_bloom_state(e, cs))) return rc;
+        const uint32_t* state = meters(e, cs) ? (const uint32_t*)cs->expo.p : nullptr; const ExposureDev ep = e->expo_frame;
+        const BloomDev bp = e->bloom_cfg; const BloomLevels lv = bloom_levels(e, cs);
+        e->run_timed(P_COMPOSITION, [=](cudaStream_t s) { launch_output_bloom(cd, sc, op, state, ep, bp, lv.up[0], lv.w[0], lv.h[0], dst8, s); });
+        return ST_OK;
+    }
     if (op == 0) { e->run_timed(P_COMPOSITION, [=](cudaStream_t s) { launch_output_rgba8(cd, sc, dst8, s); }); return ST_OK; }
     int rc = ensure_exposure_state(e, cs); if (rc) return rc;
     const uint32_t* state = meters(e, cs) ? (const uint32_t*)cs->expo.p : nullptr; const ExposureDev ep = e->expo_frame;
@@ -2002,6 +2041,12 @@ int st_read_buffer(st_engine* e, st_camera_handle h, const char* name, float* ds
         if (!cs->expo.p) return fail(ST_ERR_NOT_FOUND, "no exposure state: the camera does not meter (ST_OPT_TONEMAPPING and ST_OPT_AUTO_EXPOSURE)");
         *count = 5 + kExposureBins;
         if (dst) { CK(cudaStreamSynchronize(e->stream)); CK(cudaMemcpy(dst, cs->expo.p, 4 * std::min(cap, *count), cudaMemcpyDeviceToHost)); }
+        return ST_OK;
+    }
+    if (!std::strcmp(name, "bloom")) {   // ST_OPT_BLOOM: the header words, then the down and up levels (bloom_layout, kernels.h)
+        if (!blooms(e, cs) || !cs->bloom.p) return fail(ST_ERR_NOT_FOUND, "no bloom pyramid: ST_OPT_BLOOM is off or the camera does not bloom");
+        BloomLevels lv; *count = bloom_layout((int)cs->desc.width, (int)cs->desc.height, e->bloom_cfg.levels, nullptr, &lv) / 4;
+        if (dst) { CK(cudaStreamSynchronize(e->stream)); CK(cudaMemcpy(dst, cs->bloom.p, 4 * std::min(cap, *count), cudaMemcpyDeviceToHost)); }
         return ST_OK;
     }
     if (!std::strcmp(name, "taa_history_a") || !std::strcmp(name, "taa_history_b")) {
@@ -2216,6 +2261,10 @@ int st_set_option(st_engine* e, int option, int value) {
         if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_AUTO_EXPOSURE: 0 (manual EV) or 1 (metered)");
         e->auto_exposure = value == 1; return ST_OK;
     }
+    if (option == ST_OPT_BLOOM) {   // takes effect at the next st_tick
+        if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_BLOOM: 0 (off) or 1 (bloom the Rgba8 store)");
+        e->bloom = value == 1; return ST_OK;
+    }
     if (option == ST_OPT_BVH_REFIT) { if (value < 0) return fail(ST_ERR_INVALID, "ST_OPT_BVH_REFIT: 0 or a positive budget"); e->bvh_refit = value; return ST_OK; }
     return fail(ST_ERR_INVALID, "unknown option");
 }
@@ -2228,6 +2277,24 @@ static int exposure_from(const st_exposure* x, ExposureDev* out) {
     if (!(x->speed_up >= 0.0f && x->speed_down >= 0.0f)) return fail(ST_ERR_INVALID, "st_set_exposure: speed_up, speed_down >= 0");
     *out = {x->ev, x->compensation, x->ev_min, x->ev_max, x->low, x->high, x->speed_up, x->speed_down};
     return ST_OK;
+}
+static int bloom_from(const st_bloom* x, BloomDev* out) {
+    if (!x) { *out = kBloomDefaults; return ST_OK; }
+    const float f[4] = {x->intensity, x->scatter, x->threshold, x->softness};
+    for (float v : f) if (!std::isfinite(v)) return fail(ST_ERR_INVALID, "st_set_bloom: every float field must be finite");
+    if (x->mode != 0 && x->mode != 1) return fail(ST_ERR_INVALID, "st_set_bloom: mode 0 (energy-conserving) or 1 (additive)");
+    if (x->mode == 0 ? !(x->intensity >= 0.0f && x->intensity <= 1.0f) : !(x->intensity >= 0.0f))
+        return fail(ST_ERR_INVALID, "st_set_bloom: intensity in [0, 1] (mode 0) or >= 0 (mode 1)");
+    if (!(x->scatter >= 0.0f && x->scatter <= 1.0f) || !(x->softness >= 0.0f && x->softness <= 1.0f)) return fail(ST_ERR_INVALID, "st_set_bloom: scatter, softness in [0, 1]");
+    if (!(x->threshold >= 0.0f)) return fail(ST_ERR_INVALID, "st_set_bloom: threshold >= 0");
+    if (x->levels < 1 || x->levels > kBloomMaxLevels) return fail(ST_ERR_INVALID, "st_set_bloom: levels in 1..8");
+    *out = {x->intensity, x->scatter, x->threshold, x->softness, x->levels, x->mode};
+    return ST_OK;
+}
+int st_set_bloom(st_engine* e, const st_bloom* x) {   // takes effect at the next st_tick
+    if (!e) return fail(ST_ERR_INVALID, "null engine");
+    BloomDev v; int rc = bloom_from(x, &v); if (rc) return rc;
+    e->bloom_set = v; return ST_OK;
 }
 int st_set_exposure(st_engine* e, const st_exposure* x) {   // takes effect at the next st_tick
     if (!e) return fail(ST_ERR_INVALID, "null engine");
@@ -2278,6 +2345,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_TEXTURE_MIP_BUILDS) { *value = e->texture_mip_builds; return ST_OK; }
     if (stat == ST_STAT_TAA_RESOLVES) { *value = e->taa_resolves; return ST_OK; }
     if (stat == ST_STAT_EXPOSURE_METERINGS) { *value = e->exposure_meterings; return ST_OK; }
+    if (stat == ST_STAT_BLOOM_PYRAMIDS) { *value = e->bloom_pyramids; return ST_OK; }
     if (stat == ST_STAT_ENVIRONMENT_MAP_LAUNCHES) { *value = e->envm_launches; return ST_OK; }
     if (stat == ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS) { *value = e->envs_builds; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
@@ -2508,11 +2576,15 @@ static const char* const kTaaStripsError = "ST_OPT_TEMPORAL_AA: row strips are n
 // Metering needs the whole frame's histogram (a reduction across the strips): not supported (yet) for strips.  A fixed exposure is per pixel.
 static const char* const kAutoExposureStripsError = "ST_OPT_AUTO_EXPOSURE: row strips are not supported; use a fixed exposure or render the camera on one engine";
 static bool auto_exposure_on(const st_engine* e) { return (e->tonemapping != 0 && e->auto_exposure) || (e->tm_frame != 0 && e->ae_frame); }
+// The pyramid needs the whole frame (each level's footprint crosses strip edges): not supported (yet) for strips
+static const char* const kBloomStripsError = "ST_OPT_BLOOM: row strips are not supported; render the camera on one engine";
+static bool bloom_on(const st_engine* e) { return e->bloom || e->bloom_frame; }
 int st_render_strips(st_engine* e, st_camera_handle h, void* host_out, int format, int temporal_reach, int gather) {
     CameraSlot* cs = e ? get_camera(e, h) : nullptr;
     if (!cs) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
     if (auto_exposure_on(e)) return fail(ST_ERR_INVALID, kAutoExposureStripsError);
+    if (bloom_on(e)) return fail(ST_ERR_INVALID, kBloomStripsError);
     CK(cudaSetDevice(e->device));
     int rc = enqueue_strip_frame(e, cs, temporal_reach); if (rc) return rc;
     if (!gather) return ST_OK;
@@ -2674,6 +2746,10 @@ int st_multi_set_exposure(st_multi* m, const st_exposure* x) {
     ExposureDev v; int rc = exposure_from(x, &v); if (rc) return rc;   // validated once: a refused call changes no member
     ST_MULTI_ALL(st_set_exposure(e, x));
 }
+int st_multi_set_bloom(st_multi* m, const st_bloom* x) {
+    BloomDev v; int rc = bloom_from(x, &v); if (rc) return rc;   // validated once: a refused call changes no member
+    ST_MULTI_ALL(st_set_bloom(e, x));
+}
 int st_multi_set_seed_base(st_multi* m, uint32_t base) { ST_MULTI_ALL(st_set_seed_base(e, base)); }
 int st_multi_set_blue_noise(st_multi* m, const uint8_t* rgba) { ST_MULTI_ALL(st_set_blue_noise(e, rgba)); }
 int st_multi_tick(st_multi* m) { ST_MULTI_ALL(st_tick(e)); }
@@ -2715,6 +2791,7 @@ int st_multi_render_camera(st_multi* m, st_camera_handle h, void* host_out, int 
     if (n == 1) return st_render_camera(m->e[0], m->cams[h][0], host_out, format);
     for (st_engine* e : m->e) if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
     for (st_engine* e : m->e) if (auto_exposure_on(e)) return fail(ST_ERR_INVALID, kAutoExposureStripsError);
+    for (st_engine* e : m->e) if (bloom_on(e)) return fail(ST_ERR_INVALID, kBloomStripsError);
     std::vector<CameraSlot*> cs(n);
     for (size_t i = 0; i < n; i++) {   // first-use allocations and LUT generation synchronise their device: do them before anything can wait on a peer
         cs[i] = get_camera(m->e[i], m->cams[h][i]);

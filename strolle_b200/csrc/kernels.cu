@@ -17,6 +17,9 @@
 #include <vector>
 #include "st_device.cuh"
 #include "kernels.h"
+#if ST_BLOOM_TAIL_KIND == 2
+#include <cooperative_groups.h>
+#endif
 
 // Compiled twice (strolle_b200/build.py): as namespace st with strict IEEE arithmetic (every kernel), and with -DST_FAST=1 as
 // namespace stf, the fast-shading flavour of the ReSTIR kernels K5-K19 only (see st_math.cuh).
@@ -1568,6 +1571,269 @@ __global__ void __launch_bounds__(ST_BLOCK) k_output_display(KPARAMS, uchar4* __
     out[i] = make_uchar4((unsigned char)q[0], (unsigned char)q[1], (unsigned char)q[2], 255);
 }
 
+// ---- ST_OPT_BLOOM (DESIGN.md §2 "Bloom") -------------------------------------------------------------------------------------------
+// Every f32 step is one IEEE operation in the order written (strict build only); oracle_bloom/bloom.cpp restates it operation for
+// operation.  The small levels' shape (DESIGN.md §4 "Bloom" compares the variants; tools/bloom_variants.py builds them): one launch per
+// level, down and up (ST_BLOOM_TAIL_TEXELS 0), or the levels of at most ST_BLOOM_TAIL_TEXELS texels down and back up in one launch:
+// ST_BLOOM_TAIL_KIND 0, one CTA over global memory; 1, one CTA holding the tail in its shared memory; 2, a cluster of
+// ST_BLOOM_CLUSTER CTAs holding it in distributed shared memory.  Every shape computes each texel with the same functions; one launch
+// per level measured fastest.
+#ifndef ST_BLOOM_TAIL_TEXELS
+#define ST_BLOOM_TAIL_TEXELS 0
+#endif
+#ifndef ST_BLOOM_TAIL_KIND
+#define ST_BLOOM_TAIL_KIND 0
+#endif
+#ifndef ST_BLOOM_CLUSTER
+#define ST_BLOOM_CLUSTER 8
+#endif
+#define BLOOM_TX 32   // level-0 texels per CTA (x, y) of the first downsample
+#define BLOOM_TY 8
+#define BLOOM_SX (2 * BLOOM_TX + 4)   // the frame texels it reads: its 2 x 2 footprints plus a 2-texel halo
+#define BLOOM_SY (2 * BLOOM_TY + 4)
+#define BLOOM_TAIL_THREADS 512
+ST_DEV int bloom_clampi(int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); }
+// One channel of the frame: c where it is finite and > 0, else 0; times the exposure
+ST_DEV float bloom_in(float c, float s) { return (c > 0.0f && c < finf()) ? c * s : 0.0f; }
+// A frame texel as the pyramid takes it: cleared, exposed, through the soft-knee prefilter (threshold > 0); a non-finite channel is 0
+ST_DEV float4 bloom_input(float4 c, float s, const BloomDev& b) {
+    float x = bloom_in(c.x, s), y = bloom_in(c.y, s), z = bloom_in(c.z, s);
+    if (b.threshold > 0.0f) {
+        float m = x > y ? x : y;
+        m = m > z ? m : z;
+        const float t = b.threshold, k = t * b.softness;
+        const float q0 = rclamp((m - t) + k, 0.0f, 2.0f * k);
+        const float q = (q0 * q0) / (4.0f * k + 1e-4f);
+        const float w = (q > m - t ? q : m - t) / (m > 1e-4f ? m : 1e-4f);
+        x = x * w; y = y * w; z = z * w;
+    }
+    return f4(x < finf() ? x : 0.0f, y < finf() ? y : 0.0f, z < finf() ? z : 0.0f, 0.0f);
+}
+// The 2 x 2 box of one of the 13 taps, as {w t, w} with t its average and w its Karis weight 1 / (1 + L(t)) (KARIS) or 1
+template <bool KARIS>
+ST_DEV float4 bloom_tap(float4 a, float4 b, float4 c, float4 d) {
+    const float4 t = ((a + b) + (c + d)) * 0.25f;
+    if (!KARIS) return f4(t.x, t.y, t.z, 1.0f);
+    const float w = 1.0f / (1.0f + expo_luminance(t.x, t.y, t.z));
+    return f4(t.x * w, t.y * w, t.z * w, w);
+}
+// A group of four taps (row-major): their weighted average
+template <bool KARIS>
+ST_DEV float4 bloom_group(float4 a, float4 b, float4 c, float4 d) {
+    const float4 s = (a + b) + (c + d);
+    if (!KARIS) return f4(s.x * 0.25f, s.y * 0.25f, s.z * 0.25f, 0.0f);
+    const float w = (a.w + b.w) + (c.w + d.w);
+    return f4(s.x / w, s.y / w, s.z / w, 0.0f);
+}
+// The 13-tap texel from odd-corner taps o[n][m] (corners 2i - 1 + 2m, 2j - 1 + 2n) and even-corner taps e[n][m] (2i + 2m, 2j + 2n)
+template <bool KARIS, class O, class E>
+ST_DEV float4 bloom_13(O o, E e) {
+    const float4 C = bloom_group<KARIS>(e(0, 0), e(1, 0), e(0, 1), e(1, 1));
+    const float4 TL = bloom_group<KARIS>(o(0, 0), o(1, 0), o(0, 1), o(1, 1)), TR = bloom_group<KARIS>(o(1, 0), o(2, 0), o(1, 1), o(2, 1));
+    const float4 BL = bloom_group<KARIS>(o(0, 1), o(1, 1), o(0, 2), o(1, 2)), BR = bloom_group<KARIS>(o(1, 1), o(2, 1), o(1, 2), o(2, 2));
+    const float4 r = C * 0.5f + ((TL + TR) + (BL + BR)) * 0.125f;
+    return f4(r.x, r.y, r.z, 0.0f);
+}
+// Level k >= 1: texel (i, j) from level k - 1 (sw x sh, texel t read as src(t)), every index clamped
+template <class S>
+ST_DEV float4 bloom_down_at(S src, int sw, int sh, int i, int j) {
+    auto T = [&](int x, int y) { return src((size_t)bloom_clampi(y, sh - 1) * sw + bloom_clampi(x, sw - 1)); };
+    auto tap = [&](int cx, int cy) { return bloom_tap<false>(T(cx - 1, cy - 1), T(cx, cy - 1), T(cx - 1, cy), T(cx, cy)); };
+    return bloom_13<false>([&](int m, int n) { return tap(2 * i - 1 + 2 * m, 2 * j - 1 + 2 * n); },
+                           [&](int m, int n) { return tap(2 * i + 2 * m, 2 * j + 2 * n); });
+}
+// Plain loads: the tails read what their own CTA wrote
+ST_DEV float4 bloom_down_texel(const float4* src, int sw, int sh, int i, int j) { return bloom_down_at([&](size_t t) { return src[t]; }, sw, sh, i, j); }
+// tent(u)(fx, fy): the 3 x 3 (1 2 1) x (1 2 1) / 16 filter of the coarse level u (cw x ch) at the texel (min(fx >> 1, cw - 1),
+// min(fy >> 1, ch - 1)) that covers the fine texel, every index clamped
+template <class S>
+ST_DEV float4 bloom_tent_at(S u, int cw, int ch, int fx, int fy) {
+    const int cx = (fx >> 1) < cw - 1 ? (fx >> 1) : cw - 1, cy = (fy >> 1) < ch - 1 ? (fy >> 1) : ch - 1;
+    const int x0 = bloom_clampi(cx - 1, cw - 1), x2 = bloom_clampi(cx + 1, cw - 1);
+    float4 r[3];
+#pragma unroll
+    for (int d = 0; d < 3; d++) {
+        const size_t row = (size_t)bloom_clampi(cy - 1 + d, ch - 1) * cw;
+        r[d] = (u(row + x0) + u(row + cx) * 2.0f) + u(row + x2);
+    }
+    return ((r[0] + r[1] * 2.0f) + r[2]) * 0.0625f;
+}
+ST_DEV float4 bloom_tent(const float4* u, int cw, int ch, int fx, int fy) { return bloom_tent_at([&](size_t t) { return u[t]; }, cw, ch, fx, fy); }
+// up_k(i, j) = (1 - a) down_k + a tent(up_{k+1})
+template <class D, class C>
+ST_DEV float4 bloom_up_at(D down, C coarse, int w, int cw, int ch, int i, int j, float a) {
+    const float4 t = bloom_tent_at(coarse, cw, ch, i, j);
+    const float4 r = down((size_t)j * w + i) * (1.0f - a) + t * a;
+    return f4(r.x, r.y, r.z, 0.0f);
+}
+ST_DEV float4 bloom_up_texel(const float4* down, const float4* coarse, int w, int cw, int ch, int i, int j, float a) {
+    return bloom_up_at([&](size_t t) { return down[t]; }, [&](size_t t) { return coarse[t]; }, w, cw, ch, i, j, a);
+}
+// The first downsample, frame -> level 0 (dw x dh), BLOOM_TX x BLOOM_TY texels per CTA.  The CTA's frame texels (footprints plus the
+// 2-texel halo) are loaded once, through the input rule, into shared memory; then the 13 taps' boxes, each once with its Karis weight;
+// then each texel's groups.
+__global__ void __launch_bounds__(BLOOM_TX * BLOOM_TY) k_bloom_down0(const float4* __restrict__ output, int W, int H, float4* __restrict__ dst, int dw, int dh,
+                                                                     const u32* __restrict__ state, ExposureDev ep, int tm, BloomDev bp) {
+    __shared__ float4 s_src[BLOOM_SY][BLOOM_SX];
+    __shared__ float4 s_odd[BLOOM_TY + 2][BLOOM_TX + 2];    // corner (2 i0 - 1 + 2 m, 2 j0 - 1 + 2 n)
+    __shared__ float4 s_even[BLOOM_TY + 1][BLOOM_TX + 1];   // corner (2 i0 + 2 m, 2 j0 + 2 n)
+    const int i0 = blockIdx.x * BLOOM_TX, j0 = blockIdx.y * BLOOM_TY, x0 = 2 * i0 - 2, y0 = 2 * j0 - 2;
+    float s = 1.0f;
+    if (tm != 0) s = pow_det(2.0f, ep.compensation - (state ? __uint_as_float(state[0]) : ep.ev));
+    for (int k = threadIdx.x; k < BLOOM_SY * BLOOM_SX; k += BLOOM_TX * BLOOM_TY) {
+        const int ly = k / BLOOM_SX, lx = k - ly * BLOOM_SX;
+        (&s_src[0][0])[k] = bloom_input(output[(size_t)bloom_clampi(y0 + ly, H - 1) * W + bloom_clampi(x0 + lx, W - 1)], s, bp);
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < (BLOOM_TY + 2) * (BLOOM_TX + 2); k += BLOOM_TX * BLOOM_TY) {
+        const int n = k / (BLOOM_TX + 2), m = k - n * (BLOOM_TX + 2);
+        s_odd[n][m] = bloom_tap<true>(s_src[2 * n][2 * m], s_src[2 * n][2 * m + 1], s_src[2 * n + 1][2 * m], s_src[2 * n + 1][2 * m + 1]);
+    }
+    for (int k = threadIdx.x; k < (BLOOM_TY + 1) * (BLOOM_TX + 1); k += BLOOM_TX * BLOOM_TY) {
+        const int n = k / (BLOOM_TX + 1), m = k - n * (BLOOM_TX + 1);
+        s_even[n][m] = bloom_tap<true>(s_src[2 * n + 1][2 * m + 1], s_src[2 * n + 1][2 * m + 2], s_src[2 * n + 2][2 * m + 1], s_src[2 * n + 2][2 * m + 2]);
+    }
+    __syncthreads();
+    const int li = threadIdx.x % BLOOM_TX, lj = threadIdx.x / BLOOM_TX, i = i0 + li, j = j0 + lj;
+    if (i >= dw || j >= dh) return;
+    dst[(size_t)j * dw + i] = bloom_13<true>([&](int m, int n) { return s_odd[lj + n][li + m]; }, [&](int m, int n) { return s_even[lj + n][li + m]; });
+}
+__global__ void __launch_bounds__(ST_BLOCK) k_bloom_down(const float4* __restrict__ src, int sw, int sh, float4* __restrict__ dst, int dw, int dh) {
+    const int i = blockIdx.x * TILE_W + threadIdx.x % TILE_W, j = blockIdx.y * TILE_H + threadIdx.x / TILE_W;
+    if (i < dw && j < dh) dst[(size_t)j * dw + i] = bloom_down_texel(src, sw, sh, i, j);
+}
+__global__ void __launch_bounds__(ST_BLOCK) k_bloom_up(const float4* __restrict__ down, const float4* __restrict__ coarse, int w, int h, int cw, int ch,
+                                                       float4* __restrict__ up, float a) {
+    const int i = blockIdx.x * TILE_W + threadIdx.x % TILE_W, j = blockIdx.y * TILE_H + threadIdx.x / TILE_W;
+    if (i < w && j < h) up[(size_t)j * w + i] = bloom_up_texel(down, coarse, w, cw, ch, i, j, a);
+}
+// Levels first .. L - 1 down from level first - 1, then up_{L-2} .. up_first, by one CTA: each level is one block-wide pass over
+// global memory (L1 / L2 resident at these sizes), separated by __syncthreads
+__global__ void __launch_bounds__(BLOOM_TAIL_THREADS) k_bloom_tail(const __grid_constant__ BloomLevels lv, int first, float a) {
+    for (int k = first; k < lv.levels; k++) {
+        for (int t = threadIdx.x; t < lv.w[k] * lv.h[k]; t += BLOOM_TAIL_THREADS) {
+            const int j = t / lv.w[k], i = t - j * lv.w[k];
+            lv.down[k][t] = bloom_down_texel(lv.down[k - 1], lv.w[k - 1], lv.h[k - 1], i, j);
+        }
+        __syncthreads();
+    }
+    for (int k = lv.levels - 2; k >= first; k--) {
+        for (int t = threadIdx.x; t < lv.w[k] * lv.h[k]; t += BLOOM_TAIL_THREADS) {
+            const int j = t / lv.w[k], i = t - j * lv.w[k];
+            lv.up[k][t] = bloom_up_texel(lv.down[k], lv.up[k + 1], lv.w[k], lv.w[k + 1], lv.h[k + 1], i, j, a);
+        }
+        __syncthreads();
+    }
+}
+#if ST_BLOOM_TAIL_KIND == 1
+// The same tail held in the CTA's dynamic shared memory: down_first .. down_{L-1}, then up_first .. up_{L-2}; only level first - 1 is
+// read from global memory, every level is also written there (the "bloom" read-back)
+__global__ void __launch_bounds__(BLOOM_TAIL_THREADS) k_bloom_tail_smem(const __grid_constant__ BloomLevels lv, int first, float a) {
+    extern __shared__ float4 s_lv[];
+    const int L = lv.levels;
+    auto base = [&](bool up, int k) {   // offset of a level in s_lv
+        size_t off = 0;
+        for (int q = first; q < L; q++) { if (!up && q == k) return off; off += (size_t)lv.w[q] * lv.h[q]; }
+        for (int q = first; q + 1 < L; q++) { if (q == k) return off; off += (size_t)lv.w[q] * lv.h[q]; }
+        return off;
+    };
+    for (int k = first; k < L; k++) {
+        const float4* sp = s_lv + base(false, k - 1);
+        float4* d = s_lv + base(false, k);
+        for (int t = threadIdx.x; t < lv.w[k] * lv.h[k]; t += BLOOM_TAIL_THREADS) {
+            const int j = t / lv.w[k], i = t - j * lv.w[k];
+            const float4 v = k == first ? bloom_down_texel(lv.down[k - 1], lv.w[k - 1], lv.h[k - 1], i, j) : bloom_down_texel(sp, lv.w[k - 1], lv.h[k - 1], i, j);
+            d[t] = v; lv.down[k][t] = v;
+        }
+        __syncthreads();
+    }
+    for (int k = L - 2; k >= first; k--) {
+        const float4* sd = s_lv + base(false, k);
+        const float4* sc = s_lv + (k + 1 == L - 1 ? base(false, k + 1) : base(true, k + 1));
+        float4* u = s_lv + base(true, k);
+        for (int t = threadIdx.x; t < lv.w[k] * lv.h[k]; t += BLOOM_TAIL_THREADS) {
+            const int j = t / lv.w[k], i = t - j * lv.w[k];
+            const float4 v = bloom_up_texel(sd, sc, lv.w[k], lv.w[k + 1], lv.h[k + 1], i, j, a);
+            u[t] = v; lv.up[k][t] = v;
+        }
+        __syncthreads();
+    }
+}
+#endif
+#if ST_BLOOM_TAIL_KIND == 2
+// The same tail spread over a cluster of ST_BLOOM_CLUSTER CTAs: texel t of a level of n texels lives in the shared memory of rank
+// t / ceil(n / ST_BLOOM_CLUSTER); each rank computes its own texels, reads the others' through distributed shared memory, and the cluster
+// synchronises between levels.  Only level first - 1 is read from global memory; every level is also written there.
+__global__ void __launch_bounds__(BLOOM_TAIL_THREADS) k_bloom_tail_cluster(const __grid_constant__ BloomLevels lv, int first, float a) {
+    namespace cg = cooperative_groups;
+    cg::cluster_group cluster = cg::this_cluster();
+    extern __shared__ float4 s_lv[];
+    const int L = lv.levels, R = (int)cluster.block_rank();
+    auto chunk = [&](int k) { return (lv.w[k] * lv.h[k] + ST_BLOOM_CLUSTER - 1) / ST_BLOOM_CLUSTER; };
+    auto base = [&](bool up, int k) {   // offset of a level's chunk in s_lv (the same in every rank)
+        size_t off = 0;
+        for (int q = first; q < L; q++) { if (!up && q == k) return off; off += (size_t)chunk(q); }
+        for (int q = first; q + 1 < L; q++) { if (q == k) return off; off += (size_t)chunk(q); }
+        return off;
+    };
+    auto dsm = [&](size_t b, int c) {   // texel t of the level whose chunks start at b
+        return [&cluster, b, c](size_t t) { const unsigned r = (unsigned)(t / (size_t)c); return *cluster.map_shared_rank(s_lv + b + (t - (size_t)r * c), r); };
+    };
+    for (int k = first; k < L; k++) {
+        const int c = chunk(k), n = lv.w[k] * lv.h[k];
+        float4* d = s_lv + base(false, k);
+        for (int t = R * c + threadIdx.x; t < min(n, (R + 1) * c); t += BLOOM_TAIL_THREADS) {
+            const int j = t / lv.w[k], i = t - j * lv.w[k];
+            const float4 v = k == first ? bloom_down_texel(lv.down[k - 1], lv.w[k - 1], lv.h[k - 1], i, j)
+                                        : bloom_down_at(dsm(base(false, k - 1), chunk(k - 1)), lv.w[k - 1], lv.h[k - 1], i, j);
+            d[t - R * c] = v; lv.down[k][t] = v;
+        }
+        cluster.sync();
+    }
+    for (int k = L - 2; k >= first; k--) {
+        const int c = chunk(k), n = lv.w[k] * lv.h[k];
+        float4* u = s_lv + base(true, k);
+        const auto down = dsm(base(false, k), c);
+        const auto coarse = dsm(k + 1 == L - 1 ? base(false, k + 1) : base(true, k + 1), chunk(k + 1));
+        for (int t = R * c + threadIdx.x; t < min(n, (R + 1) * c); t += BLOOM_TAIL_THREADS) {
+            const int j = t / lv.w[k], i = t - j * lv.w[k];
+            const float4 v = bloom_up_at(down, coarse, lv.w[k], lv.w[k + 1], lv.h[k + 1], i, j, a);
+            u[t - R * c] = v; lv.up[k][t] = v;
+        }
+        cluster.sync();
+    }
+}
+#endif
+// The Rgba8UnormSrgb store with the glow: x is what k_output_rgba8 (OP 0) or k_output_display<OP> would store before T, B = tent(up_0)
+template <int OP>
+__global__ void __launch_bounds__(ST_BLOCK) k_output_bloom(KPARAMS, uchar4* __restrict__ out, const u32* __restrict__ state, ExposureDev ep, BloomDev bp,
+                                                           const float4* __restrict__ up0, int w0, int h0) {
+    Px p = pixel_full(cam);
+    if (!p.in) return;
+    size_t i = pix(cam, p.x, p.y);
+    const float4 c = cam.output[i];
+    float3 x = f3(c.x, c.y, c.z);
+    if (OP != 0) {
+        const float ev = state ? __uint_as_float(state[0]) : ep.ev;
+        const float s = pow_det(2.0f, ep.compensation - ev);
+        x = f3((c.x > 0.0f ? c.x : 0.0f) * s, (c.y > 0.0f ? c.y : 0.0f) * s, (c.z > 0.0f ? c.z : 0.0f) * s);
+    }
+    const float4 B = bloom_tent(up0, w0, h0, (int)p.x, (int)p.y);
+    const float I = bp.intensity;
+    if (bp.mode == 0) { const float k = 1.0f - I; x = f3(x.x * k + B.x * I, x.y * k + B.y * I, x.z * k + B.z * I); }
+    else x = f3(x.x + B.x * I, x.y + B.y * I, x.z + B.z * I);
+    const float3 t = expo_transform<OP>(x);
+    float v[3] = {t.x, t.y, t.z};
+    u32 q[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        float y = sat(v[k]);
+        float e = (y <= 0.0031308f) ? 12.92f * y : 1.055f * pow_det(y, 1.0f / 2.4f) - 0.055f;
+        q[k] = to_u32_sat(sat(e) * 255.0f + 0.5f);
+    }
+    out[i] = make_uchar4((unsigned char)q[0], (unsigned char)q[1], (unsigned char)q[2], 255);
+}
+
 // K1 ref_tracing::main (ref_tracing.rs:4-60); NMAP: the packed normal is the mapped one, which K2 shades with and nudges along
 template <bool NMAP>
 __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
@@ -2275,6 +2541,49 @@ void launch_output_display(const CameraDev& c, const SceneDev& s, int op, const 
     case 2: k_output_display<2><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p); break;
     case 3: k_output_display<3><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p); break;
     default: k_output_display<4><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p); break;
+    }
+}
+static dim3 grid_of(int w, int h) { return dim3((w + TILE_W - 1) / TILE_W, (h + TILE_H - 1) / TILE_H); }
+void launch_bloom_pyramid(const CameraDev& c, const BloomLevels& lv, const u32* state, ExposureDev p, int tm, BloomDev b, cudaStream_t st) {
+    const int L = lv.levels;
+    k_bloom_down0<<<dim3((lv.w[0] + BLOOM_TX - 1) / BLOOM_TX, (lv.h[0] + BLOOM_TY - 1) / BLOOM_TY), BLOOM_TX * BLOOM_TY, 0, st>>>(
+        c.output, c.w, c.h, lv.down[0], lv.w[0], lv.h[0], state, p, tm, b);
+    int tail = L;   // the first level of the one-CTA tail (L: none)
+    for (int k = 1; k < L && ST_BLOOM_TAIL_TEXELS > 0; k++) if (lv.w[k] * lv.h[k] <= ST_BLOOM_TAIL_TEXELS) { tail = k; break; }
+    for (int k = 1; k < tail; k++) k_bloom_down<<<grid_of(lv.w[k], lv.h[k]), ST_BLOCK, 0, st>>>(lv.down[k - 1], lv.w[k - 1], lv.h[k - 1], lv.down[k], lv.w[k], lv.h[k]);
+    if (tail < L) {
+#if ST_BLOOM_TAIL_KIND == 0
+        k_bloom_tail<<<1, BLOOM_TAIL_THREADS, 0, st>>>(lv, tail, b.scatter);
+#else
+        // shared memory per CTA: the tail's down and up levels (for the cluster, each level's chunk); at most 4096 texels per level
+        // keeps one CTA's copy under 180 KB
+        size_t texels = 0;
+        for (int k = tail; k < L; k++) texels += (size_t)(lv.w[k] * lv.h[k] + (ST_BLOOM_TAIL_KIND == 2 ? ST_BLOOM_CLUSTER - 1 : 0)) / (ST_BLOOM_TAIL_KIND == 2 ? ST_BLOOM_CLUSTER : 1) * (k + 1 < L ? 2 : 1);
+        const int smem = (int)(16 * texels);
+#if ST_BLOOM_TAIL_KIND == 1
+        cudaFuncSetAttribute(k_bloom_tail_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        k_bloom_tail_smem<<<1, BLOOM_TAIL_THREADS, smem, st>>>(lv, tail, b.scatter);
+#else
+        cudaFuncSetAttribute(k_bloom_tail_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaLaunchConfig_t cfg = {};
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = ST_BLOOM_CLUSTER; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.gridDim = dim3(ST_BLOOM_CLUSTER); cfg.blockDim = dim3(BLOOM_TAIL_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
+        cudaLaunchKernelEx(&cfg, k_bloom_tail_cluster, lv, tail, b.scatter);
+#endif
+#endif
+    }
+    for (int k = std::min(tail, L - 1) - 1; k >= 0; k--)
+        k_bloom_up<<<grid_of(lv.w[k], lv.h[k]), ST_BLOCK, 0, st>>>(lv.down[k], lv.up[k + 1], lv.w[k], lv.h[k], lv.w[k + 1], lv.h[k + 1], lv.up[k], b.scatter);
+}
+void launch_output_bloom(const CameraDev& c, const SceneDev& s, int op, const u32* state, ExposureDev p, BloomDev b, const float4* up0, int w0, int h0,
+                         uchar4* out, cudaStream_t st) {
+    switch (op) {
+    case 0: k_output_bloom<0><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p, b, up0, w0, h0); break;
+    case 1: k_output_bloom<1><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p, b, up0, w0, h0); break;
+    case 2: k_output_bloom<2><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p, b, up0, w0, h0); break;
+    case 3: k_output_bloom<3><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p, b, up0, w0, h0); break;
+    default: k_output_bloom<4><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p, b, up0, w0, h0); break;
     }
 }
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {

@@ -55,6 +55,34 @@ void launch_exposure_histogram(const CameraDev& c, u32* state, ExposureDev p, in
 // The Rgba8 store of rows [c.y0, c.y1) through exposure 2^(compensation - ev) and the display transform `op` (1..4); ev = state[0]
 // when `state` is non-null (auto exposure), p.ev otherwise
 void launch_output_display(const CameraDev& c, const SceneDev& s, int op, const u32* state, ExposureDev p, uchar4* out, cudaStream_t st);
+// ST_OPT_BLOOM (DESIGN.md §2 "Bloom"; strict build only).  The per-camera pyramid: kBloomHeaderWords 32-bit words {L, w_0, h_0, ..,
+// w_7, h_7, 0, 0, 0} (zero past level L - 1), then float4 texels {r, g, b, 0}: the down levels 0 .. L - 1, then the up levels
+// 0 .. L - 2 (up_{L-1} is down_{L-1}).  Level k is max(1, W >> (k + 1)) x max(1, H >> (k + 1)).
+struct BloomDev { float intensity, scatter, threshold, softness; int levels, mode; };
+enum { kBloomMaxLevels = 8, kBloomHeaderWords = 20 };
+struct BloomLevels { float4* down[kBloomMaxLevels]; float4* up[kBloomMaxLevels]; int w[kBloomMaxLevels], h[kBloomMaxLevels]; int levels; };
+// The levels of a W x H frame's pyramid of L levels at `base` (null: sizes only); returns the storage's size in bytes
+inline size_t bloom_layout(int W, int H, int L, void* base, BloomLevels* lv) {
+    float4* p = base ? (float4*)((char*)base + 4 * kBloomHeaderWords) : nullptr;
+    size_t n = 0;
+    lv->levels = L;
+    for (int k = 0; k < kBloomMaxLevels; k++) {
+        lv->w[k] = k < L ? ((W >> (k + 1)) > 1 ? (W >> (k + 1)) : 1) : 0;
+        lv->h[k] = k < L ? ((H >> (k + 1)) > 1 ? (H >> (k + 1)) : 1) : 0;
+        lv->down[k] = lv->up[k] = nullptr;
+    }
+    for (int k = 0; k < L; k++) { lv->down[k] = p ? p + n : nullptr; n += (size_t)lv->w[k] * lv->h[k]; }
+    for (int k = 0; k + 1 < L; k++) { lv->up[k] = p ? p + n : nullptr; n += (size_t)lv->w[k] * lv->h[k]; }
+    lv->up[L - 1] = lv->down[L - 1];
+    return 4 * kBloomHeaderWords + 16 * n;
+}
+// The pyramid of c.output (the whole frame) through the input clamp, exposure (tm != 0: 2^(compensation - ev), ev = state[0] when
+// `state` is non-null, p.ev otherwise), the prefilter and the down and up chains
+void launch_bloom_pyramid(const CameraDev& c, const BloomLevels& lv, const u32* state, ExposureDev p, int tm, BloomDev b, cudaStream_t st);
+// The Rgba8 store of rows [c.y0, c.y1) with the glow of up_0 composited: op 0 today's store, 1..4 exposed and tonemapped as
+// launch_output_display
+void launch_output_bloom(const CameraDev& c, const SceneDev& s, int op, const u32* state, ExposureDev p, BloomDev b, const float4* up0, int w0, int h0,
+                         uchar4* out, cudaStream_t st);
 void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st);
 void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, const EnvMapDev* em, cudaStream_t st);
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st);

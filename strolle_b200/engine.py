@@ -33,6 +33,7 @@ OPT_TEMPORAL_AA = 18         # 1: sub-pixel camera jitter + temporal resolve in 
 OPT_ENVIRONMENT_MAP_SAMPLING = 19   # 1: the GI bounce and sky draw aim at the environment map's bright texels (0 = BRDF / uniform draws)
 OPT_TONEMAPPING = 20         # Rgba8 display transform: 0 off (today's store), 1 exposure only, 2 Reinhard, 3 ACES fitted, 4 AgX
 OPT_AUTO_EXPOSURE = 21       # 1: each camera meters its frame and adapts its EV (0 = the manual ev of set_exposure); needs OPT_TONEMAPPING
+OPT_BLOOM = 22               # 1: a glow around bright light in the Rgba8 store, from a downsample / upsample pyramid (set_bloom)
 TONEMAP_OFF, TONEMAP_EXPOSURE, TONEMAP_REINHARD, TONEMAP_ACES, TONEMAP_AGX = 0, 1, 2, 3, 4
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
@@ -50,6 +51,7 @@ STAT_TAA_RESOLVES = 12         # temporal resolve launches (OPT_TEMPORAL_AA) sin
 STAT_ENVIRONMENT_MAP_LAUNCHES = 13   # launches of the environment-mapped kernel variants (set_environment_map) since creation
 STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14   # environment-map distribution builds (OPT_ENVIRONMENT_MAP_SAMPLING) since creation
 STAT_EXPOSURE_METERINGS = 15   # metering launches (OPT_AUTO_EXPOSURE) since creation
+STAT_BLOOM_PYRAMIDS = 16       # pyramid builds (OPT_BLOOM) since creation
 
 
 class StrolleError(RuntimeError):
@@ -97,6 +99,44 @@ def _exposure(fields):
     return C.byref(_Exposure(*[v[n] for n, _ in _Exposure._fields_]))
 
 
+class _Bloom(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("intensity", "scatter", "threshold", "softness")] + [("levels", C.c_int32), ("mode", C.c_int32)]
+
+
+BLOOM_DEFAULTS = dict(intensity=0.15, scatter=0.7, threshold=0.0, softness=0.0, levels=7, mode=0)
+BLOOM_ENERGY_CONSERVING, BLOOM_ADDITIVE = 0, 1
+BLOOM_HEADER_WORDS = 20
+
+
+def _bloom(fields):
+    """st_bloom from keyword fields over the defaults; None (no fields) stands for NULL."""
+    if fields is None:
+        return None
+    unknown = set(fields) - set(BLOOM_DEFAULTS)
+    if unknown:
+        raise TypeError(f"set_bloom: unknown fields {sorted(unknown)}")
+    v = dict(BLOOM_DEFAULTS, **fields)
+    return C.byref(_Bloom(*[v[n] for n, _ in _Bloom._fields_]))
+
+
+def parse_bloom(words):
+    """read_buffer(cam, "bloom") as a dict: levels L, sizes [(w, h)] per level, down [L arrays (h, w, 3)] and up [L arrays; up[L - 1]
+    is down[L - 1]]."""
+    w = np.asarray(words, np.float32).reshape(-1)
+    u = w.view(np.uint32)
+    L = int(u[0])
+    sizes = [(int(u[1 + 2 * k]), int(u[2 + 2 * k])) for k in range(L)]
+    off, down, up = BLOOM_HEADER_WORDS, [], []
+    for dst in (down, up):
+        for k, (lw, lh) in enumerate(sizes):
+            if dst is up and k == L - 1:
+                up.append(down[L - 1])
+                break
+            dst.append(w[off:off + 4 * lw * lh].reshape(lh, lw, 4)[..., :3])
+            off += 4 * lw * lh
+    return dict(levels=L, sizes=sizes, down=down, up=up)
+
+
 def parse_exposure(words):
     """read_buffer(cam, "exposure") as a dict: ev, target (float32), counted, kept, frames and the 256 bins of the last frame."""
     w = np.asarray(words, np.float32).view(np.uint32)
@@ -129,7 +169,7 @@ def load_library():
         "st_insert_image": [P, u64, C.c_void_p, u32, u32], "st_remove_image": [P, u64], "st_set_material_textures": [P, u64, C.POINTER(_MaterialTextures)],
         "st_insert_instance": [P, u64, u64, u64, f32p], "st_remove_instance": [P, u64],
         "st_insert_light": [P, u64, C.POINTER(_Light)], "st_remove_light": [P, u64], "st_update_sun": [P, C.c_float, C.c_float],
-        "st_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_set_exposure": [P, C.c_void_p],
+        "st_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_set_exposure": [P, C.c_void_p], "st_set_bloom": [P, C.c_void_p],
         "st_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_update_camera": [P, i32, C.POINTER(_Camera)], "st_delete_camera": [P, i32],
         "st_tick": [P], "st_render_camera": [P, i32, P, C.c_int], "st_copy_output": [P, i32, P, C.c_int], "st_synchronize": [P],
         "st_set_seed_base": [P, u32], "st_set_blue_noise": [P, C.c_void_p],
@@ -159,7 +199,7 @@ def load_library():
         "st_multi_insert_image": [P, u64, C.c_void_p, u32, u32], "st_multi_remove_image": [P, u64], "st_multi_set_material_textures": [P, u64, C.POINTER(_MaterialTextures)],
         "st_multi_insert_instance": [P, u64, u64, u64, f32p], "st_multi_remove_instance": [P, u64],
         "st_multi_insert_light": [P, u64, C.POINTER(_Light)], "st_multi_remove_light": [P, u64], "st_multi_update_sun": [P, C.c_float, C.c_float],
-        "st_multi_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_multi_set_exposure": [P, C.c_void_p],
+        "st_multi_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_multi_set_exposure": [P, C.c_void_p], "st_multi_set_bloom": [P, C.c_void_p],
         "st_multi_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_multi_update_camera": [P, i32, C.POINTER(_Camera)], "st_multi_delete_camera": [P, i32],
         "st_multi_tick": [P], "st_multi_render_camera": [P, i32, P, C.c_int], "st_multi_synchronize": [P],
         "st_multi_set_option": [P, C.c_int, C.c_int], "st_multi_set_seed_base": [P, u32], "st_multi_set_blue_noise": [P, C.c_void_p],
@@ -359,6 +399,12 @@ class Engine:
         speed_down (fields not given take their defaults, EXPOSURE_DEFAULTS; no fields restores them all).  Refused as a whole when a
         field is out of range (include/strolle_b200.h st_set_exposure)."""
         self._check(self.lib.st_set_exposure(self._h, _exposure(fields or None)))
+
+    def set_bloom(self, **fields):
+        """The glow of OPT_BLOOM, from the next tick: intensity, scatter, threshold, softness, levels, mode (fields not given take their
+        defaults, BLOOM_DEFAULTS; no fields restores them all).  Refused as a whole when a field is out of range
+        (include/strolle_b200.h st_set_bloom)."""
+        self._check(self.lib.st_set_bloom(self._h, _bloom(fields or None)))
 
     # ---- cameras ----------------------------------------------------------------------------
     @staticmethod
@@ -653,6 +699,9 @@ class MultiEngine:
 
     def set_exposure(self, **fields):
         self._check(self.lib.st_multi_set_exposure(self._h, _exposure(fields or None)))
+
+    def set_bloom(self, **fields):
+        self._check(self.lib.st_multi_set_bloom(self._h, _bloom(fields or None)))
 
     def read_buffer(self, cam, name):
         """The whole frame's buffer, each strip read from the member that owns it."""
