@@ -142,6 +142,15 @@ typedef struct st_bloom { float intensity, scatter, threshold, softness; int32_t
 /* NULL restores the defaults {0.15, 0.7, 0, 0, 7, 0}.  The whole call is validated first: ST_ERR_INVALID, and no change, when a field
  * is out of range.  Takes effect at the next st_tick. */
 int st_set_bloom(st_engine* e, const st_bloom* bloom);
+/* The thin lens of ST_OPT_DEPTH_OF_FIELD (DESIGN.md §2 "Depth of field").  `focal_distance` (> 0, scene units): the view depth in
+ * focus; `aperture_f_stops` (> 0): the f-number N; `sensor_height` (> 0, scene units): the sensor's height, which with the
+ * projection's vertical field of view gives the focal length f = sensor_height P11 / 2 (P11 = projection[5]); `max_radius` in [1, 32]:
+ * the largest radius of the circle of confusion, in output pixels.  Every field must be finite. */
+typedef struct st_depth_of_field { float focal_distance, aperture_f_stops, sensor_height, max_radius; } st_depth_of_field;
+/* NULL restores the defaults {10, 1, 0.01866, 16} (focus 10 units away at f/1 on a Super 35 sensor, 18.66 mm in metres, as Bevy's
+ * DepthOfField uses).  The whole call is validated first: ST_ERR_INVALID, and no change, when a field is out of range.  Takes effect
+ * at the next st_tick. */
+int st_set_depth_of_field(st_engine* e, const st_depth_of_field* dof);
 
 /* Engine::create_camera / update_camera / delete_camera (lib.rs:252-294) */
 int st_create_camera(st_engine* e, const st_camera* camera, st_camera_handle* out);
@@ -216,7 +225,24 @@ int st_wavelet_times(st_engine* e, float* ms5, uint32_t* launches5, int reset);
  * GPU's SFU approximations (ex2/sqrt/rcp.approx, <= 2 ulp) and fused multiply-adds, like a GLSL compiler
  * does for the reference's shaders; 0 selects strict IEEE arithmetic with polynomial exp, which makes the
  * denoiser bit-identical to the CPU oracle (everything else is bit-identical in both modes). */
-enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18, ST_OPT_ENVIRONMENT_MAP_SAMPLING = 19, ST_OPT_TONEMAPPING = 20, ST_OPT_AUTO_EXPOSURE = 21, ST_OPT_BLOOM = 22 };
+enum { ST_OPT_SVGF_FAST_MATH = 1, ST_OPT_ASYNC_OUTPUT = 2, ST_OPT_HALO_NCCL = 3, ST_OPT_WAVELET_TILED = 4, ST_OPT_WAVELET_TILE_CFG = 5, ST_OPT_FUSE_REPROJECT = 6, ST_OPT_BVH_REUSE = 7, ST_OPT_VARIANCE_TILED = 8, ST_OPT_SHADING_FAST_MATH = 9, ST_OPT_STRIP_FUSED = 10, ST_OPT_FUSED_PASSES = 11, ST_OPT_STRIP_DMA = 12, ST_OPT_WAVELET_PAIRED = 13, ST_OPT_NORMAL_MAPS = 14, ST_OPT_BVH_REFIT = 15, ST_OPT_LIGHT_GRID = 16, ST_OPT_TEXTURE_FILTER = 17, ST_OPT_TEMPORAL_AA = 18, ST_OPT_ENVIRONMENT_MAP_SAMPLING = 19, ST_OPT_TONEMAPPING = 20, ST_OPT_AUTO_EXPOSURE = 21, ST_OPT_BLOOM = 22, ST_OPT_DEPTH_OF_FIELD = 23 };
+/* ST_OPT_DEPTH_OF_FIELD (default 0; 1 = on, anything else is ST_ERR_INVALID): frames are defocused through a thin lens
+ * (st_set_depth_of_field).  Once per rendered frame, after the composition or the temporal resolve and before the metering and the
+ * bloom pyramid (timed as P_COMPOSITION), each pixel's signed circle-of-confusion radius r = clamp(k (z - F) / z, -R, R) is formed from
+ * its view depth z (the primary hit distance of `surface_nd` times the cosine of its ray to the view axis; the sky takes min(k, R)),
+ * and `output` is gathered over a disc of taps in 16 x 16 pixel tiles into a per-camera frame; a tile whose neighbourhood holds no
+ * circle of 1/2 pixel or more is copied bit for bit.  That frame replaces `output` as the source of the Rgba32F copy, the metering
+ * of ST_OPT_AUTO_EXPOSURE, the bloom pyramid and every Rgba8 store; `output` itself stays the sharp frame (temporal AA's history and
+ * st_read_buffer("output") are unchanged), and st_copy_output never gathers again.  With F <= f the frame is not defocused (k = 0,
+ * the frame is copied).  CameraMode::BvhHeatmap is not defocused.  Reference mode is not gathered: its depth-0 rays (K1, K2) leave a
+ * thin lens instead, from a uniform point of the aperture disc of radius A / 2 on the camera's right and up axes towards the pinhole
+ * ray's point at view depth F, drawn from a dispatch stream of its own, so that the accumulation converges to the thin-lens image; it
+ * allocates no frame.  The frame is allocated zero-filled while the camera is defocused, freed when the option turns off, and reallocated when the camera is reallocated.
+ * st_read_buffer("depth_of_field") returns, as 32-bit words: {W, H, TX, TY, defocused, f, A, k, F, R, forward.xyz, 0, 0, 0} (TX x TY
+ * tiles; f .. forward as f32 bits), then r of every pixel (f32, row-major), then every tile's gather radius (u32, 0..32); it is
+ * ST_ERR_NOT_FOUND while the camera is not defocused.  While the option is on, as set or as taken by the last st_tick,
+ * st_render_strips and st_multi_render_camera over more than one member return ST_ERR_INVALID.  ST_STAT_DEPTH_OF_FIELD_GATHERS counts
+ * the gathers.  Takes effect at the next st_tick. */
 /* ST_OPT_BLOOM (default 0; 1 = on, anything else is ST_ERR_INVALID): the Rgba8UnormSrgb store gains a glow around bright light
  * (st_set_bloom).  After the frame is composed and metered (timed as P_COMPOSITION), once per rendered frame, a pyramid of `output` is
  * built: each channel cleared to 0 where it is not finite and > 0, times the exposure 2^(compensation - ev) while ST_OPT_TONEMAPPING is
@@ -379,7 +405,8 @@ enum { ST_STAT_WAVELET_TILED_LAUNCHES = 1, ST_STAT_WAVELET_TILED_ERRORS = 2, ST_
        ST_STAT_ENVIRONMENT_MAP_LAUNCHES = 13 /* launches of the environment-mapped kernel variants (st_set_environment_map) since creation */,
        ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14 /* environment-map distribution builds (ST_OPT_ENVIRONMENT_MAP_SAMPLING) since creation */,
        ST_STAT_EXPOSURE_METERINGS = 15 /* metering launches (ST_OPT_AUTO_EXPOSURE) since creation */,
-       ST_STAT_BLOOM_PYRAMIDS = 16 /* pyramid builds (ST_OPT_BLOOM) since creation */ };
+       ST_STAT_BLOOM_PYRAMIDS = 16 /* pyramid builds (ST_OPT_BLOOM) since creation */,
+       ST_STAT_DEPTH_OF_FIELD_GATHERS = 17 /* depth-of-field gathers (ST_OPT_DEPTH_OF_FIELD) since creation */ };
 int st_get_stat(st_engine* e, int stat, uint64_t* value);
 /* The host-side BVH builder on its own (no device needed): binned-SAH build (strolle/src/bvh/builder.rs:17-319) + DFS
  * serialisation (serializer.rs:20-110) over `n` primitives of 11 floats each (triangle id bits, material id bits,
@@ -482,6 +509,7 @@ int st_multi_synchronize(st_multi* m);
 int st_multi_set_option(st_multi* m, int option, int value);
 int st_multi_set_exposure(st_multi* m, const st_exposure* exposure);
 int st_multi_set_bloom(st_multi* m, const st_bloom* bloom);
+int st_multi_set_depth_of_field(st_multi* m, const st_depth_of_field* dof);
 int st_multi_set_seed_base(st_multi* m, uint32_t base);
 int st_multi_set_blue_noise(st_multi* m, const uint8_t* rgba8_256x256);
 int st_multi_read_buffer(st_multi* m, st_camera_handle camera, const char* name, float* dst, size_t cap_floats, size_t* count);

@@ -60,6 +60,7 @@ pub struct StrolleSun {
 /// `exposure`: the manual EV, the compensation and the metering's window, clamp and speeds.
 /// `bloom`: a glow around light brighter than the display shows (None, the default, stores no glow); with `Some` the views receive
 /// `Rgba8UnormSrgb` frames, with or without tonemapping; needs one GPU.
+/// `depth_of_field`: defocus each camera's frames through a thin lens (None, the default, keeps them sharp); needs one GPU.
 #[derive(Clone, Debug, Default, Resource)]
 pub struct StrolleSettings {
     pub normal_maps: bool,
@@ -73,6 +74,7 @@ pub struct StrolleSettings {
     pub auto_exposure: bool,
     pub exposure: st::Exposure,
     pub bloom: Option<st::Bloom>,
+    pub depth_of_field: Option<st::DepthOfField>,
 }
 
 #[derive(Clone, Debug)]
@@ -123,6 +125,7 @@ impl Plugin for StrollePlugin {
         engine.set_auto_exposure(settings.auto_exposure).expect("strolle_b200: ST_OPT_AUTO_EXPOSURE");
         engine.set_exposure(&settings.exposure).expect("strolle_b200: st_set_exposure");
         engine.set_bloom(settings.bloom.as_ref()).expect("strolle_b200: st_set_bloom");
+        engine.set_depth_of_field(settings.depth_of_field.as_ref()).expect("strolle_b200: st_set_depth_of_field");
         sync::set_environment_map(&mut engine, settings.environment_map.as_ref());
         render_app.world.resource_mut::<sync::Synced>().tonemapped = settings.tonemapping != st::Tonemapping::None || settings.bloom.is_some();
         render_app.insert_resource(EngineResource(engine));

@@ -344,6 +344,25 @@ impl Default for Bloom {
     }
 }
 
+/// The thin lens of defocused frames (`st_depth_of_field`, `ST_OPT_DEPTH_OF_FIELD`): a circle-of-confusion gather of each frame.
+#[derive(Clone, Copy, Debug, PartialEq)]
+pub struct DepthOfField {
+    /// The view depth in focus, in scene units (> 0).
+    pub focal_distance: f32,
+    /// The f-number (> 0): the aperture's diameter is the focal length over it.
+    pub aperture_f_stops: f32,
+    /// The sensor's height in scene units (> 0); with the projection's vertical field of view it gives the focal length.
+    pub sensor_height: f32,
+    /// The largest radius of the circle of confusion, in output pixels, in [1, 32].
+    pub max_radius: f32,
+}
+
+impl Default for DepthOfField {
+    fn default() -> Self {
+        Self { focal_distance: 10.0, aperture_f_stops: 1.0, sensor_height: 0.01866, max_radius: 16.0 }
+    }
+}
+
 /// The two formats the engine composes into (`CameraViewport::format`, `camera.rs:170-185`)
 #[derive(Clone, Copy, Debug, PartialEq, Eq)]
 pub enum ViewportFormat {
@@ -582,6 +601,20 @@ impl<P: Params> Engine<P> {
             check(unsafe { sys::st_multi_set_bloom(self.raw, &x) })?;
         }
         check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_BLOOM, bloom.is_some() as c_int) })
+    }
+
+    /// Defocuses frames through a thin lens (`ST_OPT_DEPTH_OF_FIELD` and `st_set_depth_of_field`; `None`, the default, keeps every
+    /// frame sharp).  Both frame formats show the defocused frame; Reference mode samples the lens in its primary rays; the heat map stays sharp.  Needs an engine over one
+    /// device: row strips over several refuse to render while it is on.  Refused as a whole when a field is out of range.  Takes effect
+    /// with the next frame's scene update.
+    pub fn set_depth_of_field(&mut self, dof: Option<&DepthOfField>) -> Result<(), Error> {
+        if let Some(d) = dof {
+            let x = sys::st_depth_of_field {
+                focal_distance: d.focal_distance, aperture_f_stops: d.aperture_f_stops, sensor_height: d.sensor_height, max_radius: d.max_radius,
+            };
+            check(unsafe { sys::st_multi_set_depth_of_field(self.raw, &x) })?;
+        }
+        check(unsafe { sys::st_multi_set_option(self.raw, sys::ST_OPT_DEPTH_OF_FIELD, dof.is_some() as c_int) })
     }
 
     /// Lights the scene from an equirectangular environment map in place of the procedural sky (`st_set_environment_map`; `None`,

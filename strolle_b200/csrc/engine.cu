@@ -390,6 +390,8 @@ static uint32_t dispatch_seed(uint32_t base, uint32_t frame, uint32_t k) {
 static const ExposureDev kExposureDefaults = {0.0f, 0.0f, -8.0f, 8.0f, 0.1f, 0.9f, 0.05f, 1.0f / 60.0f};
 // st_set_bloom(e, NULL): 15 % energy-conserving glow, scatter 0.7, no threshold, 7 levels
 static const BloomDev kBloomDefaults = {0.15f, 0.7f, 0.0f, 0.0f, 7, 0};
+// st_set_depth_of_field(e, NULL): focus at 10 scene units, f/1, a Super 35 sensor height (18.66 mm in metres), circles up to 16 px
+static const st_depth_of_field kDofDefaults = {10.0f, 1.0f, 0.01866f, 16.0f};
 
 struct CameraSlot {
     bool alive = false;
@@ -405,6 +407,7 @@ struct CameraSlot {
     DevMem taa; float4* taa_hist[2] = {nullptr, nullptr};   // ST_OPT_TEMPORAL_AA history {tonemapped rgb, count}, a / b by frame parity; zero-filled
     DevMem expo;   // ST_OPT_AUTO_EXPOSURE metering state (kExposureWords words, kernels.h), zero-filled: the next metering is a first frame
     DevMem bloom;  // ST_OPT_BLOOM pyramid (bloom_layout, kernels.h), zero-filled: a store before the first pyramid composites no glow
+    DevMem dof;    // ST_OPT_DEPTH_OF_FIELD frame, words and tap table (dof_layout, kernels.h), zero-filled
     // asynchronous RGBA8 read-back: slot k of the staging buffer is converted on the engine stream (ev_ready[k]) and copied to
     // the host on the copy stream (ev_copied[k]); the engine stream only waits for ev_copied[k] before reusing slot k
     cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
@@ -516,6 +519,8 @@ struct st_engine {
     ExposureDev exposure = kExposureDefaults, expo_frame = kExposureDefaults;
     // ST_OPT_BLOOM / st_set_bloom: the option and settings as set, and as st_tick took them for the frame
     bool bloom = false, bloom_frame = false; BloomDev bloom_set = kBloomDefaults, bloom_cfg = kBloomDefaults; uint64_t bloom_pyramids = 0;
+    // ST_OPT_DEPTH_OF_FIELD / st_set_depth_of_field: the option and the lens as set, and as st_tick took them for the frame
+    bool dof = false, dof_frame = false; st_depth_of_field dof_set = kDofDefaults, dof_cfg = kDofDefaults; uint64_t dof_gathers = 0;
     bool luts_static_ready = false, sky_ready = false; float sky_for_altitude = 0.0f;
     std::vector<CameraSlot*> cameras;
     // timing ---------------------------------------------------------------------------------------
@@ -1004,6 +1009,7 @@ static int allocate_camera(st_engine* e, CameraSlot* cs) {
     cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr;   // ST_OPT_TEMPORAL_AA: history restarts (allocated zeroed at the next resolve)
     cs->expo.release();   // ST_OPT_AUTO_EXPOSURE: the next metering is a first frame
     cs->bloom.release();  // ST_OPT_BLOOM: the pyramid is reallocated (zeroed) at the new size
+    cs->dof.release();    // ST_OPT_DEPTH_OF_FIELD: the frame is reallocated (zeroed) at the new size
     return ST_OK;
 }
 
@@ -1031,6 +1037,86 @@ static int ensure_bloom_state(st_engine* e, CameraSlot* cs) {
     CK(cudaMemcpy(cs->bloom.p, head, sizeof head, cudaMemcpyHostToDevice));   // the allocation synchronised the device: nothing reads it yet
     return ST_OK;
 }
+// ST_OPT_DEPTH_OF_FIELD: whether the camera's frames are gathered (the real-time modes; not the heat map; Reference mode samples the
+// lens in its primary rays instead)
+static bool defocuses(const st_engine* e, const CameraSlot* cs) {
+    return e->dof_frame && cs->desc.mode != ST_MODE_BVH_HEATMAP && cs->desc.mode != ST_MODE_REFERENCE;
+}
+// The dispatch id of Reference mode's lens draws: no other dispatch uses it, so every other draw is unchanged by the option
+static const uint32_t K_LENS = 27;
+static DofBufs dof_bufs(const CameraSlot* cs) { DofBufs b; dof_layout((int)cs->desc.width, (int)cs->desc.height, cs->dof.p, &b); return b; }
+// The gather's taps per radius rho = 1..32 (DESIGN.md §2 "Depth of field"), in double, once: the centre, then rings j = 1..4 of 8 j
+// taps at radius rho j / 4 and angles 2 pi i / (8 j), each offset rounded to the nearest integer (halves away from 0), with its
+// distance rounded to f32
+static const std::vector<DofTap>& dof_tap_table() {
+    static const std::vector<DofTap> table = [] {
+        std::vector<DofTap> t;
+        for (int rho = 1; rho <= kDofMaxRadius; rho++) {
+            t.push_back(DofTap{0, 0, 0.0f});
+            for (int j = 1; j <= 4; j++)
+                for (int i = 0; i < 8 * j; i++) {
+                    const double a = 2.0 * M_PI * i / (8 * j), rad = rho * j / 4.0;
+                    const long dx = std::lround(rad * std::cos(a)), dy = std::lround(rad * std::sin(a));
+                    t.push_back(DofTap{(short)dx, (short)dy, (float)std::sqrt((double)(dx * dx + dy * dy))});
+                }
+        }
+        return t;
+    }();
+    return table;
+}
+static int ensure_dof_state(st_engine* e, CameraSlot* cs) {
+    if (!defocuses(e, cs) || cs->dof.p) return ST_OK;
+    DofBufs b;
+    int rc = cs->dof.ensure(dof_layout((int)cs->desc.width, (int)cs->desc.height, nullptr, &b)); if (rc) return rc;
+    b = dof_bufs(cs);
+    const std::vector<DofTap>& taps = dof_tap_table();
+    CK(cudaMemcpy((void*)b.taps, taps.data(), taps.size() * sizeof(DofTap), cudaMemcpyHostToDevice));   // the allocation synchronised the device
+    return ST_OK;
+}
+// The frame's lens constants, in double from the f32 settings and projection, each rounded to f32 once: f = sensor_height P11 / 2,
+// A = f / N, k = A f / (F - f) H / sensor_height / 2; the view axis is the camera transform's -Z column, normalised.  F <= f: the
+// frame is not defocused (k = 0, every r = 0).
+static DofDev dof_params(const st_engine* e, const CameraSlot* cs) {
+    const st_depth_of_field& l = e->dof_cfg;
+    const st_camera& c = cs->desc;
+    const double f = 0.5 * (double)l.sensor_height * (double)c.projection[5], A = f / (double)l.aperture_f_stops, F = (double)l.focal_distance;
+    const bool active = F > f;
+    const double k = active ? A * f / (F - f) * (double)c.height / (double)l.sensor_height / 2.0 : 0.0;
+    const double fx = -(double)c.transform[8], fy = -(double)c.transform[9], fz = -(double)c.transform[10];
+    const double n = std::sqrt(fx * fx + fy * fy + fz * fz);
+    DofDev p = {};
+    p.active = active ? 1 : 0; p.k = (float)k; p.F = l.focal_distance; p.R = l.max_radius;
+    p.fwd_x = (float)(fx / n); p.fwd_y = (float)(fy / n); p.fwd_z = (float)(fz / n);
+    p.reach = (int)std::ceil((double)l.max_radius / kDofTile);
+    const DofBufs b = dof_bufs(cs);
+    const float fl[8] = {(float)f, (float)A, p.k, p.F, p.R, p.fwd_x, p.fwd_y, p.fwd_z};
+    p.head[0] = c.width; p.head[1] = c.height; p.head[2] = (uint32_t)b.tx; p.head[3] = (uint32_t)b.ty; p.head[4] = (uint32_t)p.active;
+    std::memcpy(p.head + 5, fl, sizeof fl);
+    return p;
+}
+// Reference mode's thin lens for frame seed `seed`, in double from the f32 settings, each rounded to f32 once: the aperture radius
+// h = A / 2 (f and A as dof_params), F, and the camera transform's unit X, Y and -Z columns.  False while F <= f: pinhole rays.
+static bool lens_params(const st_engine* e, const CameraSlot* cs, uint32_t seed, LensDev* out) {
+    const st_depth_of_field& l = e->dof_cfg;
+    const st_camera& c = cs->desc;
+    const double f = 0.5 * (double)l.sensor_height * (double)c.projection[5], A = f / (double)l.aperture_f_stops;
+    if (!(e->dof_frame && c.mode == ST_MODE_REFERENCE && (double)l.focal_distance > f)) return false;
+    double ax[3][3];
+    for (int k = 0; k < 3; k++) {
+        const double sg = k == 2 ? -1.0 : 1.0;
+        const double x = sg * c.transform[4 * k], y = sg * c.transform[4 * k + 1], z = sg * c.transform[4 * k + 2], n = std::sqrt(x * x + y * y + z * z);
+        ax[k][0] = x / n; ax[k][1] = y / n; ax[k][2] = z / n;
+    }
+    *out = LensDev{seed, (float)(A / 2.0), l.focal_distance, (float)ax[0][0], (float)ax[0][1], (float)ax[0][2], (float)ax[1][0], (float)ax[1][1],
+                   (float)ax[1][2], (float)ax[2][0], (float)ax[2][1], (float)ax[2][2]};
+    return true;
+}
+// The camera of the consumers of the frame (the Rgba32F copy, the metering, the pyramid, the Rgba8 stores): `output` is the
+// defocused frame while the camera is defocused
+static CameraDev frame_source(const st_engine* e, const CameraSlot* cs, CameraDev c) {
+    if (defocuses(e, cs) && cs->dof.p) c.output = dof_bufs(cs).frame;
+    return c;
+}
 static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* steps, const StripExt* ext = nullptr) {
     GpuCamera jc, jp; float4 jit;
     const bool taa = taa_cameras(e, cs, &jc, &jp, &jit);   // ST_OPT_TEMPORAL_AA: every pass sees the jittered cameras
@@ -1054,16 +1140,22 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     const bool eson = emon && e->envs_frame;
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
     auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
+    const CameraDev camO = frame_source(e, cs, cam);   // ST_OPT_DEPTH_OF_FIELD: the metering and the pyramid read the defocused frame
+    auto defocus = [&]() {   // ST_OPT_DEPTH_OF_FIELD: the CoC and the gather of the frame's `output`, once per rendered frame
+        if (!defocuses(e, cs)) return;
+        const DofDev dp = dof_params(e, cs); const DofBufs db = dof_bufs(cs);
+        add(P_COMPOSITION, [=](cudaStream_t s) { e->dof_gathers++; launch_depth_of_field(cam, dp, db, s); });
+    };
     auto meter = [&]() {   // ST_OPT_AUTO_EXPOSURE: the histogram of the frame's `output` and the adaptation, once per rendered frame
         if (!meters(e, cs)) return;
         uint32_t* state = (uint32_t*)cs->expo.p; const ExposureDev ep = e->expo_frame; const int sms = e->sm_count;
-        add(P_COMPOSITION, [=](cudaStream_t s) { e->exposure_meterings++; launch_exposure_histogram(cam, state, ep, sms, s); });
+        add(P_COMPOSITION, [=](cudaStream_t s) { e->exposure_meterings++; launch_exposure_histogram(camO, state, ep, sms, s); });
     };
     auto pyramid = [&]() {   // ST_OPT_BLOOM: the pyramid of the frame's `output`, after the metering, once per rendered frame
         if (!blooms(e, cs)) return;
         const BloomLevels lv = bloom_levels(e, cs); const uint32_t* state = meters(e, cs) ? (const uint32_t*)cs->expo.p : nullptr;
         const ExposureDev ep = e->expo_frame; const int tm = e->tm_frame; const BloomDev bp = e->bloom_cfg;
-        add(P_COMPOSITION, [=](cudaStream_t s) { e->bloom_pyramids++; launch_bloom_pyramid(cam, lv, state, ep, tm, bp, s); });
+        add(P_COMPOSITION, [=](cudaStream_t s) { e->bloom_pyramids++; launch_bloom_pyramid(camO, lv, state, ep, tm, bp, s); });
     };
     const float4* di_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_DI_DIFFUSE)) ? cam.di_diff_curr_colors : cam.di_diff_samples;
     const float4* gi_final = (d.denoise && (d.mode == ST_MODE_IMAGE || d.mode == ST_MODE_GI_DIFFUSE)) ? cam.gi_diff_curr_colors : cam.gi_diff_samples;
@@ -1073,12 +1165,17 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
         return;
     }
     if (d.mode == ST_MODE_REFERENCE) {
+        LensDev lens;   // ST_OPT_DEPTH_OF_FIELD: the depth-0 rays leave a thin lens
+        const bool lon = lens_params(e, cs, seed(K_LENS), &lens);
         for (uint32_t depth = 0; depth <= (uint32_t)d.ref_depth; depth++) {
             uint32_t sd = seed(P_REF_SHADING_SEED + depth);
-            add(P_REF_TRACING, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_ref_tracing(cam, sc, depth, nm, s); });
-            add(P_REF_SHADING, [=](cudaStream_t s) { if (emon) e->envm_launches++; launch_ref_shading(cam, sc, sd, depth, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, emon ? &emd : nullptr, s); });
+            add(P_REF_TRACING, [=](cudaStream_t s) { if (nm) e->normal_map_launches++; launch_ref_tracing(cam, sc, depth, nm, lon ? &lens : nullptr, s); });
+            add(P_REF_SHADING, [=](cudaStream_t s) {
+                if (emon) e->envm_launches++;
+                launch_ref_shading(cam, sc, sd, depth, lgon ? &lgd : nullptr, tfon ? &tfd : nullptr, emon ? &emd : nullptr, lon ? &lens : nullptr, s);
+            });
         }
-        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, nullptr, nullptr, s); });
+        add(P_REF_SHADING, [=](cudaStream_t s) { launch_ref_shading(cam, sc, 0u, 255u, nullptr, nullptr, nullptr, nullptr, s); });
         add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, 6u, di_final, gi_final, s); });
         meter(); pyramid();
         return;
@@ -1194,11 +1291,11 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     if (taa) {   // the resolve composes the frame itself; history a / b alternate with the frame parity like the G-buffer
         const float4* hin = cs->taa_hist[cur ^ 1]; float4* hout = cs->taa_hist[cur];
         add(P_COMPOSITION, [=](cudaStream_t s) { e->taa_resolves++; launch_taa_resolve(cam, sc, cur, mode, di_final, gi_final, hin, hout, jit, s); });
-        meter(); pyramid();
+        defocus(); meter(); pyramid();
         return;
     }
     add(P_COMPOSITION, [=](cudaStream_t s) { launch_composition(cam, sc, cur, mode, di_final, gi_final, s); });
-    meter(); pyramid();
+    defocus(); meter(); pyramid();
 }
 
 
@@ -1767,7 +1864,7 @@ int st_delete_camera(st_engine* e, st_camera_handle h) {
     if (e->copy_stream) CK(cudaStreamSynchronize(e->copy_stream));
     for (int k = 0; k < 2; k++) if (cs->side[k]) CK(cudaStreamSynchronize(cs->side[k]));
     cs->alive = false; cs->arena.release(); cs->svgf_pairs.release(); cs->pair[0] = cs->pair[1] = nullptr; cs->rgba8.release();
-    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr; cs->expo.release(); cs->bloom.release();
+    cs->taa.release(); cs->taa_hist[0] = cs->taa_hist[1] = nullptr; cs->expo.release(); cs->bloom.release(); cs->dof.release();
     return ST_OK;
 }
 int st_camera_set_strip(st_engine* e, st_camera_handle h, int y0, int y1) {
@@ -1926,6 +2023,9 @@ int st_tick(st_engine* e) {   // Engine::tick (lib.rs:301-395)
     // ST_OPT_BLOOM: the pyramid exists only while the option is on, and is reallocated (zeroed) when its number of levels changes
     if (e->bloom != e->bloom_frame || e->bloom_set.levels != e->bloom_cfg.levels) for (CameraSlot* c : e->cameras) c->bloom.release();
     e->bloom_frame = e->bloom; e->bloom_cfg = e->bloom_set;
+    // ST_OPT_DEPTH_OF_FIELD: the defocused frame exists only while the option is on
+    if (e->dof != e->dof_frame) for (CameraSlot* c : e->cameras) c->dof.release();
+    e->dof_frame = e->dof; e->dof_cfg = e->dof_set;
     e->frame += 1;
     if (too_deep) return fail(ST_ERR_LIMIT, "BVH deeper than the 24-entry traversal stack (strolle-gpu/src/lib.rs:72-76): the scene is not drawn until it changes");
     return ST_OK;
@@ -1957,6 +2057,7 @@ int st_render_range(st_engine* e, st_camera_handle h, int first, int last) {
     if ((rc = ensure_taa_history(e, cs))) return rc;
     if ((rc = ensure_exposure_state(e, cs))) return rc;
     if ((rc = ensure_bloom_state(e, cs))) return rc;
+    if ((rc = ensure_dof_state(e, cs))) return rc;
     std::vector<Step> steps; build_schedule(e, cs, &steps);
     if (last < 0 || last >= (int)steps.size()) last = (int)steps.size() - 1;
     for (int i = std::max(first, 0); i <= last; i++) e->run_timed(steps[i].pass, steps[i].run, steps[i].sub);
@@ -1990,11 +2091,13 @@ static int store_rgba8(st_engine* e, CameraSlot* cs, const CameraDev& cd, uchar4
 static int copy_rows_out(st_engine* e, CameraSlot* cs, void* host_out, int format, int y0, int y1) {
     const size_t W = cs->desc.width, n = W * cs->desc.height;
     const size_t first = (size_t)y0 * W, count = (size_t)(y1 - y0) * W;
-    if (format == ST_FORMAT_RGBA32F) CK(cudaMemcpyAsync((char*)host_out + first * 16, cs->dev.output + first, count * 16, cudaMemcpyDeviceToHost, e->stream));
+    int rc2 = ensure_dof_state(e, cs); if (rc2) return rc2;
+    const CameraDev src = frame_source(e, cs, cs->dev);   // ST_OPT_DEPTH_OF_FIELD: the defocused frame in place of `output`
+    if (format == ST_FORMAT_RGBA32F) CK(cudaMemcpyAsync((char*)host_out + first * 16, src.output + first, count * 16, cudaMemcpyDeviceToHost, e->stream));
     else if (format == ST_FORMAT_RGBA8_SRGB) {
-        int rc2 = cs->rgba8.ensure(2 * n * 4); if (rc2) return rc2;
+        if ((rc2 = cs->rgba8.ensure(2 * n * 4))) return rc2;
         cs->rgba8_slot ^= 1;
-        uchar4* dst8 = (uchar4*)cs->rgba8.p + (cs->rgba8_slot ? n : 0); CameraDev cd = cs->dev; cd.y0 = y0; cd.y1 = y1;
+        uchar4* dst8 = (uchar4*)cs->rgba8.p + (cs->rgba8_slot ? n : 0); CameraDev cd = src; cd.y0 = y0; cd.y1 = y1;
         const int k = cs->rgba8_slot;
         if (e->async_output) {   // conversion on the engine stream, copy on the copy stream: the next frame's passes do not queue behind the copy
             if (!e->copy_stream) CK(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
@@ -2047,6 +2150,12 @@ int st_read_buffer(st_engine* e, st_camera_handle h, const char* name, float* ds
         if (!blooms(e, cs) || !cs->bloom.p) return fail(ST_ERR_NOT_FOUND, "no bloom pyramid: ST_OPT_BLOOM is off or the camera does not bloom");
         BloomLevels lv; *count = bloom_layout((int)cs->desc.width, (int)cs->desc.height, e->bloom_cfg.levels, nullptr, &lv) / 4;
         if (dst) { CK(cudaStreamSynchronize(e->stream)); CK(cudaMemcpy(dst, cs->bloom.p, 4 * std::min(cap, *count), cudaMemcpyDeviceToHost)); }
+        return ST_OK;
+    }
+    if (!std::strcmp(name, "depth_of_field")) {   // ST_OPT_DEPTH_OF_FIELD: the header words, every pixel's r, every tile's rho (dof_layout)
+        if (!defocuses(e, cs) || !cs->dof.p) return fail(ST_ERR_NOT_FOUND, "no depth of field: ST_OPT_DEPTH_OF_FIELD is off or the camera is not defocused");
+        const DofBufs b = dof_bufs(cs); *count = b.words_count;
+        if (dst) { CK(cudaStreamSynchronize(e->stream)); CK(cudaMemcpy(dst, b.words, 4 * std::min(cap, *count), cudaMemcpyDeviceToHost)); }
         return ST_OK;
     }
     if (!std::strcmp(name, "taa_history_a") || !std::strcmp(name, "taa_history_b")) {
@@ -2265,6 +2374,10 @@ int st_set_option(st_engine* e, int option, int value) {
         if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_BLOOM: 0 (off) or 1 (bloom the Rgba8 store)");
         e->bloom = value == 1; return ST_OK;
     }
+    if (option == ST_OPT_DEPTH_OF_FIELD) {   // takes effect at the next st_tick
+        if (value != 0 && value != 1) return fail(ST_ERR_INVALID, "ST_OPT_DEPTH_OF_FIELD: 0 (off) or 1 (defocus through a thin lens)");
+        e->dof = value == 1; return ST_OK;
+    }
     if (option == ST_OPT_BVH_REFIT) { if (value < 0) return fail(ST_ERR_INVALID, "ST_OPT_BVH_REFIT: 0 or a positive budget"); e->bvh_refit = value; return ST_OK; }
     return fail(ST_ERR_INVALID, "unknown option");
 }
@@ -2290,6 +2403,21 @@ static int bloom_from(const st_bloom* x, BloomDev* out) {
     if (x->levels < 1 || x->levels > kBloomMaxLevels) return fail(ST_ERR_INVALID, "st_set_bloom: levels in 1..8");
     *out = {x->intensity, x->scatter, x->threshold, x->softness, x->levels, x->mode};
     return ST_OK;
+}
+static int dof_from(const st_depth_of_field* x, st_depth_of_field* out) {
+    if (!x) { *out = kDofDefaults; return ST_OK; }
+    const float f[4] = {x->focal_distance, x->aperture_f_stops, x->sensor_height, x->max_radius};
+    for (float v : f) if (!std::isfinite(v)) return fail(ST_ERR_INVALID, "st_set_depth_of_field: every field must be finite");
+    if (!(x->focal_distance > 0.0f) || !(x->aperture_f_stops > 0.0f) || !(x->sensor_height > 0.0f))
+        return fail(ST_ERR_INVALID, "st_set_depth_of_field: focal_distance, aperture_f_stops, sensor_height > 0");
+    if (!(x->max_radius >= 1.0f && x->max_radius <= (float)kDofMaxRadius)) return fail(ST_ERR_INVALID, "st_set_depth_of_field: max_radius in [1, 32]");
+    *out = *x;
+    return ST_OK;
+}
+int st_set_depth_of_field(st_engine* e, const st_depth_of_field* x) {   // takes effect at the next st_tick
+    if (!e) return fail(ST_ERR_INVALID, "null engine");
+    st_depth_of_field v; int rc = dof_from(x, &v); if (rc) return rc;
+    e->dof_set = v; return ST_OK;
 }
 int st_set_bloom(st_engine* e, const st_bloom* x) {   // takes effect at the next st_tick
     if (!e) return fail(ST_ERR_INVALID, "null engine");
@@ -2346,6 +2474,7 @@ int st_get_stat(st_engine* e, int stat, uint64_t* value) {
     if (stat == ST_STAT_TAA_RESOLVES) { *value = e->taa_resolves; return ST_OK; }
     if (stat == ST_STAT_EXPOSURE_METERINGS) { *value = e->exposure_meterings; return ST_OK; }
     if (stat == ST_STAT_BLOOM_PYRAMIDS) { *value = e->bloom_pyramids; return ST_OK; }
+    if (stat == ST_STAT_DEPTH_OF_FIELD_GATHERS) { *value = e->dof_gathers; return ST_OK; }
     if (stat == ST_STAT_ENVIRONMENT_MAP_LAUNCHES) { *value = e->envm_launches; return ST_OK; }
     if (stat == ST_STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS) { *value = e->envs_builds; return ST_OK; }
     if (stat == ST_STAT_STRIP_PULLED_ROWS) {   // rows of last frame's buffers this rank fetched from their owners so far (fused strip transport, all cameras)
@@ -2579,12 +2708,16 @@ static bool auto_exposure_on(const st_engine* e) { return (e->tonemapping != 0 &
 // The pyramid needs the whole frame (each level's footprint crosses strip edges): not supported (yet) for strips
 static const char* const kBloomStripsError = "ST_OPT_BLOOM: row strips are not supported; render the camera on one engine";
 static bool bloom_on(const st_engine* e) { return e->bloom || e->bloom_frame; }
+// A strip's gather needs max_radius + one tile of `output` and `surface_nd` rows beyond it: not supported (yet) for strips
+static const char* const kDofStripsError = "ST_OPT_DEPTH_OF_FIELD: row strips are not supported; render the camera on one engine";
+static bool dof_on(const st_engine* e) { return e->dof || e->dof_frame; }
 int st_render_strips(st_engine* e, st_camera_handle h, void* host_out, int format, int temporal_reach, int gather) {
     CameraSlot* cs = e ? get_camera(e, h) : nullptr;
     if (!cs) return fail(ST_ERR_NOT_FOUND, "unknown camera");
     if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
     if (auto_exposure_on(e)) return fail(ST_ERR_INVALID, kAutoExposureStripsError);
     if (bloom_on(e)) return fail(ST_ERR_INVALID, kBloomStripsError);
+    if (dof_on(e)) return fail(ST_ERR_INVALID, kDofStripsError);
     CK(cudaSetDevice(e->device));
     int rc = enqueue_strip_frame(e, cs, temporal_reach); if (rc) return rc;
     if (!gather) return ST_OK;
@@ -2750,6 +2883,10 @@ int st_multi_set_bloom(st_multi* m, const st_bloom* x) {
     BloomDev v; int rc = bloom_from(x, &v); if (rc) return rc;   // validated once: a refused call changes no member
     ST_MULTI_ALL(st_set_bloom(e, x));
 }
+int st_multi_set_depth_of_field(st_multi* m, const st_depth_of_field* x) {
+    st_depth_of_field v; int rc = dof_from(x, &v); if (rc) return rc;   // validated once: a refused call changes no member
+    ST_MULTI_ALL(st_set_depth_of_field(e, x));
+}
 int st_multi_set_seed_base(st_multi* m, uint32_t base) { ST_MULTI_ALL(st_set_seed_base(e, base)); }
 int st_multi_set_blue_noise(st_multi* m, const uint8_t* rgba) { ST_MULTI_ALL(st_set_blue_noise(e, rgba)); }
 int st_multi_tick(st_multi* m) { ST_MULTI_ALL(st_tick(e)); }
@@ -2792,6 +2929,7 @@ int st_multi_render_camera(st_multi* m, st_camera_handle h, void* host_out, int 
     for (st_engine* e : m->e) if (e->temporal_aa || e->taa_frame) return fail(ST_ERR_INVALID, kTaaStripsError);
     for (st_engine* e : m->e) if (auto_exposure_on(e)) return fail(ST_ERR_INVALID, kAutoExposureStripsError);
     for (st_engine* e : m->e) if (bloom_on(e)) return fail(ST_ERR_INVALID, kBloomStripsError);
+    for (st_engine* e : m->e) if (dof_on(e)) return fail(ST_ERR_INVALID, kDofStripsError);
     std::vector<CameraSlot*> cs(n);
     for (size_t i = 0; i < n; i++) {   // first-use allocations and LUT generation synchronise their device: do them before anything can wait on a peer
         cs[i] = get_camera(m->e[i], m->cams[h][i]);

@@ -1834,15 +1834,153 @@ __global__ void __launch_bounds__(ST_BLOCK) k_output_bloom(KPARAMS, uchar4* __re
     out[i] = make_uchar4((unsigned char)q[0], (unsigned char)q[1], (unsigned char)q[2], 255);
 }
 
-// K1 ref_tracing::main (ref_tracing.rs:4-60); NMAP: the packed normal is the mapped one, which K2 shades with and nudges along
-template <bool NMAP>
-__global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
+// ---- Depth of field (ST_OPT_DEPTH_OF_FIELD; DESIGN.md §2 "Depth of field") ---------------------------------------------------------
+// The gather stages each gathering tile's colours and radii, with a halo of its radius, in shared memory while the frame's max_radius
+// is at most ST_DOF_STAGE_MAX_RADIUS, and reads every tap from global memory (L1 / L2) above it, where the stage (up to 80^2 texels,
+// 128 KB at R = 32) leaves one CTA per SM: measured on an H100, the stage is faster at R = 16 and twice as slow at R = 32 (DESIGN.md
+// §4).  Both read the same values: the words are the same (tools/depth_of_field_variants.py builds 0 and 32 as tuning builds).
+#ifndef ST_DOF_STAGE_MAX_RADIUS
+#define ST_DOF_STAGE_MAX_RADIUS 16
+#endif
+#define DOF_THREADS (kDofTile * kDofTile)
+// r = clamp(k (z - F) / z, -R, R) with z = t dot(d, forward); the sky (t = 0) takes its limit min(k, R)
+ST_DEV float dof_coc(const DofDev& p, float t, float3 d) {
+    if (!p.active) return 0.0f;
+    if (t == 0.0f) return p.k < p.R ? p.k : p.R;
+    const float z = t * ((d.x * p.fwd_x + d.y * p.fwd_y) + d.z * p.fwd_z);
+    const float r = p.k * (z - p.F) / z;
+    return r < -p.R ? -p.R : (r > p.R ? p.R : r);
+}
+ST_DEV float dof_finite(float v) { return fabsf(v) < __int_as_float(0x7f800000) ? v : 0.0f; }
+// One tap's weight: s = min(|r_q|, |r_p|) for a tap behind p (r_q > r_p: r increases with z), |r_q| otherwise;
+// w = clamp(s - delta + 1, 0, 1) / max(s, 1/2)^2
+ST_DEV float dof_weight(float rq, float rp, float delta) {
+    const float aq = fabsf(rq), ap = fabsf(rp);
+    const float s = rq > rp ? (aq < ap ? aq : ap) : aq;
+    float c = (s - delta) + 1.0f;
+    c = c < 0.0f ? 0.0f : (c > 1.0f ? 1.0f : c);
+    const float m = s > 0.5f ? s : 0.5f;
+    return c / (m * m);
+}
+// The gathered value of a pixel with radius rp, over the taps of radius rho; tap(dx, dy, &c, &r) reads the clamped neighbour
+template <class T>
+ST_DEV float4 dof_gather_px(const DofTap* __restrict__ taps, int rho, float rp, T tap) {
+    const DofTap* row = taps + (size_t)(rho - 1) * kDofTaps;
+    float ax = 0.0f, ay = 0.0f, az = 0.0f, ws = 0.0f;
+    for (int i = 0; i < kDofTaps; i++) {
+        const DofTap t = row[i];
+        float4 c; float rq;
+        tap((int)t.dx, (int)t.dy, &c, &rq);
+        const float w = dof_weight(rq, rp, t.d);
+        ax = ax + c.x * w; ay = ay + c.y * w; az = az + c.z * w; ws = ws + w;
+    }
+    return f4(ax / ws, ay / ws, az / ws, 1.0f);
+}
+// One CTA per 16 x 16 tile: every pixel's r, and the tile's max |r|; CTA (0, 0) writes the header words
+__global__ void __launch_bounds__(DOF_THREADS) k_dof_coc(const __grid_constant__ CameraDev cam, const __grid_constant__ DofDev p, float* __restrict__ words,
+                                                         float* __restrict__ tile_m) {
+    __shared__ float s_m[DOF_THREADS / 32];
+    const int x = blockIdx.x * kDofTile + threadIdx.x % kDofTile, y = blockIdx.y * kDofTile + threadIdx.x / kDofTile;
+    float a = 0.0f;
+    if (x < cam.w && y < cam.h) {
+        const size_t i = (size_t)y * cam.w + x;
+        const float r = dof_coc(p, cam.surface_nd[i].w, cam_ray(cam.curr, (u32)x, (u32)y).d);
+        words[kDofHeaderWords + i] = r;
+        a = fabsf(r);
+    }
+    for (int o = 16; o > 0; o >>= 1) { const float b = __shfl_xor_sync(0xffffffffu, a, o); a = a > b ? a : b; }
+    if ((threadIdx.x & 31) == 0) s_m[threadIdx.x >> 5] = a;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float m = s_m[0];
+        for (int k = 1; k < DOF_THREADS / 32; k++) m = m > s_m[k] ? m : s_m[k];
+        tile_m[blockIdx.y * gridDim.x + blockIdx.x] = m;
+    }
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x < kDofHeaderWords) words[threadIdx.x] = __uint_as_float(p.head[threadIdx.x]);
+}
+// One CTA per tile: rho_t = 0 when the largest max |r| of the tiles within `reach` is below 1/2 (the tile is copied), ceil of it
+// otherwise; then each pixel's gather, from the shared-memory stage (STAGE) or from global memory
+template <bool STAGE>
+__global__ void __launch_bounds__(DOF_THREADS) k_dof_gather(const float4* __restrict__ output, int W, int H, const __grid_constant__ DofDev p,
+                                                            float* __restrict__ words, const float* __restrict__ tile_m, const DofTap* __restrict__ taps,
+                                                            float4* __restrict__ dof) {
+    __shared__ int s_rho;
+    const int tx = blockIdx.x, ty = blockIdx.y, TX = gridDim.x, TY = gridDim.y;
+    if (threadIdx.x < 32) {   // the (2 reach + 1)^2 <= 25 neighbouring tiles, one per lane
+        const int n = 2 * p.reach + 1, k = threadIdx.x;
+        const int ux = tx - p.reach + k % n, uy = ty - p.reach + k / n;
+        float m = (k < n * n && ux >= 0 && uy >= 0 && ux < TX && uy < TY) ? tile_m[uy * TX + ux] : 0.0f;
+        for (int o = 16; o > 0; o >>= 1) { const float b = __shfl_xor_sync(0xffffffffu, m, o); m = m > b ? m : b; }
+        if (k == 0) {
+            const int rho = m < 0.5f ? 0 : (int)ceilf(m);
+            s_rho = rho;
+            words[kDofHeaderWords + (size_t)W * H + ty * TX + tx] = __uint_as_float((u32)rho);
+        }
+    }
+    __syncthreads();
+    const int rho = s_rho;
+    const int lx = threadIdx.x % kDofTile, ly = threadIdx.x / kDofTile, x = tx * kDofTile + lx, y = ty * kDofTile + ly;
+    const float* r = words + kDofHeaderWords;
+    if (rho == 0) {   // nothing here is blurred: the frame is copied bit for bit
+        if (x < W && y < H) dof[(size_t)y * W + x] = output[(size_t)y * W + x];
+        return;
+    }
+    auto cx = [&](int v) { return v < 0 ? 0 : (v > W - 1 ? W - 1 : v); };
+    auto cy = [&](int v) { return v < 0 ? 0 : (v > H - 1 ? H - 1 : v); };
+    if (STAGE) {
+        extern __shared__ float4 s_c[];   // (16 + 2 rho)^2 colours (non-finite channels read 0), then as many radii
+        const int S = kDofTile + 2 * rho, x0 = tx * kDofTile - rho, y0 = ty * kDofTile - rho;
+        float* s_r = (float*)(s_c + S * S);
+        for (int k = threadIdx.x; k < S * S; k += DOF_THREADS) {
+            const int sy = k / S, sx = k - sy * S;
+            const size_t i = (size_t)cy(y0 + sy) * W + cx(x0 + sx);
+            const float4 c = output[i];
+            s_c[k] = f4(dof_finite(c.x), dof_finite(c.y), dof_finite(c.z), 0.0f);
+            s_r[k] = r[i];
+        }
+        __syncthreads();
+        if (x >= W || y >= H) return;
+        const int c0 = (ly + rho) * S + lx + rho;
+        dof[(size_t)y * W + x] = dof_gather_px(taps, rho, s_r[c0], [&](int dx, int dy, float4* c, float* rq) {
+            const int k = c0 + dy * S + dx; *c = s_c[k]; *rq = s_r[k];
+        });
+        return;
+    }
+    if (x >= W || y >= H) return;
+    dof[(size_t)y * W + x] = dof_gather_px(taps, rho, r[(size_t)y * W + x], [&](int dx, int dy, float4* c, float* rq) {
+        const size_t i = (size_t)cy(y + dy) * W + cx(x + dx);
+        const float4 v = ldg4(output + i);
+        *c = f4(dof_finite(v.x), dof_finite(v.y), dof_finite(v.z), 0.0f); *rq = __ldg(r + i);
+    });
+}
+
+// The thin-lens primary ray of pixel (x, y): a uniform point u of the unit disc, drawn by rejection from pairs of the lens stream (at
+// most 16 pairs, else the centre), the origin moved to o + (right (h u.x) + up (h u.y)), aimed at the pinhole ray's point at view
+// depth F, P_F = o + d (F / dot(d, fwd))
+ST_DEV Ray lens_ray(const GpuCamera& c, const LensDev& l, u32 x, u32 y) {
+    const Ray pin = cam_ray(c, x, y);
+    Rng rng = rng_make(l.seed, x, y);
+    float a = 0.0f, b = 0.0f;
+    for (int i = 0; i < 16; i++) {
+        const float u = rng_f(rng) * 2.0f - 1.0f, v = rng_f(rng) * 2.0f - 1.0f;
+        if (u * u + v * v <= 1.0f) { a = u; b = v; break; }
+    }
+    const float ha = l.h * a, hb = l.h * b;
+    const float3 o = pin.o + (f3(l.rx, l.ry, l.rz) * ha + f3(l.ux, l.uy, l.uz) * hb);
+    const float s = l.F / ((pin.d.x * l.fx + pin.d.y * l.fy) + pin.d.z * l.fz);
+    const float3 pf = pin.o + pin.d * s;
+    return ray_make(o, norm(pf - o));
+}
+// K1 ref_tracing::main (ref_tracing.rs:4-60); NMAP: the packed normal is the mapped one, which K2 shades with and nudges along; LENS:
+// the depth-0 ray is the thin-lens ray (ST_OPT_DEPTH_OF_FIELD)
+template <bool NMAP, bool LENS>
+__global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth, const __grid_constant__ LensDev lens) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
     size_t idx = screen_idx(cam, p.x, p.y);
     Ray ray;
-    if (depth == 0u) ray = cam_ray(cam.curr, p.x, p.y);
+    if (depth == 0u) ray = LENS ? lens_ray(cam.curr, lens, p.x, p.y) : cam_ray(cam.curr, p.x, p.y);
     else {
         float4 d0 = cam.ref_rays[3 * idx], d1 = cam.ref_rays[3 * idx + 1];
         if (all_zero(d1)) return;
@@ -1856,10 +1994,11 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_tracing(KPARAMS, u32 depth) {
 
 // K2 ref_shading::main (ref_shading.rs:4-177); LGRID: the one light is drawn from the light grid's list for the nudged hit point
 // TEXF: the hit's textures are filtered; the packed hit carries no triangle, so the segment's ray is traced again (same ray, same
-// BVH: the same triangle and distance); ENVM: a path that leaves the scene sees the map
-template <bool LGRID, bool TEXF, bool ENVM>
+// BVH: the same triangle and distance); ENVM: a path that leaves the scene sees the map; LENS: the depth-0 ray is K1's thin-lens ray
+template <bool LGRID, bool TEXF, bool ENVM, bool LENS>
 __global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32 depth, const __grid_constant__ LightGridDev lg,
-                                                          const __grid_constant__ TexFilterDev tf, const __grid_constant__ EnvMapDev em) {
+                                                          const __grid_constant__ TexFilterDev tf, const __grid_constant__ EnvMapDev em,
+                                                          const __grid_constant__ LensDev lens) {
     ST_TRACE_STACK();
     Px p = pixel_full(cam);
     if (!p.in) return;
@@ -1873,7 +2012,7 @@ __global__ void __launch_bounds__(ST_BLOCK) k_ref_shading(KPARAMS, u32 seed, u32
         return;
     }
     Ray ray; float3 color, thr;
-    if (depth == 0u) { ray = cam_ray(cam.curr, p.x, p.y); color = f3s(0.f); thr = f3s(1.0f); }
+    if (depth == 0u) { ray = LENS ? lens_ray(cam.curr, lens, p.x, p.y) : cam_ray(cam.curr, p.x, p.y); color = f3s(0.f); thr = f3s(1.0f); }
     else {
         float4 d0 = rays[3 * idx], d1 = rays[3 * idx + 1], d2 = rays[3 * idx + 2];
         if (all_zero(d1)) return;   // dead path: explicit no-op (the reference reaches the same state through 0 * x)
@@ -2586,18 +2725,50 @@ void launch_output_bloom(const CameraDev& c, const SceneDev& s, int op, const u3
     default: k_output_bloom<4><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, out, state, p, b, up0, w0, h0); break;
     }
 }
-void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st) {
-    if (nmap) k_ref_tracing<true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth); else k_ref_tracing<false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth);
+void launch_depth_of_field(const CameraDev& c, const DofDev& p, const DofBufs& b, cudaStream_t st) {
+    const dim3 grid(b.tx, b.ty);
+    k_dof_coc<<<grid, DOF_THREADS, 0, st>>>(c, p, b.words, b.tile_m);
+    const int rmax = (int)ceilf(p.R);
+    if (rmax > ST_DOF_STAGE_MAX_RADIUS) {
+        k_dof_gather<false><<<grid, DOF_THREADS, 0, st>>>(c.output, c.w, c.h, p, b.words, b.tile_m, b.taps, b.frame);
+        return;
+    }
+    const int S = kDofTile + 2 * rmax;   // the stage of the largest radius the frame can gather with
+    static bool attr_set[64] = {};
+    int dev = 0; cudaGetDevice(&dev); dev &= 63;
+    if (!attr_set[dev]) {   // the largest stage this build launches: (16 + 2 ST_DOF_STAGE_MAX_RADIUS)^2 texels of 20 bytes
+        const int most = (kDofTile + 2 * ST_DOF_STAGE_MAX_RADIUS) * (kDofTile + 2 * ST_DOF_STAGE_MAX_RADIUS) * 20;
+        if (cudaFuncSetAttribute(k_dof_gather<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, most) != cudaSuccess) {
+            // the device cannot hold the stage: the global-memory gather gives the same words
+            cudaGetLastError();
+            k_dof_gather<false><<<grid, DOF_THREADS, 0, st>>>(c.output, c.w, c.h, p, b.words, b.tile_m, b.taps, b.frame);
+            return;
+        }
+        attr_set[dev] = true;
+    }
+    k_dof_gather<true><<<grid, DOF_THREADS, S * S * 20, st>>>(c.output, c.w, c.h, p, b.words, b.tile_m, b.taps, b.frame);
+}
+void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, const LensDev* lens, cudaStream_t st) {
+    const LensDev lnone{};
+    const LensDev& l = lens ? *lens : lnone;
+#define ST_RT(N_, L_) k_ref_tracing<N_, L_><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, depth, l)
+    if (lens) { if (nmap) ST_RT(true, true); else ST_RT(false, true); }
+    else { if (nmap) ST_RT(true, false); else ST_RT(false, false); }
+#undef ST_RT
 }
 void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, const EnvMapDev* em,
-                        cudaStream_t st) {
+                        const LensDev* lens, cudaStream_t st) {
     const LightGridDev none{};
     const LightGridDev& g = lg ? *lg : none;
     const TexFilterDev tnone{};
     const TexFilterDev& t = tf ? *tf : tnone;
     const EnvMapDev enone{};
     const EnvMapDev& m = em ? *em : enone;
-#define ST_RS(L_, T_, E_) k_ref_shading<L_, T_, E_><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, g, t, m)
+    const LensDev lnone{};
+    const LensDev& l = lens ? *lens : lnone;
+    // LENS only at depth 0, where the primary ray is formed
+#define ST_RS(L_, T_, E_) do { if (lens && depth == 0u) k_ref_shading<L_, T_, E_, true><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, g, t, m, l); \
+                               else k_ref_shading<L_, T_, E_, false><<<grid_full(c), ST_BLOCK, 0, st>>>(c, s, seed, depth, g, t, m, l); } while (0)
     if (em) {
         if (tf) { if (lg) ST_RS(true, true, true); else ST_RS(false, true, true); }
         else { if (lg) ST_RS(true, false, true); else ST_RS(false, false, true); }

@@ -83,8 +83,41 @@ void launch_bloom_pyramid(const CameraDev& c, const BloomLevels& lv, const u32* 
 // launch_output_display
 void launch_output_bloom(const CameraDev& c, const SceneDev& s, int op, const u32* state, ExposureDev p, BloomDev b, const float4* up0, int w0, int h0,
                          uchar4* out, cudaStream_t st);
-void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, cudaStream_t st);
-void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, const EnvMapDev* em, cudaStream_t st);
+// ST_OPT_DEPTH_OF_FIELD (DESIGN.md §2 "Depth of field"; strict build only).  16 x 16 pixel tiles; the gather's tap table holds, per
+// radius rho = 1..kDofMaxRadius, kDofTaps integer offsets and their distances (dof_tap_table, engine.cu).  The per-camera buffer:
+// the defocused frame (W x H float4), then the "depth_of_field" words {W, H, TX, TY, defocused, f, A, k, F, R, forward.xyz, 0, 0, 0}
+// (kDofHeaderWords), the signed CoC radius r of every pixel and every tile's gather radius rho_t (u32), then every tile's max |r|
+// (float) and the tap table; each section starts on a 256-byte boundary.
+enum { kDofTile = 16, kDofMaxRadius = 32, kDofTaps = 81, kDofHeaderWords = 16 };
+struct DofTap { short dx, dy; float d; };
+struct DofDev {
+    u32 head[kDofHeaderWords];   // the header words of the frame, as above
+    int active;                  // 0: not defocused this frame (F <= f): every r is 0 and the frame is copied
+    float k, F, R, fwd_x, fwd_y, fwd_z;
+    int reach;                   // ceil(R / 16): the tiles a circle of radius R can reach
+};
+struct DofBufs { float4* frame; float* words; float* tile_m; const DofTap* taps; int tx, ty; size_t words_count; };
+inline size_t dof_layout(int W, int H, void* base, DofBufs* b) {
+    auto up = [](size_t n) { return (n + 255) / 256 * 256; };
+    const size_t px = (size_t)W * H;
+    b->tx = (W + kDofTile - 1) / kDofTile; b->ty = (H + kDofTile - 1) / kDofTile;
+    const size_t tiles = (size_t)b->tx * b->ty;
+    b->words_count = kDofHeaderWords + px + tiles;
+    const size_t o_words = up(16 * px), o_m = o_words + up(4 * b->words_count), o_taps = o_m + up(4 * tiles);
+    char* p = (char*)base;
+    b->frame = p ? (float4*)p : nullptr; b->words = p ? (float*)(p + o_words) : nullptr;
+    b->tile_m = p ? (float*)(p + o_m) : nullptr; b->taps = p ? (const DofTap*)(p + o_taps) : nullptr;
+    return o_taps + sizeof(DofTap) * kDofMaxRadius * kDofTaps;
+}
+// The CoC of every pixel of c.surface_nd through c.curr's rays, each tile's max |r|, then the gather of c.output into b.frame
+void launch_depth_of_field(const CameraDev& c, const DofDev& p, const DofBufs& b, cudaStream_t st);
+// ST_OPT_DEPTH_OF_FIELD in Reference mode (DESIGN.md §2 "Depth of field"): the thin lens of K1 / K2's primary rays.  `seed` is the
+// frame's lens dispatch seed; h = A / 2 the aperture radius; F the focal distance; right, up and fwd the camera's unit axes.
+struct LensDev { u32 seed; float h, F, rx, ry, rz, ux, uy, uz, fx, fy, fz; };
+// lens (non-null): the LENS instantiations, whose depth-0 ray is the thin-lens ray of `lens`
+void launch_ref_tracing(const CameraDev& c, const SceneDev& s, u32 depth, bool nmap, const LensDev* lens, cudaStream_t st);
+void launch_ref_shading(const CameraDev& c, const SceneDev& s, u32 seed, u32 depth, const LightGridDev* lg, const TexFilterDev* tf, const EnvMapDev* em,
+                        const LensDev* lens, cudaStream_t st);
 void launch_bvh_heatmap(const CameraDev& c, const SceneDev& s, cudaStream_t st);
 void launch_trace_stream_closest(const SceneDev& s, const float4* rays, long n, float4* out, cudaStream_t st);
 void launch_trace_stream_any(const SceneDev& s, const float4* rays, long n, u32* out, cudaStream_t st);

@@ -34,6 +34,7 @@ OPT_ENVIRONMENT_MAP_SAMPLING = 19   # 1: the GI bounce and sky draw aim at the e
 OPT_TONEMAPPING = 20         # Rgba8 display transform: 0 off (today's store), 1 exposure only, 2 Reinhard, 3 ACES fitted, 4 AgX
 OPT_AUTO_EXPOSURE = 21       # 1: each camera meters its frame and adapts its EV (0 = the manual ev of set_exposure); needs OPT_TONEMAPPING
 OPT_BLOOM = 22               # 1: a glow around bright light in the Rgba8 store, from a downsample / upsample pyramid (set_bloom)
+OPT_DEPTH_OF_FIELD = 23      # 1: frames defocused through a thin lens, a circle-of-confusion gather (set_depth_of_field)
 TONEMAP_OFF, TONEMAP_EXPOSURE, TONEMAP_REINHARD, TONEMAP_ACES, TONEMAP_AGX = 0, 1, 2, 3, 4
 WAVELET_TILED_DEFAULT = 15   # include/strolle_b200.h ST_WAVELET_TILED_DEFAULT
 STAT_WAVELET_TILED_LAUNCHES = 1
@@ -52,6 +53,7 @@ STAT_ENVIRONMENT_MAP_LAUNCHES = 13   # launches of the environment-mapped kernel
 STAT_ENVIRONMENT_MAP_DISTRIBUTION_BUILDS = 14   # environment-map distribution builds (OPT_ENVIRONMENT_MAP_SAMPLING) since creation
 STAT_EXPOSURE_METERINGS = 15   # metering launches (OPT_AUTO_EXPOSURE) since creation
 STAT_BLOOM_PYRAMIDS = 16       # pyramid builds (OPT_BLOOM) since creation
+STAT_DEPTH_OF_FIELD_GATHERS = 17   # depth-of-field gathers (OPT_DEPTH_OF_FIELD) since creation
 
 
 class StrolleError(RuntimeError):
@@ -137,6 +139,37 @@ def parse_bloom(words):
     return dict(levels=L, sizes=sizes, down=down, up=up)
 
 
+class _DepthOfField(C.Structure):
+    _fields_ = [(n, C.c_float) for n in ("focal_distance", "aperture_f_stops", "sensor_height", "max_radius")]
+
+
+DEPTH_OF_FIELD_DEFAULTS = dict(focal_distance=10.0, aperture_f_stops=1.0, sensor_height=0.01866, max_radius=16.0)
+DEPTH_OF_FIELD_HEADER_WORDS = 16
+
+
+def _depth_of_field(fields):
+    """st_depth_of_field from keyword fields over the defaults; None (no fields) stands for NULL."""
+    if fields is None:
+        return None
+    unknown = set(fields) - set(DEPTH_OF_FIELD_DEFAULTS)
+    if unknown:
+        raise TypeError(f"set_depth_of_field: unknown fields {sorted(unknown)}")
+    v = dict(DEPTH_OF_FIELD_DEFAULTS, **fields)
+    return C.byref(_DepthOfField(*[v[n] for n, _ in _DepthOfField._fields_]))
+
+
+def parse_depth_of_field(words):
+    """read_buffer(cam, "depth_of_field") as a dict: w, h, tiles (tx, ty), defocused, the lens constants f, A, k, F, R and forward
+    (float32), r (h x w float32, the signed CoC radius) and rho (ty x tx, every tile's gather radius)."""
+    w = np.asarray(words, np.float32).reshape(-1)
+    u = w.view(np.uint32)
+    W, H, TX, TY = (int(v) for v in u[:4])
+    f, A, k, F, R = (w[5 + i] for i in range(5))
+    n = DEPTH_OF_FIELD_HEADER_WORDS
+    return dict(w=W, h=H, tiles=(TX, TY), defocused=bool(u[4]), f=f, A=A, k=k, F=F, R=R, forward=w[10:13].copy(),
+                r=w[n:n + W * H].reshape(H, W), rho=u[n + W * H:n + W * H + TX * TY].reshape(TY, TX).astype(np.int64))
+
+
 def parse_exposure(words):
     """read_buffer(cam, "exposure") as a dict: ev, target (float32), counted, kept, frames and the 256 bins of the last frame."""
     w = np.asarray(words, np.float32).view(np.uint32)
@@ -170,6 +203,7 @@ def load_library():
         "st_insert_instance": [P, u64, u64, u64, f32p], "st_remove_instance": [P, u64],
         "st_insert_light": [P, u64, C.POINTER(_Light)], "st_remove_light": [P, u64], "st_update_sun": [P, C.c_float, C.c_float],
         "st_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_set_exposure": [P, C.c_void_p], "st_set_bloom": [P, C.c_void_p],
+        "st_set_depth_of_field": [P, C.c_void_p],
         "st_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_update_camera": [P, i32, C.POINTER(_Camera)], "st_delete_camera": [P, i32],
         "st_tick": [P], "st_render_camera": [P, i32, P, C.c_int], "st_copy_output": [P, i32, P, C.c_int], "st_synchronize": [P],
         "st_set_seed_base": [P, u32], "st_set_blue_noise": [P, C.c_void_p],
@@ -200,6 +234,7 @@ def load_library():
         "st_multi_insert_instance": [P, u64, u64, u64, f32p], "st_multi_remove_instance": [P, u64],
         "st_multi_insert_light": [P, u64, C.POINTER(_Light)], "st_multi_remove_light": [P, u64], "st_multi_update_sun": [P, C.c_float, C.c_float],
         "st_multi_set_environment_map": [P, C.c_void_p, u32, u32, C.c_float, C.c_float], "st_multi_set_exposure": [P, C.c_void_p], "st_multi_set_bloom": [P, C.c_void_p],
+        "st_multi_set_depth_of_field": [P, C.c_void_p],
         "st_multi_create_camera": [P, C.POINTER(_Camera), C.POINTER(i32)], "st_multi_update_camera": [P, i32, C.POINTER(_Camera)], "st_multi_delete_camera": [P, i32],
         "st_multi_tick": [P], "st_multi_render_camera": [P, i32, P, C.c_int], "st_multi_synchronize": [P],
         "st_multi_set_option": [P, C.c_int, C.c_int], "st_multi_set_seed_base": [P, u32], "st_multi_set_blue_noise": [P, C.c_void_p],
@@ -405,6 +440,12 @@ class Engine:
         defaults, BLOOM_DEFAULTS; no fields restores them all).  Refused as a whole when a field is out of range
         (include/strolle_b200.h st_set_bloom)."""
         self._check(self.lib.st_set_bloom(self._h, _bloom(fields or None)))
+
+    def set_depth_of_field(self, **fields):
+        """The thin lens of OPT_DEPTH_OF_FIELD, from the next tick: focal_distance, aperture_f_stops, sensor_height, max_radius (fields
+        not given take their defaults, DEPTH_OF_FIELD_DEFAULTS; no fields restores them all).  Refused as a whole when a field is out of
+        range (include/strolle_b200.h st_set_depth_of_field)."""
+        self._check(self.lib.st_set_depth_of_field(self._h, _depth_of_field(fields or None)))
 
     # ---- cameras ----------------------------------------------------------------------------
     @staticmethod
@@ -702,6 +743,9 @@ class MultiEngine:
 
     def set_bloom(self, **fields):
         self._check(self.lib.st_multi_set_bloom(self._h, _bloom(fields or None)))
+
+    def set_depth_of_field(self, **fields):
+        self._check(self.lib.st_multi_set_depth_of_field(self._h, _depth_of_field(fields or None)))
 
     def read_buffer(self, cam, name):
         """The whole frame's buffer, each strip read from the member that owns it."""

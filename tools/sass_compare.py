@@ -1,6 +1,6 @@
 """Compare per-kernel SASS of two libstrolle_b200.so builds: every kernel of the old build against the same kernel (for a kernel that
-gained `bool NMAP` / `bool LGRID` / `bool TEXF` / `bool ENVM` template parameters: its all-<false> instantiation, whose trailing
-LightGridDev, TexFilterDev and EnvMapDev arguments are unused) of the new one.  The GI sampling kernels' ENVM is an int (EnvMode):
+gained `bool NMAP` / `bool LGRID` / `bool TEXF` / `bool ENVM` / `bool LENS` template parameters: its all-<false> instantiation, whose
+trailing LightGridDev, TexFilterDev, EnvMapDev and LensDev arguments are unused) of the new one.  The GI sampling kernels' ENVM is an int (EnvMode):
 0 compares as false, 1 (the map) as true, 2 (the map sampled, ST_OPT_ENVIRONMENT_MAP_SAMPLING) is new.  Compared: the full instruction text (opcodes,
 registers, immediates, constant-bank operands); normalised: the code-offset comments, branch targets and relocated symbol names."""
 import re, subprocess, sys
@@ -35,6 +35,11 @@ def kernels(lib):
         k = base(d)
         if k is None: return d
         args = targs(d)
+        if "LensDev)" in d:   # bool LENS (K1, K2), the last template argument
+            if args[-1] == "true": return d
+            del args[-1]
+            head = d.split("(")[0]
+            d = head.split("<")[0] + "<" + ", ".join(args) + ">" + re.sub(r", \w+::LensDev const&\)|, \w+::LensDev\)", ")", d[len(head):])
         if "EnvMapDev)" in d and args[-1] in ("0", "1", "2"):   # int ENVM: ENV_NONE / ENV_MAP as the bool it replaced
             args[-1] = {"0": "false", "1": "true", "2": "2"}[args[-1]]
             head = d.split("(")[0]
