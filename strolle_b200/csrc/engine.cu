@@ -419,7 +419,10 @@ struct CameraSlot {
     struct PeerLink { bool ready = false; bool ipc = false; std::vector<char*> arena, rgba8; std::vector<uint32_t*> flags; DevMem sync; uint32_t seq = 0, fseq = 0; } peer;
 };
 
-struct Step { int pass; std::function<void(cudaStream_t)> run; int sub = -1; };   // sub: à-trous iteration of a K22 step
+// Which ReSTIR chain a step belongs to.  The two chains share no buffer they write (DESIGN.md §4 "Chain overlap"), so a single-GPU
+// frame may run the DI chain on a second stream beside the GI chain (render_overlapped).
+enum Chain { CHAIN_FRAME = 0, CHAIN_DI = 1, CHAIN_GI = 2 };
+struct Step { int pass; std::function<void(cudaStream_t)> run; int sub = -1; int chain = CHAIN_FRAME; };   // sub: à-trous iteration of a K22 step
 
 }  // namespace st
 
@@ -429,6 +432,10 @@ struct st_engine {
     int device = 0;
     cudaStream_t stream = nullptr; bool own_stream = true;
     cudaStream_t copy_stream = nullptr;   // device->host copies of finished frames (ST_OPT_ASYNC_OUTPUT), so that they overlap the next frame
+    // the DI chain's stream of an overlapped frame (render_overlapped), forked from `stream` after the G-buffer and joined back into it
+    // before the first pass that reads both chains.  serial_chains: every frame in launch order on `stream`; overlapped_frames: frames
+    // rendered with the fork since creation (both st_debug_serial_chains)
+    cudaStream_t di_stream = nullptr; cudaEvent_t di_fork = nullptr, di_join = nullptr; bool serial_chains = false; uint64_t overlapped_frames = 0;
     // meshes / materials / instances / triangles -------------------------------------------------
     std::unordered_map<st_handle, std::vector<st_mesh_triangle>> meshes;
     std::vector<st_material> materials; std::vector<st_handle> material_handles; bool materials_dirty = false;
@@ -1139,7 +1146,8 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     if (!e->envs_frame) emd.cdf = nullptr;   // ST_OPT_ENVIRONMENT_MAP_SAMPLING: K12 / K13 draw from the map's distribution
     const bool eson = emon && e->envs_frame;
     auto seed = [&](uint32_t k) { return dispatch_seed(e->seed_base, f, k); };
-    auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn)}); };
+    int chain = CHAIN_FRAME;
+    auto add = [&](int pass, std::function<void(cudaStream_t)> fn) { steps->push_back(Step{pass, std::move(fn), -1, chain}); };
     const CameraDev camO = frame_source(e, cs, cam);   // ST_OPT_DEPTH_OF_FIELD: the metering and the pyramid read the defocused frame
     auto defocus = [&]() {   // ST_OPT_DEPTH_OF_FIELD: the CoC and the gather of the frame's `output`, once per rendered frame
         if (!defocuses(e, cs)) return;
@@ -1192,6 +1200,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
     if (!e->instances.empty()) {
         if (!k4_in_k0) add(P_FRAME_REPROJECTION, [=](cudaStream_t s) { launch_frame_reprojection(cam, sc, cur, s); });
         if (needs_di) {
+            chain = CHAIN_DI;
             uint32_t s1 = seed(P_DI_SAMPLING), s2 = seed(P_DI_TEMPORAL), s3 = seed(P_DI_SPATIAL_PICK), s5 = seed(P_DI_SPATIAL_SAMPLE);
             if (fp) {
                 add(P_DI_TEMPORAL, [=](cudaStream_t s) { (fs ? stf::launch_di_sample_temporal : st::launch_di_sample_temporal)(cam, sc, cur, s1, s2, f, lgon ? &lgd : nullptr, s); });
@@ -1206,6 +1215,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
             add(P_DI_RESOLVING, [=](cudaStream_t s) { if (emon) e->envm_launches++; (fs ? stf::launch_di_resolving : st::launch_di_resolving)(cam, sc, cur, emon ? &emd : nullptr, s); });
         }
         if (needs_gi) {
+            chain = CHAIN_GI;
             uint32_t sa = seed(P_GI_SAMPLING_A), sb = seed(P_GI_SAMPLING_B), st_ = seed(P_GI_TEMPORAL), sp = seed(P_GI_SPATIAL_PICK), ss = seed(P_GI_SPATIAL_SAMPLE), sv = seed(P_GI_PREVIEW);
             uint32_t source;
             const bool tracing = f % 6u < 4u;
@@ -1252,6 +1262,7 @@ static void build_schedule(st_engine* e, CameraSlot* cs, std::vector<Step>* step
                 add(P_GI_RESOLVING, [=](cudaStream_t s) { (fs ? stf::launch_gi_resolving : st::launch_gi_resolving)(cam, sc, cur, src0, s); });
             }
         }
+        chain = CHAIN_FRAME;
     }
     if (d.denoise) {   // FrameDenoisingPass::run (passes/frame_denoising.rs:143-190)
         if (e->fuse_reproject) {   // ST_OPT_FUSE_REPROJECT: both signals in one launch (same arithmetic, shared surface/reprojection reads)
@@ -1662,6 +1673,9 @@ int st_engine_create(int device, st_engine** out) {
     int rc = e->d_noise.ensure(256 * 256 * 4); if (rc) { delete e; return rc; }
     rc = e->d_unpacklut.ensure(512 * 4); if (rc) { delete e; return rc; }
     rc = e->d_tile_errors.ensure(4); if (rc) { delete e; return rc; }
+    // non-blocking: the DI chain beside a caller's legacy default stream (st_set_stream(NULL)) must not serialise against it
+    CK(cudaStreamCreateWithFlags(&e->di_stream, cudaStreamNonBlocking));
+    CK(cudaEventCreateWithFlags(&e->di_fork, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&e->di_join, cudaEventDisableTiming));
     launch_unpack_lut((float*)e->d_unpacklut.p, e->stream);
     *out = e;
     return ST_OK;
@@ -1682,6 +1696,9 @@ void st_engine_destroy(st_engine* e) {
     if (e->comm) g_nccl.CommDestroy(e->comm);
     if (e->own_stream) cudaStreamDestroy(e->stream);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
+    if (e->di_stream) { cudaStreamSynchronize(e->di_stream); cudaStreamDestroy(e->di_stream); }
+    if (e->di_fork) cudaEventDestroy(e->di_fork);
+    if (e->di_join) cudaEventDestroy(e->di_join);
     delete e;
 }
 
@@ -2048,6 +2065,34 @@ static int ensure_taa_history(st_engine* e, CameraSlot* cs) {
     cs->taa_hist[0] = (float4*)cs->taa.p; cs->taa_hist[1] = (float4*)((char*)cs->taa.p + bytes);
     return ST_OK;
 }
+// Whether a whole frame of the camera runs its DI chain on e->di_stream beside the GI chain: only where both chains run (Image mode)
+// and nothing keys on launch order — not a strip of a partitioned frame (its halo plans are keyed on step order), not in timing mode
+// (per-pass events must stay attributable to one launch each)
+static bool overlaps_chains(const st_engine* e, const CameraSlot* cs) {
+    const CameraDev& d = cs->dev;
+    return !e->serial_chains && !e->timing && e->n_ranks == 1 && cs->desc.mode == ST_MODE_IMAGE && d.y0 == 0 && d.y1 == d.h && d.own_y0 == 0 &&
+           d.own_y1 == d.h && d.mirror_up == 0 && d.mirror_dn == 0 && d.need_rows == nullptr;
+}
+// The frame's steps with the DI chain forked onto e->di_stream once everything before it (the G-buffer, K4) is enqueued, and joined back
+// into e->stream before the first step after the chains (K20, or the composition when denoising is off).  Both chains read only what
+// precedes the fork and write disjoint buffers (DESIGN.md §4 "Chain overlap"), so every buffer ends up with the serial order's bits.
+static int render_overlapped(st_engine* e, const std::vector<Step>& steps) {
+    bool forked = false, joined = false;
+    auto join = [&]() -> int { CK(cudaEventRecord(e->di_join, e->di_stream)); CK(cudaStreamWaitEvent(e->stream, e->di_join, 0)); joined = true; return ST_OK; };
+    int rc = ST_OK;
+    for (const Step& st : steps) {
+        if (st.chain == CHAIN_DI) {
+            if (!forked) { CK(cudaEventRecord(e->di_fork, e->stream)); CK(cudaStreamWaitEvent(e->di_stream, e->di_fork, 0)); forked = true; }
+            st.run(e->di_stream); e->pass_launches[st.pass]++;
+            continue;
+        }
+        if (forked && !joined && st.chain == CHAIN_FRAME && (rc = join())) return rc;
+        e->run_timed(st.pass, st.run, st.sub);
+    }
+    if (forked && !joined && (rc = join())) return rc;
+    if (forked) e->overlapped_frames++;
+    return ST_OK;
+}
 int st_render_range(st_engine* e, st_camera_handle h, int first, int last) {
     CameraSlot* cs = e ? get_camera(e, h) : nullptr;
     if (!cs) return fail(ST_ERR_NOT_FOUND, "unknown camera");
@@ -2060,7 +2105,8 @@ int st_render_range(st_engine* e, st_camera_handle h, int first, int last) {
     if ((rc = ensure_dof_state(e, cs))) return rc;
     std::vector<Step> steps; build_schedule(e, cs, &steps);
     if (last < 0 || last >= (int)steps.size()) last = (int)steps.size() - 1;
-    for (int i = std::max(first, 0); i <= last; i++) e->run_timed(steps[i].pass, steps[i].run, steps[i].sub);
+    if (first <= 0 && last == (int)steps.size() - 1 && overlaps_chains(e, cs)) { if ((rc = render_overlapped(e, steps))) return rc; }
+    else for (int i = std::max(first, 0); i <= last; i++) e->run_timed(steps[i].pass, steps[i].run, steps[i].sub);
     CK(cudaGetLastError());
     return ST_OK;
 }
@@ -2821,6 +2867,16 @@ int st_mark_end(st_engine* e, float* ms) {
     return ST_OK;
 }
 int st_enable_timing(st_engine* e, int enabled) { if (!e) return fail(ST_ERR_INVALID, "null engine"); e->timing = enabled != 0; return ST_OK; }
+// Development aid, not part of the public C ABI (include/strolle_b200.h does not declare it): serial != 0 runs every frame's DI and GI
+// chains in launch order on the engine's stream, so that tests/test_chain_overlap.py and tools/chain_overlap_cost.py can set the
+// overlapped frame against the serial one in one process.  *overlapped_frames (if non-NULL): frames rendered with the DI chain on its
+// own stream since the engine was created.
+int st_debug_serial_chains(st_engine* e, int serial, uint64_t* overlapped_frames) {
+    if (!e) return fail(ST_ERR_INVALID, "null engine");
+    e->serial_chains = serial != 0;
+    if (overlapped_frames) *overlapped_frames = e->overlapped_frames;
+    return ST_OK;
+}
 int st_pass_times(st_engine* e, float* ms, uint32_t* launches, int reset) {
     if (!e) return fail(ST_ERR_INVALID, "null engine");
     CK(cudaSetDevice(e->device));
